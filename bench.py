@@ -48,6 +48,9 @@ def parse():
     ap.add_argument("--controlnet", action="store_true", help="config-4 style: ControlNet encoder per window-step")
     ap.add_argument("--cpu-frames", type=int, default=4, help="frames of the bounded cpu_baseline sample (GPU arm)")
     ap.add_argument("--ref-frames", type=int, default=16, help="frames of one reference-arm step (16 = the config-2 window)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (the denoised latents) as DIR/<name>.npy "
+                         "in float32, so that two builds can be compared output for output on identical seeded inputs")
     return ap.parse_args()
 
 
@@ -274,6 +277,10 @@ def main():
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms_total = float(ms.item())
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), res.float().cpu().numpy())   # [1, 4, T, 64, 64]: 1 MB
     # ---- timed region 2 (e2e): host buffers, H2D of the step's inputs and D2H of its result inside the region
     barrier()
     e2, e3 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -343,7 +350,7 @@ def main():
         except Exception as e:   # never fail the headline on the side measurement
             forward_ms[other] = f"error: {e}"
 
-    # ---- roofline of the dominant kernel (conv/linear tcgen05 GEMM): CUDA events around every launch of one more
+    # ---- roofline of the dominant kernel (conv/linear wgmma GEMM): CUDA events around every launch of one more
     # denoise step on the launching stream (separate pass so the event records do not perturb the timed regions)
     roof = None
     # every rank runs the pass (the loop contains a collective); only rank 0 reports it
@@ -364,18 +371,12 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak = peaks.get("bf16_tflops_sustained", 989.0)
         achieved = fl["gemm"] * n_fwd / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else None
-        # DRAM bytes per launch of this kernel from the committed ncu capture of one forward (same shapes as here)
-        traffic, traffic_src = None, None
-        try:
-            tr = json.load(open(os.path.join(ROOT, "profiles", "r01_gemm_dram_traffic.json")))
-            traffic, traffic_src = tr["dram_bytes_per_launch"], "profiles/r01_gemm_dram_traffic.json (ncu dram__bytes_read+write, mean over the 440 GEMM launches of a forward; algorithmic %.0f MB/launch)" % (tr["algorithmic_bytes_per_launch"] / 1e6)
-        except Exception:
-            pass
-        roof = {"kernel": "conv_gemm_kernel (tcgen05 implicit-GEMM conv / linear)", "bound": "tensor",
+        traffic, traffic_src = None, None     # DRAM traffic per launch: not measured
+        roof = {"kernel": "conv_gemm_kernel (wgmma implicit-GEMM conv / linear)", "bound": "tensor",
                 "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak if achieved else None,
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1.4 PFLOP/s sustained",
+                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "H100 SXM data sheet, dense FP16 989 TFLOP/s at 700 W",
                 "traffic": traffic, "traffic_unit": "bytes/launch", "traffic_source": traffic_src, "launches_per_step": gemm_n, "avg_launch_ms": gemm_ms / max(gemm_n, 1),
                 "algorithmic_tflop_per_forward": fl["gemm"] / 1e12,
                 "step_share": {k: round(v["ms"], 2) for k, v in prof.items()}}
@@ -396,7 +397,7 @@ def main():
         fl_total = unet_forward_flops(cfg, 2, WINDOW + 1, LAT_H, LAT_W)["total"]
         extra = {"parallelism": (f"windows sharded over {world} GPU(s), 1 NCCL all-reduce/step" if not args.cfg_split else
                                  f"CFG split: {n_windows} window(s) over {world} GPUs, each GPU of a pair runs one half of the CFG batch, 1 NCCL all-reduce/step"),
-                 "l2_policy": "per-forward activation working set (~4 GB) >> 126 MB L2; no explicit flush",
+                 "l2_policy": "per-forward activation working set (~4 GB) >> 50 MB L2; no explicit flush",
                  "achieved_tflops_whole_step": fl_total * DDIM_STEPS * args.steps * n_windows / (ms_total * 1e-3) / 1e12,
                  # what bounds the weak-scaling curve: each added window brings 12 new frames for 17 computed ones
                  "ideal_efficiency": T / (WINDOW * world),

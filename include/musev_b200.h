@@ -1,4 +1,4 @@
-/* musev_b200 C ABI -- B200 (sm_100a) kernels for MuseV's denoising hot path.
+/* musev_b200 C ABI -- H100 (sm_90a) kernels for MuseV's denoising hot path.
  *
  * Conventions (mirrors how the reference drives its model, SURVEY.md section 8b):
  *   - every data pointer is a DEVICE pointer into caller-owned memory (e.g. torch `tensor.data_ptr()`);
@@ -26,7 +26,7 @@ const char* mvb_last_error(void);
 int mvb_version(void);
 
 /* ---------------------------------------------------------------------------------------------------------
- * Op level: implicit-GEMM convolution / linear on tcgen05 tensor cores.
+ * Op level: implicit-GEMM convolution / linear on wgmma tensor cores.
  *
  * Replaces, for channels-last fp16 activations:
  *   F.conv2d 3x3 pad 1      diffusers/src/diffusers/models/resnet.py:643,666 (ResnetBlock2D.conv1/conv2),
@@ -63,7 +63,7 @@ int mvb_op_conv_gemm(const mvb_conv_gemm_desc* desc, void* stream);
 
 
 /* ---------------------------------------------------------------------------------------------------------
- * Op level: flash attention on tcgen05 (spatial self / reference / cross attention of the transformer blocks).
+ * Op level: flash attention on wgmma (spatial self / reference / cross attention of the transformer blocks).
  *
  * Replaces xformers.ops.memory_efficient_attention at musev/models/attention_processor.py:258,292,519,724 and
  * F.scaled_dot_product_attention at diffusers/src/diffusers/models/attention_processor.py:1166-1250.
@@ -83,7 +83,7 @@ typedef struct mvb_attention_desc {
   float out_scale;
   int accumulate;
   int v_ones_col;  /* every V row holds 1.0 at column h*dp + d (dp > d): the P.V MMA also yields the softmax row sum */
-  int variant;     /* 0: default kernel; 2: split-KV kernel (dp <= 64 only; two independent softmax groups, kept for A/B runs) */
+  int variant;     /* accepted for ABI compatibility; every value runs the same kernel */
 } mvb_attention_desc;
 
 int mvb_op_attention(const mvb_attention_desc* desc, void* stream);

@@ -1,4 +1,4 @@
-"""musev_b200 -- B200 (sm_100a) denoising engine behind MuseV's UNet3DConditionModel / DDIMScheduler / pipeline API.
+"""musev_b200 -- H100 (sm_90a) denoising engine behind MuseV's UNet3DConditionModel / DDIMScheduler / pipeline API.
 
 The compute path is the in-tree CUDA library (musev_b200/_lib/libmusevb200.so, built by musev_b200.build);
 importing this package does not load it, using any op does -- and fails loudly if it is missing.

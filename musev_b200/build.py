@@ -1,4 +1,4 @@
-"""Builds the in-tree CUDA library (sm_100a only) with a plain nvcc command line.
+"""Builds the in-tree CUDA library (sm_90a only) with a plain nvcc command line.
 
 The .so is written next to the package (musev_b200/_lib/libmusevb200.so) so that it travels with the
 repo snapshot to the GPU box; it is git-ignored.
@@ -19,7 +19,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libmusevb200.so")
 INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

@@ -62,11 +62,11 @@ class ControlNetOutput(SimpleNamespace):
 
 
 class ControlNetModel:
-    """B200 engine behind the call surface of diffusers `ControlNetModel` (models/controlnet.py:114)."""
+    """CUDA engine behind the call surface of diffusers `ControlNetModel` (models/controlnet.py:114)."""
 
     def __init__(self, config: ControlNetConfig, device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16):
         if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_100a) device; there is no CPU path")
+            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.cfg = config
         self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
         self.dtype = dtype

@@ -1,23 +1,14 @@
-// tcgen05 flash attention (see attention.cuh). Four kernels, selected in launch_attention():
+// wgmma flash attention (see attention.cuh). One kernel, templated on the padded head dim dp (the N of the P.V MMA).
 //
-//   attention_pp_kernel   head dims that fit one 64-column atom (dp <= 64: level 0 of the UNet, 75 % of the attention time).
-//                         One CTA per SM = 256 queries = two 128-query tiles ping-ponged on one MMA-issuing warp, one thread per
-//                         query row, P kept in TMEM (TS-form P.V). Description, measurements and the phase trace: the comment
-//                         above the kernel and DESIGN.md 4.2. attention_pp2_kernel (variant 4) = the same with two threads per row.
-//   attention_kernel      head dims 80 / 160 (and variant 1 for A/B runs). One CTA = 320 threads = 128 queries of one (frame, head):
-//     warp 0      : TMA producer (Q once; K ring one tile ahead; V ring) -- boxes of 128 rows x 64 fp16, 128-byte swizzle;
-//                   warp-uniform loop, elect.sync picks the issuing lane
-//     warp 1      : TMEM allocator + MMA issuer (warp-uniform loop, one elected lane issues)
-//                     S = Q K^T   (M=128 queries, N=128 keys, K=dp)      -> TMEM columns [0,128); S_{j+1} is issued as
-//                                 soon as the softmax warps hold S_j in registers, i.e. it runs under softmax j
-//                     O += P V    (M=128, N=dp, K=128 keys; V consumed MN-major straight from its row-major tile)
-//     warps 2..9  : softmax, two threads per query row (64 key columns each): tcgen05.ld S into registers, online max
-//                   (the two halves of a row pair exchange it through smem behind a 64-thread named barrier) with lazy
-//                   rescaling of the TMEM accumulator (only when the running max grows by > 2^8), exp2 on packed f32x2
-//                   arguments with a fixed share on the FMA pipe (degree-3 polynomial) and the rest on the SFU,
-//                   P -> fp16 -> swizzled smem as MMA A operand; row sums come from the MMA (ones column in V)
-//   attention_split_kernel  split-KV variant of attention_kernel (two independent 4-warp softmax groups on alternating 64-key
-//                         tiles); correct but slower, only on request (AttnArgs.variant = 2).
+// CTA = 384 threads = 3 warpgroups = 128 queries of one (frame, head):
+//   warpgroup 0, warp 0 : TMA producer -- Q once, then K and V tiles of 128 keys through their own smem rings (boxes of
+//                         128 rows x 64 fp16, 128-byte swizzle); warp-uniform loop, elect.sync picks the issuing lane.
+//                         The warpgroup gives its registers to the other two (setmaxnreg).
+//   warpgroups 1, 2     : 64 query rows each. Per key tile: S = Q K^T (wgmma m64n128k16, both operands in smem) into
+//                         registers; masked online softmax (row max / sum over the four lanes that share a row); P is
+//                         rounded to fp16 in registers and fed straight back as the A operand of O += P V (wgmma
+//                         m64n{dp}k16, V read MN-major from its row-major tile); O stays in registers until the end.
+// The two consumer warpgroups run independently, so one's softmax overlaps the other's MMAs.
 #include "attention.cuh"
 
 #include <cuda.h>
@@ -39,42 +30,20 @@ struct AttnParams {
   int nk[2], fdiv[2];
   long long fmul[2], fadd[2];
   int sk, sv;  // K / V ring depth
-  int tmem_cols;
   __half* out;
   long long ldo;
   int accumulate;
-  int sum_in_v;   // V has a column of ones at index d (d % 8 == 0, d < dp): the PV MMA accumulates the softmax row sum
-  int pp_order;       // ping-pong kernel, MMA issue order: 0 = S0 S1 PV0 PV1 (default), 1 = S0 PV0 S1 PV1 (A/B runs)
-  int pp_alternate;   // ping-pong kernel: alternate the exponential phases of the two softmax warpgroups (named-barrier token)
-  long long* trace;   // ping-pong kernel, measurement aid (mvb_debug_attention_trace): CTA (0,0,0) writes clock64 stamps of its
-                      // phases here, [role 0..9][KV tile j < 32][8 slots]; null in normal runs
+  long long* trace;   // measurement aid (mvb_debug_attention_trace): CTA (0,0,0) writes clock64 stamps of its phases
+                      // here, [role 0..2][KV tile j < 32][8 slots]; null in normal runs
 };
 
-// clock64 stamp of one phase of the ping-pong kernel (only the traced CTA's three reporting lanes get a non-null pointer)
-__device__ __forceinline__ void pp_stamp(long long* tr, int j, int slot) {
+// clock64 stamp of one phase (only the traced CTA's reporting threads get a non-null pointer)
+__device__ __forceinline__ void att_stamp(long long* tr, int j, int slot) {
   if (tr != nullptr && j < 32) tr[j * 8 + slot] = clock64();
 }
 
 static constexpr int kAtomBytes = 128 * 128;  // 128 rows x 64 fp16
-
-// 2^x for a pair of arguments on the FMA / ALU pipes (no SFU): round-to-nearest split x = n + f, |f| <= 0.5, degree-3
-// minimax polynomial for 2^f (relative error < 7.5e-5, well below the 4.9e-4 fp16 rounding of P), exponent patched in
-// with one integer multiply-add. Used for a fixed share of the softmax columns so that the SFU (16 ex2/clk/SM), which
-// bounds this kernel at head dim 40, and the FMA pipe work in parallel.
-__device__ __forceinline__ void poly_exp2_pair(float a0, float a1, float& p0, float& p1) {
-  const F2 a = f2_make(fmaxf(a0, -125.f), fmaxf(a1, -125.f));
-  const F2 t = f2_add(a, f2_make(12582912.f, 12582912.f));
-  const F2 nf = f2_add(t, f2_make(-12582912.f, -12582912.f));
-  const F2 f = f2_fma(nf, f2_make(-1.f, -1.f), a);
-  F2 q = f2_fma(f, f2_make(0.0551716648f, 0.0551716648f), f2_make(0.242611125f, 0.242611125f));
-  q = f2_fma(q, f, f2_make(0.693260968f, 0.693260968f));
-  q = f2_fma(q, f, f2_make(0.999928057f, 0.999928057f));
-  float q0, q1, t0, t1;
-  f2_get(q, q0, q1);
-  f2_get(t, t0, t1);
-  p0 = __int_as_float(__float_as_int(q0) + (__float_as_int(t0) << 23));
-  p1 = __int_as_float(__float_as_int(q1) + (__float_as_int(t1) << 23));
-}
+static constexpr int kMaxRing = 4;
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -91,1243 +60,219 @@ __device__ __forceinline__ void tile_info(const AttnParams& p, int j, int* seg, 
   }
 }
 
-// kPolyOf8: of every 8 column pairs, this many take the FMA-pipe exp2 (the rest go to the SFU)
-template <bool kSumInV, int kPolyOf8>
-__global__ void __launch_bounds__(320, 2)
+__device__ __forceinline__ uint32_t pack_half2(float a, float b, float& back_sum) {
+  const __half2 h = __floats2half2_rn(a, b);
+  const float2 f = __half22float2(h);
+  back_sum += f.x + f.y;     // the row sum is taken over the fp16 probabilities the MMA actually sees
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+template <int DP>
+__global__ void __launch_bounds__(384, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
                  const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
                  const __grid_constant__ CUtensorMap tmV1, const __grid_constant__ AttnParams p) {
+  constexpr int kAtoms = (DP + 63) / 64;
+  constexpr int kTileBytes = kAtoms * kAtomBytes;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int tile_bytes = p.natoms * kAtomBytes;
   uint8_t* sQ = smem;
-  uint8_t* sK = sQ + tile_bytes;
-  uint8_t* sV = sK + p.sk * tile_bytes;
-  uint8_t* sP = sV + p.sv * tile_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * kAtomBytes);
-  uint64_t* bar_q = bars;          // 1
-  uint64_t* full_k = bars + 1;     // [2]
-  uint64_t* empty_k = bars + 3;    // [2]
-  uint64_t* full_v = bars + 5;     // [2]
-  uint64_t* empty_v = bars + 7;    // [2]
-  uint64_t* bar_s = bars + 9;
-  uint64_t* bar_p = bars + 10;
-  uint64_t* bar_o = bars + 11;
-  uint64_t* bar_sfree = bars + 12;  // softmax has pulled S_j into registers: S_{j+1} may overwrite the TMEM tile
-  uint64_t* bar_pv = bars + 13;     // P.V of tile j complete: P smem buffer reusable, O stable
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14);
-  float* smax = reinterpret_cast<float*>(bars + 16);   // [2 buffers][2 column halves][128 rows] row-max exchange
+  uint8_t* sK = sQ + kTileBytes;
+  uint8_t* sV = sK + p.sk * kTileBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + p.sv * kTileBytes);
+  uint64_t* bar_q = bars;                      // 1
+  uint64_t* full_k = bars + 1;                 // [kMaxRing]
+  uint64_t* empty_k = full_k + kMaxRing;
+  uint64_t* full_v = empty_k + kMaxRing;
+  uint64_t* empty_v = full_v + kMaxRing;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128;
   const int h = blockIdx.y;
   const int f = blockIdx.z;
   const int ntiles = (p.nk[0] + 127) / 128 + (p.nseg > 1 ? (p.nk[1] + 127) / 128 : 0);
+  const bool traced = p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
     mbar_init(bar_q, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&full_k[s], 1); mbar_init(&empty_k[s], 1);
-      mbar_init(&full_v[s], 1); mbar_init(&empty_v[s], 1);
+    for (int s = 0; s < kMaxRing; ++s) {
+      mbar_init(&full_k[s], 1); mbar_init(&empty_k[s], 8);   // one arrival per consumer warp
+      mbar_init(&full_v[s], 1); mbar_init(&empty_v[s], 8);
     }
-    mbar_init(bar_s, 1);
-    mbar_init(bar_p, 256);
-    mbar_init(bar_o, 1);
-    mbar_init(bar_sfree, 256);
-    mbar_init(bar_pv, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base;
-  const uint32_t tmem_O = tmem_base + 128;
 
-  if (warp == 0) {
-    // producer: warp-uniform control flow, one elected lane issues the copies
-    {
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0) {
+      long long* tr = (traced && lane == 0) ? p.trace : nullptr;
       if (elect_one()) {
-        mbar_expect_tx(bar_q, (uint32_t)tile_bytes);
-        for (int a = 0; a < p.natoms; ++a)
+        mbar_expect_tx(bar_q, (uint32_t)kTileBytes);
+        for (int a = 0; a < kAtoms; ++a)
           tma_load_2d(sQ + a * kAtomBytes, &tmQ, bar_q, h * p.dp + a * 64, f * p.Nq + q0);
       }
       __syncwarp();
-      auto load_k = [&](int j) {
+      for (int j = 0; j < ntiles; ++j) {
         int seg, k0, valid;
         tile_info(p, j, &seg, &k0, &valid);
-        const long long row = (long long)(f / p.fdiv[seg]) * p.fmul[seg] + p.fadd[seg] + k0;
+        const int row = (int)((long long)(f / p.fdiv[seg]) * p.fmul[seg] + p.fadd[seg] + k0);
         const CUtensorMap* mk = seg ? &tmK1 : &tmK0;
-        const int ks = j % p.sk;
+        const CUtensorMap* mv = seg ? &tmV1 : &tmV0;
+        const int ks = j % p.sk, vs = j % p.sv;
         mbar_wait(&empty_k[ks], ((j / p.sk) & 1) ^ 1);
         if (elect_one()) {
-          mbar_expect_tx(&full_k[ks], (uint32_t)tile_bytes);
-          for (int a = 0; a < p.natoms; ++a)
-            tma_load_2d(sK + ks * tile_bytes + a * kAtomBytes, mk, &full_k[ks], h * p.dp + a * 64, (int)row);
+          mbar_expect_tx(&full_k[ks], (uint32_t)kTileBytes);
+          for (int a = 0; a < kAtoms; ++a)
+            tma_load_2d(sK + ks * kTileBytes + a * kAtomBytes, mk, &full_k[ks], h * p.dp + a * 64, row);
         }
         __syncwarp();
-      };
-      load_k(0);
-      for (int j = 0; j < ntiles; ++j) {
-        if (j + 1 < ntiles) load_k(j + 1);     // K runs one tile ahead: S_{j+1} is computed under softmax j
-        int seg, k0, valid;
-        tile_info(p, j, &seg, &k0, &valid);
-        const long long row = (long long)(f / p.fdiv[seg]) * p.fmul[seg] + p.fadd[seg] + k0;
-        const CUtensorMap* mv = seg ? &tmV1 : &tmV0;
-        const int vs = j % p.sv;
+        att_stamp(tr, j, 0);
         mbar_wait(&empty_v[vs], ((j / p.sv) & 1) ^ 1);
         if (elect_one()) {
-          mbar_expect_tx(&full_v[vs], (uint32_t)tile_bytes);
-          for (int a = 0; a < p.natoms; ++a)
-            tma_load_2d(sV + vs * tile_bytes + a * kAtomBytes, mv, &full_v[vs], h * p.dp + a * 64, (int)row);
+          mbar_expect_tx(&full_v[vs], (uint32_t)kTileBytes);
+          for (int a = 0; a < kAtoms; ++a)
+            tma_load_2d(sV + vs * kTileBytes + a * kAtomBytes, mv, &full_v[vs], h * p.dp + a * 64, row);
         }
         __syncwarp();
+        att_stamp(tr, j, 1);
       }
     }
-  } else if (warp == 1) {
-    // MMA issue: warp-uniform loop, elected lane issues
-    {
-      const uint32_t idesc_s = make_idesc_f16(128, 128, 0, 0);
-      const uint32_t idesc_o = make_idesc_f16(128, p.dp, 0, 1);   // B (= V) is MN-major
-      const int ksteps = p.dp / 16;
-      mbar_wait(bar_q, 0);
-      const uint32_t aQ = smem_u32(sQ);
-      auto issue_s = [&](int j) {
-        const int ks = j % p.sk;
-        mbar_wait(&full_k[ks], (j / p.sk) & 1);
-        tc_fence_after();
-        const uint32_t aK = smem_u32(sK + ks * tile_bytes);
-        if (elect_one()) {
-          for (int kk = 0; kk < ksteps; ++kk) {
-            const uint32_t off = (uint32_t)(kk >> 2) * kAtomBytes + (uint32_t)(kk & 3) * 32;
-            umma_f16_ss(tmem_S, make_desc_k_sw128(aQ + off), make_desc_k_sw128(aK + off), idesc_s, kk != 0);
-          }
-          umma_commit(&empty_k[ks]);   // K stage free once S_j is done
-          umma_commit(bar_s);
-        }
-        __syncwarp();
-      };
-      issue_s(0);
-      for (int j = 0; j < ntiles; ++j) {
-        // S_{j+1} is issued as soon as the softmax warps hold S_j in registers, i.e. it runs under softmax j
-        if (j + 1 < ntiles) {
-          mbar_wait(bar_sfree, j & 1);
-          issue_s(j + 1);
-        }
-        const int vs = j % p.sv;
-        mbar_wait(&full_v[vs], (j / p.sv) & 1);
-        mbar_wait(bar_p, j & 1);     // P_j in smem, O rescaled
-        tc_fence_after();
-        const uint32_t aP = smem_u32(sP);
-        const uint32_t aV = smem_u32(sV + vs * tile_bytes);
-        if (elect_one()) {
-#pragma unroll
-          for (int k16 = 0; k16 < 8; ++k16) {
-            const uint32_t offp = (uint32_t)(k16 >> 2) * kAtomBytes + (uint32_t)(k16 & 3) * 32;
-            umma_f16_ss(tmem_O, make_desc_k_sw128(aP + offp), make_desc_mn_sw128(aV + (uint32_t)k16 * 2048, kAtomBytes),
-                        idesc_o, (j | k16) != 0);
-          }
-          umma_commit(&empty_v[vs]);
-          umma_commit(bar_pv);
-          if (j == ntiles - 1) umma_commit(bar_o);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // 8 softmax warps: two threads per query row, each owning 64 of the 128 key columns of the tile. Warps w and w+4
-    // hold the two halves of the same 32 rows and are the only ones that have to agree on the row max, so each such
-    // pair has its own 64-thread named barrier: the four pairs drift apart and cover each other's stalls.
-    const int qd = warp & 3;
-    const int ch = (warp - 2) >> 2;                 // column half: keys [64 ch, 64 ch + 64) = P atom `ch`
-    const int row = qd * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-    const uint32_t a_prow = smem_u32(sP) + (uint32_t)ch * kAtomBytes + (uint32_t)row * 128;
-    const uint32_t rx = (uint32_t)(row & 7) << 4;
-    const uint32_t a_mine = smem_u32(smax) + (uint32_t)(ch * 128 + row) * 4;
-    const uint32_t a_peer = smem_u32(smax) + (uint32_t)((ch ^ 1) * 128 + row) * 4;
-    const uint32_t a_bar_s = smem_u32(bar_s), a_bar_sfree = smem_u32(bar_sfree), a_bar_pv = smem_u32(bar_pv),
-                   a_bar_p = smem_u32(bar_p);
-    const int t0 = (p.nk[0] + 127) / 128;
-    float m = -INFINITY, l = 0.f;
-    const float sl2 = p.scale_log2;
-    for (int j = 0; j < ntiles; ++j) {
-      const int valid = j < t0 ? min(128, p.nk[0] - j * 128) : min(128, p.nk[1] - (j - t0) * 128);
-      mbar_wait_a(a_bar_s, j & 1);
-      tc_fence_after();
-      uint32_t v[64];
-      tmem_ld32(tmem_S + lane_off + ch * 64, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-      tmem_ld32(tmem_S + lane_off + ch * 64 + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive_a(a_bar_sfree);        // the tensor core may start S_{j+1} now
-      if (valid < 128) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i)
-          if (ch * 64 + i >= valid) v[i] = 0xff800000u;   // -inf
-      }
-      float mxs[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) mxs[i] = __uint_as_float(v[i]);
-#pragma unroll
-      for (int i = 8; i < 64; i += 8) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) mxs[e] = fmaxf(mxs[e], __uint_as_float(v[i + e]));
-      }
-      float mx = fmaxf(fmaxf(fmaxf(mxs[0], mxs[1]), fmaxf(mxs[2], mxs[3])),
-                       fmaxf(fmaxf(mxs[4], mxs[5]), fmaxf(mxs[6], mxs[7])));
-      // combine with the partner thread (other column half of the same row) through smem
-      const uint32_t xoff = (uint32_t)(j & 1) * 1024;
-      sts32f(a_mine + xoff, mx);
-      named_bar_sync(1 + qd, 64);
-      mx = fmaxf(mx, lds32f(a_peer + xoff)) * sl2;
-      const bool need = mx > m + 8.f;
-      float alpha = 1.f;
-      if (need) { alpha = fast_exp2(m - mx); m = mx; }
-      if (j > 0) {
-        mbar_wait_a(a_bar_pv, (j - 1) & 1);  // P buffer free again and O_{j-1} final before it is rescaled
-        tc_fence_after();
-      }
-      if (j > 0 && __any_sync(0xffffffffu, need)) {
-        // the two threads of a row split the O columns by 16-column chunk parity
-        for (int c0 = ch * 16; c0 < p.dp; c0 += 32) {
-          uint32_t o[16];
-          tmem_ld16(tmem_O + lane_off + c0, o);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st16(tmem_O + lane_off + c0, o);
-        }
-        tmem_st_wait();
-      }
-      const F2 sl2x2 = f2_make(sl2, sl2), nmx2 = f2_make(-m, -m);
-      float ls0 = 0.f, ls1 = 0.f;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {   // 8 chunks of 8 keys = one 16-byte smem store each
-        uint32_t ph[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int i = c * 4 + e;    // column pair; kPolyOf8 of every 8 pairs, evenly spread, take the FMA-pipe exp2
-          float a0, a1;
-          f2_get(f2_fma(f2_make(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])), sl2x2, nmx2), a0, a1);
-          float p0, p1;
-          if (((i * kPolyOf8) & 7) < kPolyOf8) {
-            poly_exp2_pair(a0, a1, p0, p1);
-          } else {
-            p0 = fast_exp2(a0);
-            p1 = fast_exp2(a1);
-          }
-          const __half2 hp = __floats2half2_rn(p0, p1);
-          ph[e] = *reinterpret_cast<const uint32_t*>(&hp);
-          if (!kSumInV) {
-            const float2 back = __half22float2(hp);
-            ls0 += back.x; ls1 += back.y;
-          }
-        }
-        sts128(a_prow + (((uint32_t)c << 4) ^ rx), ph[0], ph[1], ph[2], ph[3]);
-      }
-      if (!kSumInV) l = l * alpha + (ls0 + ls1);
-      fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive_a(a_bar_p);
-    }
-    // epilogue
-    mbar_wait(bar_o, 0);
-    tc_fence_after();
-    if (kSumInV) {
-      // the row sum was accumulated by the tensor core: V carries a column of ones at index d
-      uint32_t o[16];
-      tmem_ld16(tmem_O + lane_off + (p.d / 16) * 16, o);
-      tmem_ld_wait();
-      l = __uint_as_float(o[p.d % 16 == 8 ? 8 : 0]);
-    } else {
-      const uint32_t xoff = (uint32_t)(ntiles & 1) * 1024;
-      sts32f(a_mine + xoff, l);
-      named_bar_sync(1 + qd, 64);
-      l += lds32f(a_peer + xoff);
-    }
-    const float inv = p.out_scale / l;
-    const int qrow = q0 + row;
-    const bool ok = qrow < p.Nq;
-    __half* orow = p.out + ((long long)f * p.Nq + qrow) * p.ldo + h * p.d;
-    for (int c0 = ch * 16; c0 < p.dp; c0 += 32) {
-      uint32_t o[16];
-      tmem_ld16(tmem_O + lane_off + c0, o);
-      tmem_ld_wait();
-      if (ok) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          const int cc = c0 + g * 8;
-          if (cc < p.d) {
-            __align__(16) __half oh[8];
-            if (p.accumulate) *reinterpret_cast<uint4*>(oh) = *reinterpret_cast<const uint4*>(orow + cc);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              float x = __uint_as_float(o[g * 8 + e]) * inv;
-              if (p.accumulate) x += __half2float(oh[e]);
-              oh[e] = __float2half_rn(x);
-            }
-            *reinterpret_cast<uint4*>(orow + cc) = *reinterpret_cast<const uint4*>(oh);
-          }
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-}
 
-// ------------------------------------------------------------------------------------------------ split-KV variant
-// Same math, different decomposition, for head dims that fit one 64-column atom (dp <= 64: level 0, where attention
-// time is). The 128-query tile is served by TWO independent softmax groups of 4 warps; group g owns the 64-key tiles
-// j = g, g+2, g+4, ... with its own S tile, P buffer, running max and O accumulator in TMEM, and the two partial
-// results are merged once at the end (O = (O_A 2^(mA-M) + O_B 2^(mB-M)) / (lA' + lB')), as in split-KV decoding. One
-// thread owns a whole row of its tile, so the main loop has no cross-thread exchange and no intra-CTA barrier; with
-// two CTAs per SM there are four independent softmax pipelines per SM whose phases (TMEM load / max / exp / P store)
-// interleave instead of running in lock step.
-//   TMEM (256 columns): S_A 0..63 | S_B 64..127 | O_A 128..191 | O_B 192..255.
-//   smem: Q 16 KB | K ring 3 x 8 KB | V ring 3 x 8 KB | P_A, P_B 16 KB each | barriers | (m, l) exchange.
-static constexpr int kSplitStages = 3;
-static constexpr int kKvTileBytes = 64 * 128;   // 64 keys x 64 fp16
-
-template <bool kSumInV>
-__global__ void __launch_bounds__(320, 2)
-attention_split_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
-                       const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
-                       const __grid_constant__ CUtensorMap tmV1, const __grid_constant__ AttnParams p) {
-  constexpr int kPolyOf8 = 2;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sK = sQ + kAtomBytes;
-  uint8_t* sV = sK + kSplitStages * kKvTileBytes;
-  uint8_t* sP = sV + kSplitStages * kKvTileBytes;          // [2 groups][128 rows][64 keys]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * kAtomBytes);
-  uint64_t* bar_q = bars;
-  uint64_t* full_k = bars + 1;                   // [3]
-  uint64_t* empty_k = bars + 4;                  // [3]
-  uint64_t* full_v = bars + 7;                   // [3]
-  uint64_t* empty_v = bars + 10;                 // [3]
-  uint64_t* bar_s = bars + 13;                   // [2] S_g ready
-  uint64_t* bar_sfree = bars + 15;               // [2] group g holds S in registers (128 arrivals)
-  uint64_t* bar_p = bars + 17;                   // [2] P_g written, O_g rescaled (128 arrivals)
-  uint64_t* bar_pv = bars + 19;                  // [2] P_g V done: P_g reusable, O_g stable
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 21);
-  float* xch = reinterpret_cast<float*>(bars + 22);        // [2 groups][128 rows] (m, l)
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 128;
-  const int h = blockIdx.y;
-  const int f = blockIdx.z;
-  const int t0 = (p.nk[0] + 63) / 64;
-  const int ntiles = t0 + (p.nseg > 1 ? (p.nk[1] + 63) / 64 : 0);
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
-    mbar_init(bar_q, 1);
-    for (int s = 0; s < kSplitStages; ++s) {
-      mbar_init(&full_k[s], 1); mbar_init(&empty_k[s], 1);
-      mbar_init(&full_v[s], 1); mbar_init(&empty_v[s], 1);
-    }
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(&bar_s[g], 1); mbar_init(&bar_sfree[g], 128);
-      mbar_init(&bar_p[g], 128); mbar_init(&bar_pv[g], 1);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 256u);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  // key rows of tile j in its segment's K / V matrix
-  auto tile_row = [&](int j, int* seg) -> long long {
-    const int sg = j < t0 ? 0 : 1;
-    *seg = sg;
-    const int k0 = (sg ? j - t0 : j) * 64;
-    return (long long)(f / p.fdiv[sg]) * p.fmul[sg] + p.fadd[sg] + k0;
-  };
-
-  if (warp == 0) {
-    if (elect_one()) {
-      mbar_expect_tx(bar_q, (uint32_t)kAtomBytes);
-      tma_load_2d(sQ, &tmQ, bar_q, h * p.dp, f * p.Nq + q0);
-    }
-    __syncwarp();
-    auto load_k = [&](int j) {
-      int seg;
-      const long long row = tile_row(j, &seg);
-      const int st = j % kSplitStages;
-      mbar_wait(&empty_k[st], ((j / kSplitStages) & 1) ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&full_k[st], (uint32_t)kKvTileBytes);
-        tma_load_2d(sK + st * kKvTileBytes, seg ? &tmK1 : &tmK0, &full_k[st], h * p.dp, (int)row);
-      }
-      __syncwarp();
-    };
-    load_k(0);
-    if (ntiles > 1) load_k(1);
-    for (int j = 0; j < ntiles; ++j) {
-      if (j + 2 < ntiles) load_k(j + 2);     // K runs two tiles ahead: S_{j+2} is computed under softmax j
-      int seg;
-      const long long row = tile_row(j, &seg);
-      const int st = j % kSplitStages;
-      mbar_wait(&empty_v[st], ((j / kSplitStages) & 1) ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&full_v[st], (uint32_t)kKvTileBytes);
-        tma_load_2d(sV + st * kKvTileBytes, seg ? &tmV1 : &tmV0, &full_v[st], h * p.dp, (int)row);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc_s = make_idesc_f16(128, 64, 0, 0);
-    const uint32_t idesc_o = make_idesc_f16(128, p.dp, 0, 1);   // B (= V) is MN-major
-    const int ksteps = p.dp / 16;
-    mbar_wait(bar_q, 0);
-    const uint32_t aQ = smem_u32(sQ);
-    auto issue_s = [&](int j) {
-      const int st = j % kSplitStages;
-      mbar_wait(&full_k[st], (j / kSplitStages) & 1);
-      tc_fence_after();
-      const uint32_t aK = smem_u32(sK + st * kKvTileBytes);
-      if (elect_one()) {
-        for (int kk = 0; kk < ksteps; ++kk)
-          umma_f16_ss(tmem_base + (uint32_t)(j & 1) * 64, make_desc_k_sw128(aQ + kk * 32), make_desc_k_sw128(aK + kk * 32),
-                      idesc_s, kk != 0);
-        umma_commit(&empty_k[st]);
-        umma_commit(&bar_s[j & 1]);
-      }
-      __syncwarp();
-    };
-    issue_s(0);
-    if (ntiles > 1) issue_s(1);
-    for (int j = 0; j < ntiles; ++j) {
-      const int g = j & 1, i = j >> 1;
-      if (j + 2 < ntiles) {
-        mbar_wait(&bar_sfree[g], i & 1);     // group g holds S_j in registers: its S tile may be overwritten
-        issue_s(j + 2);
-      }
-      const int st = j % kSplitStages;
-      mbar_wait(&full_v[st], (j / kSplitStages) & 1);
-      mbar_wait(&bar_p[g], i & 1);
-      tc_fence_after();
-      const uint32_t aP = smem_u32(sP + g * kAtomBytes);
-      const uint32_t aV = smem_u32(sV + st * kKvTileBytes);
-      if (elect_one()) {
+  setmaxnreg_inc<232>();
+  const int wg = (warp - 4) >> 2;                  // query rows [64 wg, 64 wg + 64) of the tile
+  const int wq = warp & 3;
+  long long* tr = (traced && (threadIdx.x & 127) == 0) ? p.trace + (1 + wg) * 32 * 8 : nullptr;
+  // this thread's two rows: 16 wq + lane/4 and +8; its columns of every 8-column group: 2 (lane % 4) + {0, 1}
+  const int cq = 2 * (lane & 3);
+  const uint32_t aQ = smem_u32(sQ) + (uint32_t)wg * 64 * 128;
+  const float sl2 = p.scale_log2;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  float o[DP / 2];
 #pragma unroll
-        for (int k16 = 0; k16 < 4; ++k16)
-          umma_f16_ss(tmem_base + 128 + (uint32_t)g * 64, make_desc_k_sw128(aP + (uint32_t)k16 * 32),
-                      make_desc_mn_sw128(aV + (uint32_t)k16 * 2048, kKvTileBytes), idesc_o, (i | k16) != 0);
-        umma_commit(&empty_v[st]);
-        umma_commit(&bar_pv[g]);
-      }
-      __syncwarp();
-    }
-  } else {
-    const int qd = warp & 3;
-    const int g = (warp - 2) >> 2;                  // softmax group: KV tiles j = g, g + 2, ...
-    const int row = qd * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-    const uint32_t tmem_S = tmem_base + (uint32_t)g * 64 + lane_off;
-    const uint32_t tmem_O = tmem_base + 128 + (uint32_t)g * 64 + lane_off;
-    const uint32_t a_prow = smem_u32(sP) + (uint32_t)g * kAtomBytes + (uint32_t)row * 128;
-    const uint32_t rx = (uint32_t)(row & 7) << 4;
-    const uint32_t a_bar_s = smem_u32(&bar_s[g]), a_bar_sfree = smem_u32(&bar_sfree[g]), a_bar_pv = smem_u32(&bar_pv[g]),
-                   a_bar_p = smem_u32(&bar_p[g]);
-    const int ng = (ntiles - g + 1) / 2;            // tiles of this group
-    float m = -INFINITY, l = 0.f;
-    const float sl2 = p.scale_log2;
-    for (int i = 0; i < ng; ++i) {
-      const int j = 2 * i + g;
-      const int valid = j < t0 ? min(64, p.nk[0] - j * 64) : min(64, p.nk[1] - (j - t0) * 64);
-      mbar_wait_a(a_bar_s, i & 1);
-      tc_fence_after();
-      uint32_t v[64];
-      tmem_ld32(tmem_S, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-      tmem_ld32(tmem_S + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive_a(a_bar_sfree);
-      if (valid < 64) {
-#pragma unroll
-        for (int c = 0; c < 64; ++c)
-          if (c >= valid) v[c] = 0xff800000u;   // -inf
-      }
-      float mxs[8];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) mxs[c] = __uint_as_float(v[c]);
-#pragma unroll
-      for (int c = 8; c < 64; c += 8) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) mxs[e] = fmaxf(mxs[e], __uint_as_float(v[c + e]));
-      }
-      const float mx = fmaxf(fmaxf(fmaxf(mxs[0], mxs[1]), fmaxf(mxs[2], mxs[3])),
-                             fmaxf(fmaxf(mxs[4], mxs[5]), fmaxf(mxs[6], mxs[7]))) * sl2;
-      const bool need = mx > m + 8.f;      // lazy rescale: P stays below 2^8, far inside fp16 range
-      float alpha = 1.f;
-      if (need) { alpha = fast_exp2(m - mx); m = mx; }
-      if (i > 0) {
-        mbar_wait_a(a_bar_pv, (i - 1) & 1);  // P_g free again and O_g final before it is rescaled
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, need)) {
-          for (int c0 = 0; c0 < p.dp; c0 += 16) {
-            uint32_t o[16];
-            tmem_ld16(tmem_O + c0, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-            tmem_st16(tmem_O + c0, o);
-          }
-          tmem_st_wait();
-        }
-      }
-      const F2 sl2x2 = f2_make(sl2, sl2), nmx2 = f2_make(-m, -m);
-      float ls0 = 0.f, ls1 = 0.f;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {   // 8 chunks of 8 keys = one 16-byte smem store each
-        uint32_t ph[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int pi = c * 4 + e;
-          float a0, a1;
-          f2_get(f2_fma(f2_make(__uint_as_float(v[2 * pi]), __uint_as_float(v[2 * pi + 1])), sl2x2, nmx2), a0, a1);
-          float p0, p1;
-          if (((pi * kPolyOf8) & 7) < kPolyOf8) {
-            poly_exp2_pair(a0, a1, p0, p1);
-          } else {
-            p0 = fast_exp2(a0);
-            p1 = fast_exp2(a1);
-          }
-          const __half2 hp = __floats2half2_rn(p0, p1);
-          ph[e] = *reinterpret_cast<const uint32_t*>(&hp);
-          if (!kSumInV) {
-            const float2 back = __half22float2(hp);
-            ls0 += back.x; ls1 += back.y;
-          }
-        }
-        sts128(a_prow + (((uint32_t)c << 4) ^ rx), ph[0], ph[1], ph[2], ph[3]);
-      }
-      if (!kSumInV) l = l * alpha + (ls0 + ls1);
-      fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive_a(a_bar_p);
-    }
-    // ---- merge the two groups
-    if (ng > 0) {
-      mbar_wait_a(a_bar_pv, (ng - 1) & 1);
-      tc_fence_after();
-    }
-    if (kSumInV && ng > 0) {
-      // the row sum was accumulated by the tensor core: V carries a column of ones at index d
-      uint32_t o[16];
-      tmem_ld16(tmem_O + (p.d / 16) * 16, o);
-      tmem_ld_wait();
-      l = __uint_as_float(o[p.d % 16 == 8 ? 8 : 0]);
-    }
-    xch[(g * 128 + row) * 2] = m;
-    xch[(g * 128 + row) * 2 + 1] = l;
-    tc_fence_before();
-    named_bar_sync(1, 256);
-    tc_fence_after();
-    const float m_o = xch[((g ^ 1) * 128 + row) * 2], l_o = xch[((g ^ 1) * 128 + row) * 2 + 1];
-    const float mm = fmaxf(m, m_o);
-    const float w_me = fast_exp2(m - mm), w_o = (m_o == -INFINITY) ? 0.f : fast_exp2(m_o - mm);
-    const float wa = g == 0 ? w_me : w_o, wb = g == 0 ? w_o : w_me;     // weights of O_A / O_B
-    const bool has_b = ntiles > 1;
-    const float inv = p.out_scale / (l * w_me + l_o * w_o);
-    const int qrow = q0 + row;
-    const bool ok = qrow < p.Nq;
-    __half* orow = p.out + ((long long)f * p.Nq + qrow) * p.ldo + h * p.d;
-    const uint32_t tmem_OA = tmem_base + 128 + lane_off, tmem_OB = tmem_base + 192 + lane_off;
-    for (int c0 = g * 16; c0 < p.dp; c0 += 32) {    // the two threads of a row split the columns by chunk parity
-      uint32_t oa[16], ob[16];
-      tmem_ld16(tmem_OA + c0, oa);
-      if (has_b) tmem_ld16(tmem_OB + c0, ob);
-      tmem_ld_wait();
-      if (ok) {
-#pragma unroll
-        for (int gg = 0; gg < 2; ++gg) {
-          const int cc = c0 + gg * 8;
-          if (cc < p.d) {
-            __align__(16) __half oh[8];
-            if (p.accumulate) *reinterpret_cast<uint4*>(oh) = *reinterpret_cast<const uint4*>(orow + cc);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              float x = __uint_as_float(oa[gg * 8 + e]) * wa;
-              if (has_b) x = fmaf(__uint_as_float(ob[gg * 8 + e]), wb, x);
-              x *= inv;
-              if (p.accumulate) x += __half2float(oh[e]);
-              oh[e] = __float2half_rn(x);
-            }
-            *reinterpret_cast<uint4*>(orow + cc) = *reinterpret_cast<const uint4*>(oh);
-          }
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 256u);
-}
-
-
-// exponentials of one score row of the ping-pong kernel: p = 2^(v * scale_log2 - m) for 64 column pairs, packed to fp16;
-// kPolyOf8 of every 8 pairs take the FMA-pipe polynomial, the rest the SFU
-template <bool kSumInV, int kPolyOf8>
-__device__ __forceinline__ void pp_exp_row(const uint32_t (&v)[128], uint32_t (&pk)[64], F2 sl2x2, F2 nmx2, float& ls0, float& ls1) {
-#pragma unroll
-  for (int i = 0; i < 64; ++i) {
-    float a0, a1;
-    f2_get(f2_fma(f2_make(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])), sl2x2, nmx2), a0, a1);
-    float p0, p1;
-    if (((i * kPolyOf8) & 7) < kPolyOf8) {
-      poly_exp2_pair(a0, a1, p0, p1);
-    } else {
-      p0 = fast_exp2(a0);
-      p1 = fast_exp2(a1);
-    }
-    const __half2 hp = __floats2half2_rn(p0, p1);
-    pk[i] = *reinterpret_cast<const uint32_t*>(&hp);
-    if (!kSumInV) {
-      const float2 back = __half22float2(hp);
-      ls0 += back.x; ls1 += back.y;
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------ ping-pong kernel
-// Head dims that fit one 64-column atom (dp <= 64: level 0 of the UNet, where 80 % of the attention time is). The
-// previous kernel was bound by the dependent-issue latency of its softmax: eight warps in lock step on ONE 128x128 score
-// tile, a row max exchanged through smem behind a named barrier, P staged through smem behind a proxy fence, and a
-// single P buffer that serialised softmax j+1 behind P.V j. This kernel restructures the work instead of tuning it:
-//   * one CTA per SM = 256 queries of one (frame, head) = TWO independent 128-query tiles; softmax warpgroup t (4 warps)
-//     owns tile t, ONE THREAD PER QUERY ROW (all 128 scores of the row in registers): no cross-thread max exchange, no
-//     named barrier, 128 independent exp chains per thread for the scheduler to interleave; the two warpgroups run half
-//     an iteration apart, so on every SM sub-partition one warp's waits are covered by the other's arithmetic;
-//   * P never touches shared memory: fp16 probabilities go registers -> TMEM (tcgen05.st) and P.V is a TS-form MMA
-//     (A operand read from tensor memory), which removes 16 st.shared.v4 + a proxy fence per thread per tile;
-//   * row max with 3-input FMNMX3 (half the instructions); exp2 split between SFU and a degree-3 FMA-pipe polynomial.
-//   TMEM (512 columns): S0 0..127 | S1 128..255 | P0 256..319 | P1 320..383 | O0 384..447 | O1 448..511.
-//   smem: Q0, Q1 16 KB each | K ring 4 x 16 KB | V ring 4 x 16 KB | barriers.
-//   warp 0 TMA producer, warp 1 MMA issuer (+ TMEM allocator), warps 2-5 softmax tile 0, warps 6-9 softmax tile 1.
-static constexpr int kPpStages = 4;
-
-template <bool kSumInV, int kPolyOf8, bool kTrace>
-__global__ void __launch_bounds__(320, 1)
-attention_pp_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
-                    const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
-                    const __grid_constant__ CUtensorMap tmV1, const __grid_constant__ AttnParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                                   // [2] tiles
-  uint8_t* sK = sQ + 2 * kAtomBytes;                    // [kPpStages]
-  uint8_t* sV = sK + kPpStages * kAtomBytes;            // [kPpStages]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kPpStages * kAtomBytes);
-  uint64_t* bar_q = bars;                               // 1
-  uint64_t* full_k = bars + 1;                          // [kPpStages]
-  uint64_t* empty_k = full_k + kPpStages;
-  uint64_t* full_v = empty_k + kPpStages;
-  uint64_t* empty_v = full_v + kPpStages;
-  uint64_t* bar_s = empty_v + kPpStages;                // [2] S_t(j) complete in TMEM
-  uint64_t* bar_sfree = bar_s + 2;                      // [2] warpgroup t holds S_t(j) in registers (4 warp arrivals)
-  uint64_t* bar_p = bar_sfree + 2;                      // [2] P_t(j) in TMEM, O_t rescaled (4 warp arrivals)
-  uint64_t* bar_pv = bar_p + 2;                         // [2] P_t(j) V(j) complete: P_t reusable, O_t stable
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_pv + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // (Placing the two service warps at the HIGHEST warp indices instead -- the sub-partition arbiter prefers the highest index
-  // among eligible warps -- was measured: 2.747 vs 2.735 ms, no effect; their issue time is tensor-pipe back-pressure.)
-  const int role = warp;            // 0 = producer, 1 = MMA issuer, 2-5 / 6-9 = softmax of query tile 0 / 1
-  const int q0 = blockIdx.x * 256;
-  const int h = blockIdx.y;
-  const int f = blockIdx.z;
+  for (int i = 0; i < DP / 2; ++i) o[i] = 0.f;
   const int t0 = (p.nk[0] + 127) / 128;
-  const int ntiles = t0 + (p.nseg > 1 ? (p.nk[1] + 127) / 128 : 0);
 
-  if (role == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
-    mbar_init(bar_q, 1);
-    for (int s = 0; s < kPpStages; ++s) {
-      mbar_init(&full_k[s], 1); mbar_init(&empty_k[s], 1);
-      mbar_init(&full_v[s], 1); mbar_init(&empty_v[s], 1);
+  mbar_wait(bar_q, 0);
+  for (int j = 0; j < ntiles; ++j) {
+    const int valid = j < t0 ? min(128, p.nk[0] - j * 128) : min(128, p.nk[1] - (j - t0) * 128);
+    const int ks = j % p.sk, vs = j % p.sv;
+    // ---- S = Q K^T
+    float s[64];
+    mbar_wait(&full_k[ks], (j / p.sk) & 1);
+    const uint32_t aK = smem_u32(sK + ks * kTileBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < DP / 16; ++kk) {
+      const uint32_t off = (uint32_t)(kk >> 2) * kAtomBytes + (uint32_t)(kk & 3) * 32;
+      Wgmma<128>::ss(s, make_desc_k_sw128(aQ + off), make_desc_k_sw128(aK + off), kk != 0);
     }
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&bar_s[t], 1); mbar_init(&bar_sfree[t], 4);
-      mbar_init(&bar_p[t], 4); mbar_init(&bar_pv[t], 1);
-    }
-    fence_barrier_init();
-  }
-  if (role == 1) {
-    tmem_alloc(tmem_slot, 512u);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (role == 0) {
-    // ---- TMA producer
-    if (elect_one()) {
-      mbar_expect_tx(bar_q, 2u * kAtomBytes);
-      tma_load_2d(sQ, &tmQ, bar_q, h * p.dp, f * p.Nq + q0);
-      tma_load_2d(sQ + kAtomBytes, &tmQ, bar_q, h * p.dp, f * p.Nq + q0 + 128);
-    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
     __syncwarp();
-    for (int j = 0; j < ntiles; ++j) {
-      int seg, k0, valid;
-      tile_info(p, j, &seg, &k0, &valid);
-      const long long row = (long long)(f / p.fdiv[seg]) * p.fmul[seg] + p.fadd[seg] + k0;
-      const int st = j % kPpStages;
-      const uint32_t ph = ((uint32_t)(j / kPpStages) & 1u) ^ 1u;
-      mbar_wait(&empty_k[st], ph);
-      if (elect_one()) {
-        mbar_expect_tx(&full_k[st], (uint32_t)kAtomBytes);
-        tma_load_2d(sK + st * kAtomBytes, seg ? &tmK1 : &tmK0, &full_k[st], h * p.dp, (int)row);
-      }
-      __syncwarp();
-      mbar_wait(&empty_v[st], ph);
-      if (elect_one()) {
-        mbar_expect_tx(&full_v[st], (uint32_t)kAtomBytes);
-        tma_load_2d(sV + st * kAtomBytes, seg ? &tmV1 : &tmV0, &full_v[st], h * p.dp, (int)row);
-      }
-      __syncwarp();
-    }
-  } else if (role == 1) {
-    // ---- MMA issuer (warp-uniform loop, one elected lane issues), blocking mbarrier waits. Issue order per KV tile j:
-    // S_0(j+1), P_0(j) V(j), S_1(j+1), P_1(j) V(j). All descriptors are built once (the per-stage / per-k-step variation is an
-    // add on the 14-bit start-address field) and the k loops are fully unrolled.
-    // What the phase trace (tools/gpu_attention_trace.py, profiles/r02_attention_trace.txt) says about this warp: each issue
-    // sequence takes 240-390 cycles (tcgen05.mma issue blocks while the tensor-pipe queue is full), so it is busy half of every
-    // KV-tile period, and the two softmax warps that share its scheduler run ~300 cycles per tile behind their siblings and set
-    // the period. Three restructurings were built and measured against it on one box, all slower: both S tiles first, then both
-    // P.V (+2 %); readiness polling instead of a fixed order (+50 %: the spinning warp starves its scheduler's softmax warps);
-    // the MMAs of each tile issued by one of that tile's own softmax warps (+24 %: the issuing warp blocks 400-500 cycles per
-    // sequence); one MMA warp per tile in a 384-thread CTA (+10 %: the two softmax warpgroups then run in lock step and collide
-    // on the SFU instead of alternating; 384 threads alone cost 6 %).
-    const uint32_t idesc_s = make_idesc_f16(128, 128, 0, 0);
-    const uint32_t idesc_o = make_idesc_f16(128, p.dp, 0, 1);   // B (= V) is MN-major
-    const int ksteps = p.dp / 16;
-    const uint64_t dQ0 = make_desc_k_sw128(smem_u32(sQ));
-    constexpr uint64_t kTileStep = kAtomBytes >> 4;            // descriptor start-address units (16 bytes) per Q tile / ring stage
-    const uint64_t dK0 = make_desc_k_sw128(smem_u32(sK));
-    const uint64_t dV0 = make_desc_mn_sw128(smem_u32(sV), kAtomBytes);
-    const uint32_t tS0 = tmem_base, tP0 = tmem_base + 256u, tO0 = tmem_base + 384u;
-    long long* const tr = (kTrace && p.trace != nullptr && (blockIdx.x | blockIdx.y | blockIdx.z) == 0 && lane == 0) ? p.trace + 8 * 256 : nullptr;
-    auto issue_s = [&](int t, int j) {        // S_t(j) = Q_t K(j)^T
-      const int st = j % kPpStages;
-      if (t == 0) mbar_wait(&full_k[st], (uint32_t)(j / kPpStages) & 1u);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t dq = dQ0 + (uint64_t)t * kTileStep, dk = dK0 + (uint64_t)st * kTileStep;
-        const uint32_t ts = tS0 + (uint32_t)t * 128u;
-        umma_f16_ss(ts, dq, dk, idesc_s, 0);
-        if (ksteps > 1) umma_f16_ss(ts, dq + 2, dk + 2, idesc_s, 1);
-        if (ksteps > 2) umma_f16_ss(ts, dq + 4, dk + 4, idesc_s, 1);
-        if (ksteps > 3) umma_f16_ss(ts, dq + 6, dk + 6, idesc_s, 1);
-        umma_commit(&bar_s[t]);
-        if (t == 1) umma_commit(&empty_k[st]);   // both tiles have read this K stage
-      }
-      __syncwarp();
-    };
-    auto issue_pv = [&](int t, int j) {       // O_t += P_t(j) V(j)
-      const int st = j % kPpStages;
-      if (t == 0) mbar_wait(&full_v[st], (uint32_t)(j / kPpStages) & 1u);
-      mbar_wait(&bar_p[t], (uint32_t)j & 1u);           // P_t(j) in TMEM, O_t rescaled
-      if constexpr (kTrace) pp_stamp(tr, j, t * 4 + 2);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t dv = dV0 + (uint64_t)st * kTileStep;
-        const uint32_t to = tO0 + (uint32_t)t * 64u, tp = tP0 + (uint32_t)t * 64u;
-#pragma unroll
-        for (int k16 = 0; k16 < 8; ++k16)       // 16 keys = 16 rows of 128 bytes = 2048 bytes = 128 address units per step
-          umma_f16_ts(to, tp + (uint32_t)k16 * 8u, dv + (uint64_t)k16 * 128u, idesc_o, (j | k16) != 0);
-        umma_commit(&bar_pv[t]);
-        if (t == 1) umma_commit(&empty_v[st]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(bar_q, 0);
-    issue_s(0, 0);
-    issue_s(1, 0);
-    if (p.pp_order == 0) {                    // A/B: both S tiles first, then both P.V
-      for (int j = 0; j < ntiles; ++j) {
-        if (j + 1 < ntiles) {
-          for (int t = 0; t < 2; ++t) {
-            mbar_wait(&bar_sfree[t], (uint32_t)j & 1u);   // S_t(j) is in registers: its TMEM tile may be overwritten
-            issue_s(t, j + 1);
-          }
-        }
-        issue_pv(0, j);
-        issue_pv(1, j);
-      }
-    } else {
-      for (int j = 0; j < ntiles; ++j) {
-        for (int t = 0; t < 2; ++t) {
-          if (j + 1 < ntiles) {
-            mbar_wait(&bar_sfree[t], (uint32_t)j & 1u);
-            if constexpr (kTrace) pp_stamp(tr, j, t * 4 + 0);                   // S_t(j) left TMEM
-            issue_s(t, j + 1);
-            if constexpr (kTrace) pp_stamp(tr, j, t * 4 + 1);                   // S_t(j+1) issued
-          }
-          issue_pv(t, j);
-          if constexpr (kTrace) pp_stamp(tr, j, t * 4 + 3);                     // P_t(j) V(j) issued
-        }
-      }
-    }
-  } else {
-    // ---- softmax warpgroup t: one thread per query row of tile t
-    const int t = (role - 2) >> 2;
-    const int qd = warp & 3;                            // TMEM lane quarter this warp may access
-    const int row = qd * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-    const uint32_t tS = tmem_base + (uint32_t)t * 128u + lane_off;
-    const uint32_t tP = tmem_base + 256u + (uint32_t)t * 64u + lane_off;
-    const uint32_t tO = tmem_base + 384u + (uint32_t)t * 64u + lane_off;
-    const uint32_t a_bar_s = smem_u32(&bar_s[t]), a_bar_sfree = smem_u32(&bar_sfree[t]), a_bar_p = smem_u32(&bar_p[t]),
-                   a_bar_pv = smem_u32(&bar_pv[t]);
-    float m = -INFINITY, l = 0.f;
-    const float sl2 = p.scale_log2;
-    // Optional (p.pp_alternate, off by default): a token passed through two named barriers per lane quarter makes the
-    // exponential phases of the tile-0 and tile-1 warps that share an SM sub-partition (and its SFU) ALTERNATE, the ordering
-    // FlashAttention-4 imposes between its softmax warpgroups. Measured: no effect with MMA order 1 (2.887 vs 2.884 ms),
-    // needed with order 0 (2.95 vs 3.39 ms). Kept for A/B runs.
-    const int bar_mine = 1 + qd * 2 + t, bar_other = 1 + qd * 2 + (t ^ 1);
-    const bool alternate = p.pp_alternate != 0;
-    if (alternate && t == 1) named_bar_arrive(bar_other, 64);
-    long long* const tr = (kTrace && p.trace != nullptr && (blockIdx.x | blockIdx.y | blockIdx.z) == 0 && lane == 0) ? p.trace + (t * 4 + qd) * 256 : nullptr;
-    for (int j = 0; j < ntiles; ++j) {
-      const int valid = j < t0 ? min(128, p.nk[0] - j * 128) : min(128, p.nk[1] - (j - t0) * 128);
-      if constexpr (kTrace) pp_stamp(tr, j, 0);
-      mbar_wait_a(a_bar_s, (uint32_t)j & 1u);
-      if constexpr (kTrace) pp_stamp(tr, j, 1);                                // S_t(j) complete
-      tc_fence_after();
-      uint32_t v[128];                                  // the whole score row of this thread
-      tmem_ld32(tS, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-      tmem_ld32(tS + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-      tmem_ld32(tS + 64, *reinterpret_cast<uint32_t(*)[32]>(&v[64]));
-      tmem_ld32(tS + 96, *reinterpret_cast<uint32_t(*)[32]>(&v[96]));
-      tmem_ld_wait();
-      if constexpr (kTrace) pp_stamp(tr, j, 2);                                // scores in registers
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_a(a_bar_sfree);       // the tensor core may start S_t(j+1)
-      if (valid < 128) {
-#pragma unroll
-        for (int i = 0; i < 128; ++i)
-          if (i >= valid) v[i] = 0xff800000u;          // -inf
-      }
-      float mx0 = __uint_as_float(v[0]), mx1 = __uint_as_float(v[1]), mx2 = __uint_as_float(v[2]), mx3 = __uint_as_float(v[3]);
-      float mx4 = __uint_as_float(v[4]), mx5 = __uint_as_float(v[5]), mx6 = __uint_as_float(v[6]), mx7 = __uint_as_float(v[7]);
-#pragma unroll
-      for (int i = 8; i < 120; i += 16) {               // eight independent FMNMX3 chains (a chain of 16 was latency-bound)
-        mx0 = fmax3(mx0, __uint_as_float(v[i]), __uint_as_float(v[i + 1]));
-        mx1 = fmax3(mx1, __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-        mx2 = fmax3(mx2, __uint_as_float(v[i + 4]), __uint_as_float(v[i + 5]));
-        mx3 = fmax3(mx3, __uint_as_float(v[i + 6]), __uint_as_float(v[i + 7]));
-        mx4 = fmax3(mx4, __uint_as_float(v[i + 8]), __uint_as_float(v[i + 9]));
-        mx5 = fmax3(mx5, __uint_as_float(v[i + 10]), __uint_as_float(v[i + 11]));
-        mx6 = fmax3(mx6, __uint_as_float(v[i + 12]), __uint_as_float(v[i + 13]));
-        mx7 = fmax3(mx7, __uint_as_float(v[i + 14]), __uint_as_float(v[i + 15]));
-      }
-      mx0 = fmax3(mx0, __uint_as_float(v[120]), __uint_as_float(v[121]));
-      mx1 = fmax3(mx1, __uint_as_float(v[122]), __uint_as_float(v[123]));
-      mx2 = fmax3(mx2, __uint_as_float(v[124]), __uint_as_float(v[125]));
-      mx3 = fmax3(mx3, __uint_as_float(v[126]), __uint_as_float(v[127]));
-      const float mx = fmax3(fmax3(mx0, mx1, mx2), fmax3(mx3, mx4, mx5), fmaxf(mx6, mx7)) * sl2;
-      const bool need = mx > m + 8.f;                   // lazy rescale: P stays below 2^8, far inside fp16 range
-      if constexpr (kTrace) pp_stamp(tr, j, 3);                                // row max known
-      float alpha = 1.f;
-      if (need) { alpha = fast_exp2(m - mx); m = mx; }
-      const F2 sl2x2 = f2_make(sl2, sl2), nmx2 = f2_make(-m, -m);
-      float ls0 = 0.f, ls1 = 0.f;
-      if (alternate) named_bar_sync(bar_mine, 64);      // my turn on the SFU
-      uint32_t pk[64];
-      // (Giving the two warps that share the MMA-issuing warp's scheduler a different FMA-pipe share was measured: 0/8 +12 %, 4/8 +3 %.)
-      pp_exp_row<kSumInV, kPolyOf8>(v, pk, sl2x2, nmx2, ls0, ls1);
-      if (alternate) named_bar_arrive(bar_other, 64);   // the other tile's warp may start its exponentials
-      // P_t's TMEM columns and O_t are free / final once P_t(j-1) V(j-1) has completed. That MMA was issued when this
-      // thread finished the PREVIOUS tile, so taking the wait here, after the whole softmax of this tile, gives it a full
-      // iteration of slack. (Taking it before the exponentials, to let the P stores leave chunk by chunk, cost 7 % of the
-      // softmax warps' samples on this wait and bought nothing.)
-      if constexpr (kTrace) pp_stamp(tr, j, 4);                                // exponentials done
-      if (j > 0) {
-        mbar_wait_a(a_bar_pv, (uint32_t)(j - 1) & 1u);
-        if constexpr (kTrace) pp_stamp(tr, j, 5);                              // P_t(j-1) V(j-1) complete
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, need)) {
-          for (int c0 = 0; c0 < p.dp; c0 += 16) {
-            uint32_t o[16];
-            tmem_ld16(tO + c0, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-            tmem_st16(tO + c0, o);
-          }
-        }
-      }
-      tmem_st32(tP, *reinterpret_cast<uint32_t(*)[32]>(&pk[0]));
-      tmem_st32(tP + 32, *reinterpret_cast<uint32_t(*)[32]>(&pk[32]));
-      if (!kSumInV) l = l * alpha + (ls0 + ls1);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_a(a_bar_p);
-      if constexpr (kTrace) pp_stamp(tr, j, 6);                                // P_t(j) published
-    }
-    if (alternate && t == 0) named_bar_sync(bar_mine, 64);   // consume the last token so that no arrival is left pending
-    // ---- epilogue: O_t row / row sum -> global
-    mbar_wait_a(a_bar_pv, (uint32_t)(ntiles - 1) & 1u);
-    tc_fence_after();
-    if (kSumInV) {
-      uint32_t o[16];
-      tmem_ld16(tO + (p.d / 16) * 16, o);
-      tmem_ld_wait();
-      l = __uint_as_float(o[p.d % 16 == 8 ? 8 : 0]);     // the ones column of V accumulated the row sum
-    }
-    const float inv = p.out_scale / l;
-    const int qrow = q0 + t * 128 + row;
-    const bool ok = qrow < p.Nq;
-    __half* orow = p.out + ((long long)f * p.Nq + qrow) * p.ldo + h * p.d;
-    for (int c0 = 0; c0 < p.dp; c0 += 16) {
-      uint32_t o[16];
-      tmem_ld16(tO + c0, o);
-      tmem_ld_wait();
-      if (ok) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          const int cc = c0 + g * 8;
-          if (cc < p.d) {
-            __align__(16) __half oh[8];
-            if (p.accumulate) *reinterpret_cast<uint4*>(oh) = *reinterpret_cast<const uint4*>(orow + cc);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              float x = __uint_as_float(o[g * 8 + e]) * inv;
-              if (p.accumulate) x += __half2float(oh[e]);
-              oh[e] = __float2half_rn(x);
-            }
-            *reinterpret_cast<uint4*>(orow + cc) = *reinterpret_cast<const uint4*>(oh);
-          }
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (role == 1) tmem_dealloc(tmem_base, 512u);
-}
+    if (lane == 0) mbar_arrive(&empty_k[ks]);
+    att_stamp(tr, j, 0);
 
-
-// Same kernel with TWO threads per query row (16 softmax warps): see the comment at its softmax section.
-template <bool kSumInV, int kPolyOf8>
-__global__ void __launch_bounds__(576, 1)
-attention_pp2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
-                    const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
-                    const __grid_constant__ CUtensorMap tmV1, const __grid_constant__ AttnParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                                   // [2] tiles
-  uint8_t* sK = sQ + 2 * kAtomBytes;                    // [kPpStages]
-  uint8_t* sV = sK + kPpStages * kAtomBytes;            // [kPpStages]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kPpStages * kAtomBytes);
-  uint64_t* bar_q = bars;                               // 1
-  uint64_t* full_k = bars + 1;                          // [kPpStages]
-  uint64_t* empty_k = full_k + kPpStages;
-  uint64_t* full_v = empty_k + kPpStages;
-  uint64_t* empty_v = full_v + kPpStages;
-  uint64_t* bar_s = empty_v + kPpStages;                // [2] S_t(j) complete in TMEM
-  uint64_t* bar_sfree = bar_s + 2;                      // [2] warpgroup t holds S_t(j) in registers (4 warp arrivals)
-  uint64_t* bar_p = bar_sfree + 2;                      // [2] P_t(j) in TMEM, O_t rescaled (4 warp arrivals)
-  uint64_t* bar_pv = bar_p + 2;                         // [2] P_t(j) V(j) complete: P_t reusable, O_t stable
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_pv + 2);
-  float* smax = reinterpret_cast<float*>(bar_pv + 4);   // [2 tiles][2 buffers][2 column halves][128 rows] row-max exchange
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 256;
-  const int h = blockIdx.y;
-  const int f = blockIdx.z;
-  const int t0 = (p.nk[0] + 127) / 128;
-  const int ntiles = t0 + (p.nseg > 1 ? (p.nk[1] + 127) / 128 : 0);
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
-    mbar_init(bar_q, 1);
-    for (int s = 0; s < kPpStages; ++s) {
-      mbar_init(&full_k[s], 1); mbar_init(&empty_k[s], 1);
-      mbar_init(&full_v[s], 1); mbar_init(&empty_v[s], 1);
+    // ---- online softmax on the two rows
+    if (valid < 128) {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        if (8 * i + cq >= valid) { s[4 * i] = -INFINITY; s[4 * i + 2] = -INFINITY; }
+        if (8 * i + cq + 1 >= valid) { s[4 * i + 1] = -INFINITY; s[4 * i + 3] = -INFINITY; }
+      }
     }
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&bar_s[t], 1); mbar_init(&bar_sfree[t], 8);
-      mbar_init(&bar_p[t], 8); mbar_init(&bar_pv[t], 1);
+    float mx0 = s[0], mx1 = s[2];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      mx0 = fmaxf(mx0, fmaxf(s[4 * i], s[4 * i + 1]));
+      mx1 = fmaxf(mx1, fmaxf(s[4 * i + 2], s[4 * i + 3]));
     }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512u);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float mn0 = fmaxf(m0, mx0 * sl2), mn1 = fmaxf(m1, mx1 * sl2);
+    const float alpha0 = fast_exp2(m0 - mn0), alpha1 = fast_exp2(m1 - mn1);   // 0 on the first tile (m = -inf)
+    m0 = mn0; m1 = mn1;
+    // P as the wgmma A fragment: k-slice kk (keys 16 kk .. 16 kk + 15) = accumulator column groups 2 kk, 2 kk + 1
+    uint32_t pa[8][4];
+    float ls0 = 0.f, ls1 = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int i = 2 * kk + hh;
+        pa[kk][2 * hh] = pack_half2(fast_exp2(fmaf(s[4 * i], sl2, -mn0)), fast_exp2(fmaf(s[4 * i + 1], sl2, -mn0)), ls0);
+        pa[kk][2 * hh + 1] =
+            pack_half2(fast_exp2(fmaf(s[4 * i + 2], sl2, -mn1)), fast_exp2(fmaf(s[4 * i + 3], sl2, -mn1)), ls1);
+      }
+    }
+    l0 = l0 * alpha0 + ls0;
+    l1 = l1 * alpha1 + ls1;
+#pragma unroll
+    for (int i = 0; i < DP / 8; ++i) {
+      o[4 * i] *= alpha0; o[4 * i + 1] *= alpha0;
+      o[4 * i + 2] *= alpha1; o[4 * i + 3] *= alpha1;
+    }
+    att_stamp(tr, j, 1);
 
-  if (warp == 0) {
-    // ---- TMA producer
-    if (elect_one()) {
-      mbar_expect_tx(bar_q, 2u * kAtomBytes);
-      tma_load_2d(sQ, &tmQ, bar_q, h * p.dp, f * p.Nq + q0);
-      tma_load_2d(sQ + kAtomBytes, &tmQ, bar_q, h * p.dp, f * p.Nq + q0 + 128);
-    }
+    // ---- O += P V
+    mbar_wait(&full_v[vs], (j / p.sv) & 1);
+    const uint32_t aV = smem_u32(sV + vs * kTileBytes);
+    wgmma_fence();
+    fence_regs(o);
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+      WgmmaRs<DP>::rs(o, pa[kk], make_desc_mn_sw128(aV + (uint32_t)kk * 2048, kAtomBytes), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
     __syncwarp();
-    for (int j = 0; j < ntiles; ++j) {
-      int seg, k0, valid;
-      tile_info(p, j, &seg, &k0, &valid);
-      const long long row = (long long)(f / p.fdiv[seg]) * p.fmul[seg] + p.fadd[seg] + k0;
-      const int st = j % kPpStages;
-      const uint32_t ph = ((uint32_t)(j / kPpStages) & 1u) ^ 1u;
-      mbar_wait(&empty_k[st], ph);
-      if (elect_one()) {
-        mbar_expect_tx(&full_k[st], (uint32_t)kAtomBytes);
-        tma_load_2d(sK + st * kAtomBytes, seg ? &tmK1 : &tmK0, &full_k[st], h * p.dp, (int)row);
-      }
-      __syncwarp();
-      mbar_wait(&empty_v[st], ph);
-      if (elect_one()) {
-        mbar_expect_tx(&full_v[st], (uint32_t)kAtomBytes);
-        tma_load_2d(sV + st * kAtomBytes, seg ? &tmV1 : &tmV0, &full_v[st], h * p.dp, (int)row);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    // ---- MMA issuer (warp-uniform loop, one elected lane issues), blocking mbarrier waits. Issue order per KV tile j
-    // (p.pp_order): 1 (default) = S_0(j+1), P_0(j) V(j), S_1(j+1), P_1(j) V(j); 0 = both S first, then both P.V.
-    // Measured on one box (level 0, 20 launches each): order 1 2.884 ms, order 0 2.948 ms (3.39 ms without the SFU token
-    // below). A third variant that polled all four conditions with non-blocking probes and issued in readiness order was
-    // 50 % SLOWER: the spinning MMA warp starves the two softmax warps that share its scheduler.
-    // The issuing warp shares its scheduler with two softmax warps, so every instruction it needs costs it a turn: all
-    // descriptors are built once (the per-stage / per-k-step variation is an add on the 14-bit start-address field) and
-    // the k loops are fully unrolled. (ncu: the first version spent ~300 scalar instructions per KV tile here.)
-    const uint32_t idesc_s = make_idesc_f16(128, 128, 0, 0);
-    const uint32_t idesc_o = make_idesc_f16(128, p.dp, 0, 1);   // B (= V) is MN-major
-    const int ksteps = p.dp / 16;
-    const uint64_t dQ[2] = {make_desc_k_sw128(smem_u32(sQ)), make_desc_k_sw128(smem_u32(sQ + kAtomBytes))};
-    const uint64_t dK0 = make_desc_k_sw128(smem_u32(sK));
-    const uint64_t dV0 = make_desc_mn_sw128(smem_u32(sV), kAtomBytes);
-    constexpr uint64_t kStageStep = kAtomBytes >> 4;           // descriptor start-address units (16 bytes) per ring stage
-    const uint32_t tS0 = tmem_base, tP0 = tmem_base + 256u, tO0 = tmem_base + 384u;
-    mbar_wait(bar_q, 0);
-    auto issue_s = [&](int t, int j) {        // S_t(j) = Q_t K(j)^T
-      const int st = j % kPpStages;
-      if (t == 0) mbar_wait(&full_k[st], (uint32_t)(j / kPpStages) & 1u);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t dq = dQ[t], dk = dK0 + (uint64_t)st * kStageStep;
-        const uint32_t ts = tS0 + (uint32_t)t * 128u;
-        umma_f16_ss(ts, dq, dk, idesc_s, 0);
-        if (ksteps > 1) umma_f16_ss(ts, dq + 2, dk + 2, idesc_s, 1);
-        if (ksteps > 2) umma_f16_ss(ts, dq + 4, dk + 4, idesc_s, 1);
-        if (ksteps > 3) umma_f16_ss(ts, dq + 6, dk + 6, idesc_s, 1);
-        umma_commit(&bar_s[t]);
-        if (t == 1) umma_commit(&empty_k[st]);   // both tiles have read this K stage
-      }
-      __syncwarp();
-    };
-    issue_s(0, 0);
-    issue_s(1, 0);
-    auto issue_pv = [&](int t, int j) {       // O_t += P_t(j) V(j)
-      const int st = j % kPpStages;
-      if (t == 0) mbar_wait(&full_v[st], (uint32_t)(j / kPpStages) & 1u);
-      mbar_wait(&bar_p[t], (uint32_t)j & 1u);           // P_t(j) in TMEM, O_t rescaled
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t dv = dV0 + (uint64_t)st * kStageStep;
-        const uint32_t to = tO0 + (uint32_t)t * 64u, tp = tP0 + (uint32_t)t * 64u;
+    if (lane == 0) mbar_arrive(&empty_v[vs]);
+    att_stamp(tr, j, 2);
+  }
+
+  // ---- epilogue: full row sums, out = out_scale * O / l (+ out)
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv[2] = {p.out_scale / l0, p.out_scale / l1};
 #pragma unroll
-        for (int k16 = 0; k16 < 8; ++k16)       // 16 keys = 16 rows of 128 bytes = 2048 bytes = 128 address units per step
-          umma_f16_ts(to, tp + (uint32_t)k16 * 8u, dv + (uint64_t)k16 * 128u, idesc_o, (j | k16) != 0);
-        umma_commit(&bar_pv[t]);
-        if (t == 1) umma_commit(&empty_v[st]);
-      }
-      __syncwarp();
-    };
-    if (p.pp_order == 0) {
-      for (int j = 0; j < ntiles; ++j) {
-        if (j + 1 < ntiles) {
-          for (int t = 0; t < 2; ++t) {
-            mbar_wait(&bar_sfree[t], (uint32_t)j & 1u);   // S_t(j) is in registers: its TMEM tile may be overwritten
-            issue_s(t, j + 1);
-          }
-        }
-        issue_pv(0, j);
-        issue_pv(1, j);
-      }
-    } else {                                  // A/B: the interleaved order S_0, PV_0, S_1, PV_1
-      for (int j = 0; j < ntiles; ++j) {
-        for (int t = 0; t < 2; ++t) {
-          if (j + 1 < ntiles) {
-            mbar_wait(&bar_sfree[t], (uint32_t)j & 1u);
-            issue_s(t, j + 1);
-          }
-          issue_pv(t, j);
-        }
-      }
-    }
-  } else {
-    // ---- softmax: 8 warps per query tile, TWO threads per query row (64 of the 128 key columns each). Warps w and w+4 of a
-    // tile hold the two halves of the same 32 rows and agree on the row max through smem behind a 64-thread named barrier.
-    // Four softmax warps per SM sub-partition instead of two: tools/microbench/mufu_rate shows that two warps in the
-    // exponential phase drive the SFU at ~90 %, one alone at ~65-70 %, and with one thread per row each warp is in that
-    // phase only about half of the time.
-    const int sw = warp - 2;
-    const int t = sw >> 3;                              // query tile
-    const int ch = (sw >> 2) & 1;                       // column half: keys [64 ch, 64 ch + 64) of the KV tile
-    const int qd = warp & 3;                            // TMEM lane quarter this warp may access
-    const int row = qd * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-    const uint32_t tS = tmem_base + (uint32_t)t * 128u + (uint32_t)ch * 64u + lane_off;
-    const uint32_t tP = tmem_base + 256u + (uint32_t)t * 64u + (uint32_t)ch * 32u + lane_off;
-    const uint32_t tO = tmem_base + 384u + (uint32_t)t * 64u + lane_off;
-    const uint32_t a_bar_s = smem_u32(&bar_s[t]), a_bar_sfree = smem_u32(&bar_sfree[t]), a_bar_p = smem_u32(&bar_p[t]),
-                   a_bar_pv = smem_u32(&bar_pv[t]);
-    const uint32_t a_mine = smem_u32(smax) + (uint32_t)((t * 4 + ch) * 128 + row) * 4;
-    const uint32_t a_peer = smem_u32(smax) + (uint32_t)((t * 4 + (ch ^ 1)) * 128 + row) * 4;
-    const int pair_bar = 1 + t * 4 + qd;                // named barrier of this row pair (64 threads)
-    float m = -INFINITY, l = 0.f;
-    const float sl2 = p.scale_log2;
-    for (int j = 0; j < ntiles; ++j) {
-      const int valid = j < t0 ? min(128, p.nk[0] - j * 128) : min(128, p.nk[1] - (j - t0) * 128);
-      mbar_wait_a(a_bar_s, (uint32_t)j & 1u);
-      tc_fence_after();
-      uint32_t v[64];
-      tmem_ld32(tS, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-      tmem_ld32(tS + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_a(a_bar_sfree);       // the tensor core may start S_t(j+1)
-      if (valid < 128) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i)
-          if (ch * 64 + i >= valid) v[i] = 0xff800000u;   // -inf
-      }
-      float mx0 = __uint_as_float(v[0]), mx1 = __uint_as_float(v[1]), mx2 = __uint_as_float(v[2]), mx3 = __uint_as_float(v[3]);
-#pragma unroll
-      for (int i = 4; i < 60; i += 8) {
-        mx0 = fmax3(mx0, __uint_as_float(v[i]), __uint_as_float(v[i + 1]));
-        mx1 = fmax3(mx1, __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-        mx2 = fmax3(mx2, __uint_as_float(v[i + 4]), __uint_as_float(v[i + 5]));
-        mx3 = fmax3(mx3, __uint_as_float(v[i + 6]), __uint_as_float(v[i + 7]));
-      }
-      mx0 = fmax3(mx0, __uint_as_float(v[60]), __uint_as_float(v[61]));
-      mx1 = fmax3(mx1, __uint_as_float(v[62]), __uint_as_float(v[63]));
-      float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-      const uint32_t xoff = (uint32_t)(j & 1) * 1024;   // second buffer = [.. + 2 halves * 128 rows * 4 B]
-      sts32f(a_mine + xoff, mx);
-      named_bar_sync(pair_bar, 64);
-      mx = fmaxf(mx, lds32f(a_peer + xoff)) * sl2;
-      const bool need = mx > m + 8.f;                   // lazy rescale: P stays below 2^8, far inside fp16 range
-      float alpha = 1.f;
-      if (need) { alpha = fast_exp2(m - mx); m = mx; }
-      const F2 sl2x2 = f2_make(sl2, sl2), nmx2 = f2_make(-m, -m);
-      float ls0 = 0.f, ls1 = 0.f;
-      uint32_t pk[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {                    // column pair i; kPolyOf8 of every 8 pairs take the FMA-pipe exp2
-        float a0, a1;
-        f2_get(f2_fma(f2_make(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])), sl2x2, nmx2), a0, a1);
-        float p0, p1;
-        if (((i * kPolyOf8) & 7) < kPolyOf8) {
-          poly_exp2_pair(a0, a1, p0, p1);
-        } else {
-          p0 = fast_exp2(a0);
-          p1 = fast_exp2(a1);
-        }
-        const __half2 hp = __floats2half2_rn(p0, p1);
-        pk[i] = *reinterpret_cast<const uint32_t*>(&hp);
-        if (!kSumInV) {
-          const float2 back = __half22float2(hp);
-          ls0 += back.x; ls1 += back.y;
-        }
-      }
-      if (j > 0) {
-        mbar_wait_a(a_bar_pv, (uint32_t)(j - 1) & 1u);  // P_t free again and O_t(j-1) final before it is rescaled
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, need)) {
-          for (int c0 = ch * 16; c0 < p.dp; c0 += 32) { // the two threads of a row split the O columns by chunk parity
-            uint32_t o[16];
-            tmem_ld16(tO + c0, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-            tmem_st16(tO + c0, o);
-          }
-        }
-      }
-      tmem_st32(tP, pk);
-      if (!kSumInV) l = l * alpha + (ls0 + ls1);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_a(a_bar_p);
-    }
-    // ---- epilogue: O_t row / row sum -> global
-    mbar_wait_a(a_bar_pv, (uint32_t)(ntiles - 1) & 1u);
-    tc_fence_after();
-    if (kSumInV) {
-      uint32_t o[16];
-      tmem_ld16(tO + (p.d / 16) * 16, o);
-      tmem_ld_wait();
-      l = __uint_as_float(o[p.d % 16 == 8 ? 8 : 0]);     // the ones column of V accumulated the row sum
-    } else {
-      const uint32_t xoff = (uint32_t)(ntiles & 1) * 1024;
-      sts32f(a_mine + xoff, l);
-      named_bar_sync(pair_bar, 64);
-      l += lds32f(a_peer + xoff);
-    }
-    const float inv = p.out_scale / l;
-    const int qrow = q0 + t * 128 + row;
-    const bool ok = qrow < p.Nq;
+  for (int rr = 0; rr < 2; ++rr) {
+    const int qrow = q0 + 64 * wg + 16 * wq + (lane >> 2) + 8 * rr;
+    if (qrow >= p.Nq) continue;
     __half* orow = p.out + ((long long)f * p.Nq + qrow) * p.ldo + h * p.d;
-    for (int c0 = ch * 16; c0 < p.dp; c0 += 32) {
-      uint32_t o[16];
-      tmem_ld16(tO + c0, o);
-      tmem_ld_wait();
-      if (ok) {
 #pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          const int cc = c0 + g * 8;
-          if (cc < p.d) {
-            __align__(16) __half oh[8];
-            if (p.accumulate) *reinterpret_cast<uint4*>(oh) = *reinterpret_cast<const uint4*>(orow + cc);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              float x = __uint_as_float(o[g * 8 + e]) * inv;
-              if (p.accumulate) x += __half2float(oh[e]);
-              oh[e] = __float2half_rn(x);
-            }
-            *reinterpret_cast<uint4*>(orow + cc) = *reinterpret_cast<const uint4*>(oh);
-          }
+    for (int i = 0; i < DP / 8; ++i) {
+      const int cc = 8 * i + cq;
+      if (cc < p.d) {
+        float x0 = o[4 * i + 2 * rr] * inv[rr], x1 = o[4 * i + 2 * rr + 1] * inv[rr];
+        __half2* dst = reinterpret_cast<__half2*>(orow + cc);
+        if (p.accumulate) {
+          const float2 prev = __half22float2(*dst);
+          x0 += prev.x; x1 += prev.y;
         }
+        *dst = __floats2half2_rn(x0, x1);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512u);
 }
 
 static long long* g_attention_trace = nullptr;
 void set_attention_trace(long long* device_buffer) { g_attention_trace = device_buffer; }
+
+typedef void (*AttnKernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+                             const AttnParams);
+// instantiations for every padded head dim the launcher accepts (multiples of 16 up to 192)
+static const AttnKernelFn kAttnKernels[12] = {
+    attention_kernel<16>,  attention_kernel<32>,  attention_kernel<48>,  attention_kernel<64>,
+    attention_kernel<80>,  attention_kernel<96>,  attention_kernel<112>, attention_kernel<128>,
+    attention_kernel<144>, attention_kernel<160>, attention_kernel<176>, attention_kernel<192>};
 
 cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char** err) {
   if (a.d % 8 || a.dp % 16 || a.dp < a.d || a.dp > 192 || a.nseg < 1 || a.nseg > 2 || a.heads < 1) {
@@ -1348,32 +293,21 @@ cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char*
     if (s < a.nseg && g.nk < 1) { *err = "attention: empty KV segment"; return cudaErrorInvalidValue; }
   }
   p.out = a.out; p.ldo = a.ldo; p.accumulate = a.accumulate;
-  p.sum_in_v = (a.v_ones_col && a.dp > a.d) ? 1 : 0;
-  if (p.natoms == 1) { p.sk = 2; p.sv = 1; }
-  else if (p.natoms == 2) { p.sk = 2; p.sv = 1; }
-  else { p.sk = 1; p.sv = 1; }
-  p.tmem_cols = (128 + a.dp <= 256) ? 256 : 512;
-  const int smem = (1 + p.sk + p.sv) * p.natoms * kAtomBytes + 2 * kAtomBytes + 1024 + 128 + 2048;
-  typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
-                           const AttnParams);
-  static const KernelFn kernels[2][4] = {
-      {attention_kernel<false, 0>, attention_kernel<false, 2>, attention_kernel<false, 3>, attention_kernel<false, 4>},
-      {attention_kernel<true, 0>, attention_kernel<true, 2>, attention_kernel<true, 3>, attention_kernel<true, 4>}};
-  // share of the exp2 work moved from the SFU to the FMA pipe: 0, 2/8 (default), 3/8 or 4/8 (env MVB_POLY, experiments)
-  static const int poly_env = getenv("MVB_POLY") ? atoi(getenv("MVB_POLY")) : 2;
-  const int poly_idx = poly_env <= 0 ? 0 : poly_env == 2 ? 1 : poly_env >= 4 ? 3 : 2;
-  static int max_set_dev[64] = {};     // per device (the attribute belongs to the device's context)
+  p.trace = g_attention_trace;
+  // ring depths: Q + sk K tiles + sv V tiles within the 227 KB of shared memory a block may use
+  if (p.natoms == 1) { p.sk = 4; p.sv = 4; }
+  else if (p.natoms == 2) { p.sk = 2; p.sv = 2; }
+  else { p.sk = 2; p.sv = 1; }
+  const int smem = (1 + p.sk + p.sv) * p.natoms * kAtomBytes + 1024 + 128 + 256;
+  const AttnKernelFn kernel = kAttnKernels[a.dp / 16 - 1];
+  static int max_set_dev[64][12] = {};     // per device (the attribute belongs to the device's context)
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
-  int& max_set = max_set_dev[cur_dev & 63];
+  int& max_set = max_set_dev[cur_dev & 63][a.dp / 16 - 1];
   if (smem > max_set) {
-    cudaError_t e = cudaSuccess;
-    for (int a = 0; a < 2 && e == cudaSuccess; ++a)
-      for (int b = 0; b < 4 && e == cudaSuccess; ++b)
-        e = cudaFuncSetAttribute(reinterpret_cast<const void*>(kernels[a][b]), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(attention_kernel)"; return e; }
-    max_set = 227 * 1024;
+    max_set = smem;
   }
   CUtensorMap tq, tk0, tv0, tk1, tv1;
   const uint64_t cols = (uint64_t)a.heads * a.dp;
@@ -1394,94 +328,7 @@ cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char*
             p.nk[1], a.accumulate);
   dim3 grid((a.Nq + 127) / 128, a.heads, a.NF);
   ProfScope prof(stream, KC_ATTENTION);
-  // split-KV variant for one-atom head dims: measured 12 % SLOWER than the default kernel at level 0 (3.44 vs 3.06 ms,
-  // DESIGN.md section 7), so it only runs on request (AttnArgs.variant = 2 or env MVB_ATTN=2)
-  static const int attn_env = getenv("MVB_ATTN") ? atoi(getenv("MVB_ATTN")) : 0;
-  if (a.dp <= 64 && (a.variant == 2 || attn_env == 2)) {
-    static bool split_set_dev[64] = {};
-    bool& split_set = split_set_dev[cur_dev & 63];
-    const int smem_split = kAtomBytes + 2 * kSplitStages * kKvTileBytes + 2 * kAtomBytes + 1024 + 256 + 2048;
-    if (!split_set) {
-      cudaError_t e = cudaFuncSetAttribute(attention_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_split);
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(attention_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_split);
-      if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(attention_split_kernel)"; return e; }
-      split_set = true;
-    }
-    CUtensorMap sk0, sv0, sk1, sv1;   // 64-key boxes
-    if (!encode_map_2d(&sk0, s0.k, cols, (uint64_t)s0.rows, (uint64_t)s0.ld, 64, 64) ||
-        !encode_map_2d(&sv0, s0.v, cols, (uint64_t)s0.rows, (uint64_t)s0.ld, 64, 64) ||
-        !encode_map_2d(&sk1, s1.k, cols, (uint64_t)s1.rows, (uint64_t)s1.ld, 64, 64) ||
-        !encode_map_2d(&sv1, s1.v, cols, (uint64_t)s1.rows, (uint64_t)s1.ld, 64, 64)) {
-      *err = "cuTensorMapEncodeTiled(K/V, 64-key box) failed"; return cudaErrorInvalidValue;
-    }
-    if (p.sum_in_v) attention_split_kernel<true><<<grid, 320, smem_split, stream>>>(tq, sk0, sv0, sk1, sv1, p);
-    else attention_split_kernel<false><<<grid, 320, smem_split, stream>>>(tq, sk0, sv0, sk1, sv1, p);
-    cudaError_t e2 = cudaGetLastError();
-    if (e2 != cudaSuccess) *err = "attention_split_kernel launch";
-    return e2;
-  }
-  // ping-pong kernel (two query tiles per CTA, P in TMEM) for one-atom head dims; variant 1 / MVB_ATTN=1 forces the
-  // previous kernel for A/B runs
-  if (a.dp <= 64 && a.variant != 1 && attn_env != 1) {
-    static const KernelFn pp_kernels[2][5] = {
-        {attention_pp_kernel<false, 0, false>, attention_pp_kernel<false, 1, false>, attention_pp_kernel<false, 2, false>,
-         attention_pp_kernel<false, 3, false>, attention_pp_kernel<false, 4, false>},
-        {attention_pp_kernel<true, 0, false>, attention_pp_kernel<true, 1, false>, attention_pp_kernel<true, 2, false>,
-         attention_pp_kernel<true, 3, false>, attention_pp_kernel<true, 4, false>}};
-    static const int pp_poly_env = getenv("MVB_POLY") ? atoi(getenv("MVB_POLY")) : 2;
-    const int pp_idx = pp_poly_env <= 0 ? 0 : pp_poly_env >= 4 ? 4 : pp_poly_env;   // FMA-pipe share of the exponentials, n/8
-    const int smem_pp = (2 + 2 * kPpStages) * kAtomBytes + 1024 + 512;
-    static bool pp_set_dev[64] = {};
-    if (!pp_set_dev[cur_dev & 63]) {
-      cudaError_t e = cudaSuccess;
-      for (int x = 0; x < 2 && e == cudaSuccess; ++x)
-        for (int y = 0; y < 5 && e == cudaSuccess; ++y)
-          e = cudaFuncSetAttribute(reinterpret_cast<const void*>(pp_kernels[x][y]), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_pp);
-      if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(attention_pp_kernel)"; return e; }
-      pp_set_dev[cur_dev & 63] = true;
-    }
-    static const int pp_alt_env = getenv("MVB_PP_ALT") ? atoi(getenv("MVB_PP_ALT")) : 0;
-    p.pp_alternate = pp_alt_env;
-    static const int pp_order_env = getenv("MVB_PP_ORDER") ? atoi(getenv("MVB_PP_ORDER")) : 1;
-    p.pp_order = pp_order_env;
-    p.trace = g_attention_trace;
-    dim3 grid_pp((a.Nq + 255) / 256, a.heads, a.NF);
-    // two threads per query row (16 softmax warps per CTA): variant 4 / MVB_ATTN=4
-    static const KernelFn pp2_kernels[2][4] = {
-        {attention_pp2_kernel<false, 0>, attention_pp2_kernel<false, 2>, attention_pp2_kernel<false, 3>, attention_pp2_kernel<false, 4>},
-        {attention_pp2_kernel<true, 0>, attention_pp2_kernel<true, 2>, attention_pp2_kernel<true, 3>, attention_pp2_kernel<true, 4>}};
-    static const int pp2_default = getenv("MVB_PP2") ? atoi(getenv("MVB_PP2")) : 0;
-    if (a.variant == 4 || attn_env == 4 || (a.variant == 0 && attn_env == 0 && pp2_default)) {
-      const int smem_pp2 = smem_pp + 4096;
-      static bool pp2_set_dev[64] = {};
-      if (!pp2_set_dev[cur_dev & 63]) {
-        cudaError_t e = cudaSuccess;
-        for (int x = 0; x < 2 && e == cudaSuccess; ++x)
-          for (int y = 0; y < 4 && e == cudaSuccess; ++y)
-            e = cudaFuncSetAttribute(reinterpret_cast<const void*>(pp2_kernels[x][y]), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_pp2);
-        if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(attention_pp2_kernel)"; return e; }
-        pp2_set_dev[cur_dev & 63] = true;
-      }
-      const int pp2_idx = pp_idx == 0 ? 0 : pp_idx <= 2 ? 1 : pp_idx == 3 ? 2 : 3;
-      pp2_kernels[p.sum_in_v ? 1 : 0][pp2_idx]<<<grid_pp, 576, smem_pp2, stream>>>(tq, tk0, tv0, tk1, tv1, p);
-      cudaError_t e = cudaGetLastError();
-      if (e != cudaSuccess) *err = "attention_pp2_kernel launch";
-      return e;
-    }
-    if (p.trace != nullptr && p.sum_in_v && pp_idx == 2) {   // traced build of the default instantiation (mvb_debug_attention_trace)
-      const KernelFn traced = attention_pp_kernel<true, 2, true>;
-      cudaError_t e = cudaFuncSetAttribute(reinterpret_cast<const void*>(traced), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_pp);
-      if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(attention_pp_kernel, traced)"; return e; }
-      traced<<<grid_pp, 320, smem_pp, stream>>>(tq, tk0, tv0, tk1, tv1, p);
-    } else {
-      pp_kernels[p.sum_in_v ? 1 : 0][pp_idx]<<<grid_pp, 320, smem_pp, stream>>>(tq, tk0, tv0, tk1, tv1, p);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) *err = "attention_pp_kernel launch";
-    return e;
-  }
-  kernels[p.sum_in_v ? 1 : 0][poly_idx]<<<grid, 320, smem, stream>>>(tq, tk0, tv0, tk1, tv1, p);
+  kernel<<<grid, 384, smem, stream>>>(tq, tk0, tv0, tk1, tv1, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) *err = "attention_kernel launch";
   return e;

@@ -1,4 +1,4 @@
-// FlashAttention-style attention on tcgen05 / TMEM for the spatial layers of the denoiser:
+// FlashAttention-style attention on wgmma for the spatial layers of the denoiser:
 //   * reference-only self attention  (musev/models/attention_processor.py:378-546, K/V = own frame (+) vis-cond frame)
 //   * ReferEmbFuseAttention          (musev/models/attention_processor.py:629-750, K/V = reference tokens (+) own frame)
 //   * text / IP-Adapter cross attention (musev/models/attention_processor.py:176-359; diffusers attention_processor.py
@@ -33,7 +33,7 @@ struct AttnArgs {
   float out_scale;
   int accumulate;         // out += result
   int v_ones_col;         // every V row holds 1.0 at column h*dp + d (needs dp > d): row sums come from the MMA
-  int variant = 0;        // 0: default kernel, 2: split-KV kernel (dp <= 64)
+  int variant = 0;        // accepted for ABI compatibility; every value runs the same kernel
 };
 
 cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char** err);

@@ -22,8 +22,8 @@ static int sm_count() {
   static int n = 0;
   if (!n) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
@@ -108,7 +108,7 @@ int mvb_op_groupnorm_fused(const void* x0, int c0, const void* x1, int c1, int N
                            float eps, const float* gamma, const float* beta, int silu, void* y, float* scratch,
                            unsigned int* barrier_word, unsigned int* arrivals, void* stream) {
   if (!barrier_word || !arrivals) return fail("mvb_op_groupnorm_fused: null barrier word", cudaSuccess);
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaError_t e = gn_fused((cudaStream_t)stream, (const __half*)x0, c0, (const __half*)x1, c1, NF, HW, groups, scratch,

@@ -1,16 +1,16 @@
-// tcgen05 / TMA implicit-GEMM kernel. See conv_gemm.cuh for the math and the reference call sites.
+// wgmma / TMA implicit-GEMM kernel. See conv_gemm.cuh for the math and the reference call sites.
 //
-// CTA = 384 threads, persistent over output tiles (128 rows x block_n columns; 256 rows on a CTA pair):
-//   warp 0   : TMA producer  -- per K block (64 channels of one tap) loads the A box {64, bw, bh, bn}
-//              (out-of-image taps are zero-filled by TMA = conv padding) and the weight tile {64, block_n};
-//              warp-uniform loop, elect.sync picks the issuing lane (a single-thread loop was the mainloop bottleneck)
-//   warp 1   : MMA issuer    -- 4 x tcgen05.mma (K=16 each) per K block into TMEM, same warp-uniform structure
-//   warp 2   : TMEM allocator (512 columns = 2 accumulator stages x up to 256 fp32 columns)
-//   warps 4-11: epilogue     -- two warps per TMEM lane quarter, alternating 32-column chunks: tcgen05.ld accumulator
-//              rows -> bias / time-embedding / residual / GEGLU (four template variants) -> fp16 -> swizzled smem
-//              staging -> TMA store (4-deep staging ring per column half, one named barrier per chunk)
-// Pipelines: smem operand ring (full/empty mbarriers, 160 KB cut into 3..8 stages per launch) and the TMEM double
-// buffer (tmem_full/tmem_empty). kTwoCta: cluster of 2 with cta_group::2 MMAs (M = 256), used for K >= 1280.
+// CTA = 384 threads = 3 warpgroups, persistent over output tiles of 128 rows x BN columns:
+//   warpgroup 0, warp 0 : TMA producer -- per K block (64 channels of one tap) loads the A box {64, bw, bh, bn}
+//                         (out-of-image taps are zero-filled by TMA = conv padding) and the weight tile {64, BN};
+//                         warp-uniform loop, elect.sync picks the issuing lane. The warpgroup gives its registers to
+//                         the other two (setmaxnreg).
+//   warpgroups 1, 2     : MMA + epilogue -- warpgroup g owns accumulator rows [64 g, 64 g + 64) of the tile: 4 x
+//                         wgmma m64nBNk16 per K block, one K block kept in flight; then the accumulator goes through a
+//                         padded fp32 smem slice (128 columns at a time) so that each thread finishes whole 32-column
+//                         runs of one output row: bias / time-embedding / residual / GEGLU (four template variants) ->
+//                         fp16 -> 16-byte global stores.
+// Pipeline: smem operand ring (full/empty mbarriers, 3..8 stages depending on BN).
 #include "conv_gemm.cuh"
 
 #include <dlfcn.h>
@@ -25,18 +25,15 @@
 
 namespace mvb {
 
-static constexpr int kMaxStages = 8;   // ring depth is chosen per launch: as many (16 KB A + block_n x 128 B) stages as fit
+static constexpr int kMaxStages = 8;   // ring depth is chosen per launch: as many (16 KB A + BN x 128 B) stages as fit
 static constexpr int kBlockM = 128;
 static constexpr int kBlockK = 64;
-static constexpr int kMaxBlockN = 256;
 static constexpr int kABytes = kBlockM * kBlockK * 2;        // 16 KB
-static constexpr int kStagingBufBytes = 128 * 64;               // 128 rows x 32 fp16 output columns
-static constexpr int kStagingDepth = 4;                         // staging buffers per column half (3 TMA stores in flight)
-static constexpr int kStagingBytes = 2 * kStagingDepth * kStagingBufBytes;
-static constexpr int kRingBytes = 156 * 1024;                 // operand ring, split into nstages stages
-static constexpr int kBiasBytes = 8 * 128 * 4;                // per epilogue warp: the bias of its (up to) 128 accumulator columns of a tile
-static constexpr int kSmemBytes = kRingBytes + kStagingBytes + kBiasBytes + 1024 /*align*/ + 256 /*barriers*/;
-
+static constexpr int kAccLd = 132;                            // fp32 accumulator slice row stride (conflict-free float4 reads)
+static constexpr int kAccBytes = 2 * 64 * kAccLd * 4;         // per consumer warpgroup: 64 rows x 128 columns
+static constexpr int kBiasBytes = 2 * 256 * 4;                // per consumer warpgroup: the bias of the tile's columns
+static constexpr int kRingBytes = 227 * 1024 - kAccBytes - kBiasBytes - 1024 /*align*/ - 256 /*barriers*/;
+static constexpr int kSmemBytes = kRingBytes + kAccBytes + kBiasBytes + 1024 + 256;
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
 __device__ __forceinline__ float silu(float x) { return __fdividef(x, 1.f + __expf(-x)); }
 // exact-erf GELU (diffusers activations.py:89-102 uses F.gelu default) with erf from Abramowitz-Stegun 7.1.26
@@ -95,88 +92,62 @@ enum : int {
   kEpiGeglu = 3       // fp16 out, value * gelu(gate) on the packed [16 value | 16 gate] column layout
 };
 
-// kTwoCta: the kernel runs as CTA pairs (cluster of 2, tcgen05 cta_group::2): one 256 x block_n tile per pair, each CTA
-// stages its own 128 A rows and HALF of the weight tile, the leader issues M=256 MMAs that read both halves. This cuts
-// the L2->SM operand traffic per FLOP (the measured bound of the 1-CTA kernel, profiles/r01_ncu_full_summary.txt) and
-// halves the MMA issue count.
 struct AMaps {
   CUtensorMap m[4];   // activation views: [0] source 0, [1] skip-concat source / stride-2 phases 1..3
 };
 
-template <bool kTwoCta, int kEpi>
+template <int kEpi, int BN>
 __global__ void __launch_bounds__(384, 1)
 conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmC,
                  const __grid_constant__ ConvGemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + kRingBytes;
-  float* sbias = reinterpret_cast<float*>(staging + kStagingBytes);      // [8 epilogue warps][128]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + kStagingBytes + kBiasBytes);
+  float* sacc = reinterpret_cast<float*>(smem + kRingBytes);               // [2 warpgroups][64][kAccLd]
+  float* sbias = reinterpret_cast<float*>(smem + kRingBytes + kAccBytes);  // [2 warpgroups][256]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes + kAccBytes + kBiasBytes);
   uint64_t* full = bars;                       // [kMaxStages]
   uint64_t* empty = bars + kMaxStages;         // [kMaxStages]
-  uint64_t* tfull = bars + 2 * kMaxStages;     // [2]
-  uint64_t* tempty = bars + 2 * kMaxStages + 2;// [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 4);
   const int nstages = p.nstages;
   const int stage_bytes = p.stage_bytes;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA.m[0]);
     tma_prefetch_desc(&tmA.m[1]);
     tma_prefetch_desc(&tmA.m[2]);
     tma_prefetch_desc(&tmA.m[3]);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmC);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < kMaxStages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], kTwoCta ? 16 : 8);   // every epilogue warp of the pair reports to the leader
+      mbar_init(&empty[s], 8);                 // one arrival per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if (kTwoCta) { tmem_alloc_2sm(tmem_slot, 512); tmem_relinquish_2sm(); }
-    else { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  }
-  tc_fence_before();
-  if (kTwoCta) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
   const int kb_per_tap = p.kb0 + p.kb1;
   const int num_kb = p.ntaps * kb_per_tap;
   const int tiles_m = p.tiles_w * p.tiles_h * p.tiles_n;
-  // work units: a unit is one tile (1-CTA) or a pair of vertically adjacent tiles (2-CTA), n fastest
-  const uint32_t crank = kTwoCta ? cluster_ctarank() : 0u;
-  const int unit0 = kTwoCta ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int unit_stride = kTwoCta ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int num_units = (kTwoCta ? (tiles_m + 1) / 2 : tiles_m) * p.tiles_nn;
-  const int b_rows = kTwoCta ? p.block_n / 2 : p.block_n;      // weight rows staged by this CTA
-  const uint32_t stage_tx = kABytes + (uint32_t)b_rows * kBlockK * 2;
+  const int num_units = tiles_m * p.tiles_nn;   // one unit = one output tile, n fastest
+  const uint32_t stage_tx = kABytes + (uint32_t)BN * kBlockK * 2;
 
-  if (warp == 0) {
-    // TMA producer: warp-uniform loop, one elected lane issues the copies of a stage
-    {
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0) {
+      // TMA producer: warp-uniform loop, one elected lane issues the copies of a stage
       int stage = 0;
       uint32_t phase = 0;
-      for (int unit = unit0; unit < num_units; unit += unit_stride) {
+      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
         const int nt = unit % p.tiles_nn;
-        const int mt = kTwoCta ? 2 * (unit / p.tiles_nn) + (int)crank : unit / p.tiles_nn;
+        const int mt = unit / p.tiles_nn;
         const int tw = mt % p.tiles_w;
         const int th = (mt / p.tiles_w) % p.tiles_h;
-        const int tn = mt / (p.tiles_w * p.tiles_h);   // may run past the last frame in the odd tail of a pair: TMA zero-fills
+        const int tn = mt / (p.tiles_w * p.tiles_h);
         const int w0 = tw * p.bw, h0 = th * p.bh, n0 = tn * p.bn;
         int kcol = 0;                                   // K coordinate of the weight tile
-        const int ncoord = nt * p.block_n + (kTwoCta ? (int)crank * b_rows : 0);
+        const int ncoord = nt * BN;
         for (int tap = 0; tap < p.ntaps; ++tap) {
           const int xw = w0 + p.dx[tap], yh = h0 + p.dy[tap];
           const int src0 = p.tap_src[tap];
@@ -189,16 +160,9 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
             if (elect_one()) {
               uint8_t* sa = smem + stage * stage_bytes;
               uint8_t* sb = sa + kABytes;
-              if (kTwoCta) {
-                // both CTAs' copies complete on the LEADER's barrier, which expects the bytes of the whole pair
-                if (crank == 0) mbar_expect_tx(&full[stage], 2 * stage_tx);
-                tma_load_4d_2sm(sa, tm, &full[stage], c0, xw, yh, n0);
-                tma_load_2d_2sm(sb, &tmB, &full[stage], kcol, ncoord);
-              } else {
-                mbar_expect_tx(&full[stage], stage_tx);
-                tma_load_4d(sa, tm, &full[stage], c0, xw, yh, n0);
-                tma_load_2d(sb, &tmB, &full[stage], kcol, ncoord);
-              }
+              mbar_expect_tx(&full[stage], stage_tx);
+              tma_load_4d(sa, tm, &full[stage], c0, xw, yh, n0);
+              tma_load_2d(sb, &tmB, &full[stage], kcol, ncoord);
             }
             __syncwarp();
             if (++stage == nstages) { stage = 0; phase ^= 1; }
@@ -206,119 +170,122 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
         }
       }
     }
-  } else if (warp == 1) {
-    // MMA issue: the whole warp walks the loop (warp-uniform control flow keeps the operands in uniform registers and
-    // avoids the per-instruction lane-election loops a divergent single-thread region needs); one elected lane issues.
-    if (crank == 0) {
-      const uint32_t idesc = make_idesc_f16(kTwoCta ? 2 * kBlockM : kBlockM, p.block_n, 0, 0);
-      const uint64_t desc0_a = make_desc_k_sw128(smem_u32(smem));
-      const uint64_t desc0_b = make_desc_k_sw128(smem_u32(smem) + kABytes);
-      const uint32_t stage_step = (uint32_t)stage_bytes >> 4;     // descriptor address field counts 16-byte units
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int unit = unit0; unit < num_units; unit += unit_stride) {
-        mbar_wait(&tempty[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)as * kMaxBlockN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint64_t da = desc0_a + (uint64_t)((uint32_t)stage * stage_step);
-          const uint64_t db = desc0_b + (uint64_t)((uint32_t)stage * stage_step);
-          if (elect_one()) {
+    return;
+  }
+
+  setmaxnreg_inc<232>();
+  const int wg = (warp - 4) >> 2;                 // accumulator rows [64 wg, 64 wg + 64)
+  const int t = threadIdx.x - 128 * (1 + wg);     // thread in the warpgroup
+  const int wq = t >> 5;
+  // epilogue mapping: one accumulator row per thread, the two halves of the warpgroup take alternating column chunks
+  const int row_local = t & 63;
+  const int half = t >> 6;
+  const int r = 64 * wg + row_local;
+  float* acc_slice = sacc + wg * 64 * kAccLd;
+  float* wbias = sbias + wg * 256;
+  const bool use_res = (p.res != nullptr) && !p.geglu && !p.out_f32;
+  const int acc_step = p.geglu ? 64 : 32;             // accumulator columns consumed per 32 output columns
+  const uint64_t desc0_a = make_desc_k_sw128(smem_u32(smem) + (uint32_t)wg * 64 * 128);
+  const uint64_t desc0_b = make_desc_k_sw128(smem_u32(smem) + kABytes);
+  const uint32_t stage_step = (uint32_t)stage_bytes >> 4;     // descriptor address field counts 16-byte units
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BN / 2];
+
+  for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+    const int nt = unit % p.tiles_nn;
+    const int mt = unit / p.tiles_nn;
+    const int tw = mt % p.tiles_w;
+    const int th = (mt / p.tiles_w) % p.tiles_h;
+    const int tn = mt / (p.tiles_w * p.tiles_h);
+    const int ncol0 = nt * BN;
+
+    // ---- mainloop: one K block (4 wgmma) in flight while the next is issued
+    int prev_stage = 0;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint64_t da = desc0_a + (uint64_t)((uint32_t)stage * stage_step);
+      const uint64_t db = desc0_b + (uint64_t)((uint32_t)stage * stage_step);
+      wgmma_fence();
+      fence_regs(acc);
 #pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k) {
-              // advance 16 K-elements = 32 bytes inside the 128-byte swizzle atom: +2 in the (addr >> 4) field
-              if (kTwoCta) umma_f16_ss_2sm(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-              else umma_f16_ss(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-            }
-            if (kTwoCta) umma_commit_2sm(&empty[stage], 3); else umma_commit(&empty[stage]);
-          }
-          __syncwarp();
-          if (++stage == nstages) { stage = 0; phase ^= 1; }
-        }
-        if (elect_one()) {
-          if (kTwoCta) umma_commit_2sm(&tfull[as], 3); else umma_commit(&tfull[as]);
-        }
+      for (int k = 0; k < kBlockK / 16; ++k)
+        Wgmma<BN>::ss(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) != 0);
+      wgmma_commit();
+      fence_regs(acc);
+      if (kb > 0) {
+        wgmma_wait<1>();
+        fence_regs(acc);
         __syncwarp();
-        if (++as == 2) { as = 0; aphase ^= 1; }
+        if (lane == 0) mbar_arrive(&empty[prev_stage]);
       }
+      prev_stage = stage;
+      if (++stage == nstages) { stage = 0; phase ^= 1; }
     }
-  } else if (warp >= 4) {
-    // 8 epilogue warps: warp (q, half) owns TMEM lanes [32q, 32q+32) and every other group of output columns.
-    // fp16 results leave through smem staging (64-byte swizzle) + TMA store: full-line coalesced writes, clipped by the
-    // tensor map at the image / matrix edges, so the store path needs no masks.
-    const int q = warp & 3;
-    const int half = (warp - 4) >> 2;
-    const int r = q * 32 + lane;     // accumulator row
-    int as = 0;
-    uint32_t aphase = 0;
-    const bool use_res = (p.res != nullptr) && !p.geglu && !p.out_f32;
-    const bool issuer = (q == 0) && (lane == 0);
-    const int acc_step = p.geglu ? 64 : 32;             // accumulator columns consumed per 32 output columns
-    uint32_t chunk_iter = 0;
-    for (int unit = unit0; unit < num_units; unit += unit_stride) {
-      const int nt = unit % p.tiles_nn;
-      const int mt = kTwoCta ? 2 * (unit / p.tiles_nn) + (int)crank : unit / p.tiles_nn;
-      const int tw = mt % p.tiles_w;
-      const int th = (mt / p.tiles_w) % p.tiles_h;
-      const int tn = mt / (p.tiles_w * p.tiles_h);
-      const int rw = r % p.bw;
-      const int rh = (r / p.bw) % p.bh;
-      const int rn = r / (p.bw * p.bh);
-      const int w = tw * p.bw + rw, h = th * p.bh + rh, n = tn * p.bn + rn;
-      const bool row_ok = (w < p.W) && (h < p.H) && (n < p.NF);
-      const long long m = ((long long)n * p.H + h) * p.W + w;
-      const float* radd = (p.rowadd && row_ok) ? p.rowadd + (long long)(m / p.rows_per_group) * p.ld_rowadd : nullptr;
-      const int ncol0 = nt * p.block_n;
-      const __half* res_row = use_res ? p.res + m * p.ld_res : nullptr;
+    wgmma_wait<0>();
+    fence_regs(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev_stage]);
 
-      uint4 rcur[4] = {}, rnxt[4] = {};
-      auto load_res = [&](int c0, uint4 (&dst)[4]) {
-        if (!use_res || !row_ok) return;
+    // ---- epilogue
+    const int rw = r % p.bw;
+    const int rh = (r / p.bw) % p.bh;
+    const int rn = r / (p.bw * p.bh);
+    const int w = tw * p.bw + rw, h = th * p.bh + rh, n = tn * p.bn + rn;
+    const bool row_ok = (w < p.W) && (h < p.H) && (n < p.NF);
+    const long long m = ((long long)n * p.H + h) * p.W + w;
+    const float* radd = (p.rowadd && row_ok) ? p.rowadd + (long long)(m / p.rows_per_group) * p.ld_rowadd : nullptr;
+    const __half* res_row = use_res ? p.res + m * p.ld_res : nullptr;
+    __half* out_row = reinterpret_cast<__half*>(p.out) + m * p.ldc;
+
+    uint4 rcur[4] = {};
+    auto load_res = [&](int c0, uint4 (&dst)[4]) {
+      if (!use_res || !row_ok) return;
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int nn = ncol0 + c0 + g * 8;
-          if (c0 + g * 8 < p.block_n && nn < p.N) dst[g] = __ldg(reinterpret_cast<const uint4*>(res_row + nn));
-        }
-      };
-      load_res(half * acc_step, rcur);
-      // Bias of this warp's accumulator columns of the tile -> its private smem slice, issued BEFORE the accumulator wait so
-      // that the global-load latency hides behind the mainloop. (ncu on the level-0 N = K = 320 + residual GEMM: 20 % of
-      // all samples were long-scoreboard stalls on the per-chunk bias LDGs, which every thread issued and consumed at once.)
-      float* wbias = sbias + (warp - 4) * 128;
-      if constexpr (kEpi != kEpiGeneric) {
-        __syncwarp();                                   // the previous tile's reads of this slice are done
-#pragma unroll
-        for (int k = 0; k < 128 / 32; ++k) {
-          const int cw = k * 32 + lane;                 // position inside this warp's column list
-          const int cc = half * acc_step + (cw / acc_step) * 2 * acc_step + (cw % acc_step);   // accumulator column in the tile
-          float bv = 0.f;
-          if (p.bias && cc < p.block_n && ncol0 + cc < p.N) bv = __ldg(p.bias + ncol0 + cc);
-          wbias[cw] = bv;
-        }
-        __syncwarp();
+      for (int g = 0; g < 4; ++g) {
+        const int nn = ncol0 + c0 + g * 8;
+        if (c0 + g * 8 < BN && nn < p.N) dst[g] = __ldg(reinterpret_cast<const uint4*>(res_row + nn));
       }
-
-      mbar_wait(&tfull[as], aphase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)as * kMaxBlockN;
-      for (int c0 = half * acc_step; c0 < p.block_n; c0 += 2 * acc_step) {
+    };
+    named_bar_sync(1 + wg, 128);                      // the previous tile's reads of the bias / accumulator slices are done
+    if constexpr (kEpi != kEpiGeneric) {
+      for (int c = t; c < BN; c += 128) wbias[c] = (p.bias && ncol0 + c < p.N) ? __ldg(p.bias + ncol0 + c) : 0.f;
+    }
+#pragma unroll
+    for (int u = 0; u < (BN + 127) / 128; ++u) {
+      if (u > 0) named_bar_sync(1 + wg, 128);         // previous slice consumed
+      // accumulator fragment (rows 16 wq + lane/4 (+8), columns 8 i + 2 (lane%4)) -> fp32 slice, columns [128 u, 128 u + 128)
+#pragma unroll
+      for (int i = 16 * u; i < 16 * u + 16 && i < BN / 8; ++i) {
+        const int rr = 16 * wq + (lane >> 2);
+        const int cc = 8 * (i - 16 * u) + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(acc_slice + rr * kAccLd + cc) = make_float2(acc[4 * i], acc[4 * i + 1]);
+        *reinterpret_cast<float2*>(acc_slice + (rr + 8) * kAccLd + cc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+      }
+      named_bar_sync(1 + wg, 128);
+      const int cend = (128 * u + 128 < BN) ? 128 * u + 128 : BN;
+      for (int c0 = 128 * u + half * acc_step; c0 < cend; c0 += 2 * acc_step) {
+        const float* srow = acc_slice + row_local * kAccLd + (c0 - 128 * u);
+        auto ld32 = [&](const float* src, uint32_t (&v)[32]) {
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            const float4 x = *reinterpret_cast<const float4*>(src + 4 * k);
+            v[4 * k] = __float_as_uint(x.x); v[4 * k + 1] = __float_as_uint(x.y);
+            v[4 * k + 2] = __float_as_uint(x.z); v[4 * k + 3] = __float_as_uint(x.w);
+          }
+        };
+        load_res(c0, rcur);
         if constexpr (kEpi != kEpiGeneric) {
           const int nbase = ncol0 + c0;
           uint32_t v[32], vg[32];
-          tmem_ld32(t_row + c0, v);
-          if constexpr (kEpi == kEpiGeglu) tmem_ld32(t_row + c0 + 32, vg);
-          if constexpr (kEpi == kEpiResidual) load_res(c0 + 2 * acc_step, rnxt);
-          tmem_ld_wait();
-          if (nbase < p.N) {     // uniform per column half: the skipped chunks skip their barrier as a group
-            uint8_t* buf = staging + (half * kStagingDepth + (chunk_iter % kStagingDepth)) * kStagingBufBytes;
+          ld32(srow, v);
+          if constexpr (kEpi == kEpiGeglu) ld32(srow + 32, vg);
+          if (nbase < p.N && row_ok) {
             const F2 alpha2 = f2_make(p.alpha, p.alpha);
-            const float* cbias = wbias + ((c0 - half * acc_step) / (2 * acc_step)) * acc_step;   // this chunk's staged bias
+            const float* cbias = wbias + c0;           // this chunk's bias
+            const int oc = (kEpi == kEpiGeglu) ? nbase / 2 : nbase;
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {      // 8 output columns = one 16-byte staging store
+            for (int g = 0; g < 4; ++g) {      // 8 output columns = one 16-byte store
               uint32_t o[4];
               if constexpr (kEpi == kEpiGeglu) {
                 // output columns 8g..8g+7 of this chunk: accumulator block g/2 (va | vb), value j, gate 16 + j
@@ -327,7 +294,7 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                   const int j = j0 + 2 * e;
-                  // staged bias: this chunk's 64 accumulator columns start at cbias; block g/2 holds [16 value | 16 gate]
+                  // this chunk's 64 accumulator columns start at cbias; block g/2 holds [16 value | 16 gate]
                   const float2 bv = *reinterpret_cast<const float2*>(cbias + (g >> 1) * 32 + j);
                   const float2 bg = *reinterpret_cast<const float2*>(cbias + (g >> 1) * 32 + 16 + j);
                   const F2 val = f2_add(f2_make(__uint_as_float(vv[j]), __uint_as_float(vv[j + 1])), f2_make(bv.x, bv.y));
@@ -363,17 +330,8 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
                   o[e] = *reinterpret_cast<const uint32_t*>(&h2);
                 }
               }
-              *reinterpret_cast<uint4*>(buf + r * 64 + ((g ^ ((r >> 1) & 3)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
+              *reinterpret_cast<uint4*>(out_row + oc + 8 * g) = make_uint4(o[0], o[1], o[2], o[3]);
             }
-            fence_proxy_async();
-            if (issuer) tma_store_wait_read<kStagingDepth - 2>();
-            named_bar_sync(1 + half, 128);
-            if (issuer) {
-              const int oc = (kEpi == kEpiGeglu) ? nbase / 2 : nbase;
-              tma_store_4d(&tmC, buf, oc, tw * p.bw, th * p.bh, tn * p.bn);
-              tma_store_commit();
-            }
-            ++chunk_iter;
           }
         } else {
           // accumulator -> f[32] = the 32 output columns of this chunk, bias / row-add applied
@@ -381,19 +339,19 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
           const int nbase = ncol0 + c0;
           if (p.geglu) {
             uint32_t va[32], vb[32];
-            tmem_ld32(t_row + c0, va);
-            tmem_ld32(t_row + c0 + 32, vb);
-            tmem_ld_wait();
+            ld32(srow, va);
+            ld32(srow + 32, vb);
             // packed columns: [16 value | 16 gate] per 32 accumulator columns
-  #pragma unroll
+#pragma unroll
             for (int hsel = 0; hsel < 2; ++hsel) {
               const uint32_t* v = hsel ? vb : va;
               const int nb = nbase + hsel * 32;
-  #pragma unroll
+#pragma unroll
               for (int j4 = 0; j4 < 4; ++j4) {
                 // bias of 4 value columns and their 4 gate columns (nb is a multiple of 32: 16-byte aligned float4)
-                const float4 bv = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + nb) + j4) : make_float4(0, 0, 0, 0);
-                const float4 bg = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + nb + 16) + j4) : make_float4(0, 0, 0, 0);
+                const bool bok = p.bias && nb < p.N;
+                const float4 bv = bok ? __ldg(reinterpret_cast<const float4*>(p.bias + nb) + j4) : make_float4(0, 0, 0, 0);
+                const float4 bg = bok ? __ldg(reinterpret_cast<const float4*>(p.bias + nb + 16) + j4) : make_float4(0, 0, 0, 0);
                 const int j = j4 * 4;
                 const F2 v01 = f2_add(f2_make(__uint_as_float(v[j]), __uint_as_float(v[j + 1])), f2_make(bv.x, bv.y));
                 const F2 v23 = f2_add(f2_make(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3])), f2_make(bv.z, bv.w));
@@ -405,11 +363,9 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
             }
           } else {
             uint32_t v[32];
-            tmem_ld32(t_row + c0, v);      // block_n is a multiple of 32
-            load_res(c0 + 2 * acc_step, rnxt);
-            tmem_ld_wait();
+            ld32(srow, v);      // BN is a multiple of 32
             if (nbase + 32 <= p.N) {
-  #pragma unroll
+#pragma unroll
               for (int g = 0; g < 8; ++g) {
                 float4 b = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + nbase) + g) : make_float4(0, 0, 0, 0);
                 if (radd) {
@@ -422,7 +378,7 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
                 f[g * 4 + 3] = __uint_as_float(v[g * 4 + 3]) + b.w;
               }
             } else {
-  #pragma unroll
+#pragma unroll
               for (int j = 0; j < 32; ++j) {
                 const int nn = nbase + j;
                 float x = __uint_as_float(v[j]);
@@ -434,9 +390,9 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
               }
             }
           }
-          if (p.out_f32) {
-            if (row_ok) {
-  #pragma unroll
+          if (row_ok) {
+            if (p.out_f32) {
+#pragma unroll
               for (int g = 0; g < 8; ++g) {
                 const int nn = nbase + g * 4;
                 if (nn < p.N) {
@@ -447,57 +403,32 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
                   *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + m * p.ldc + nn) = o4;
                 }
               }
-            }
-          } else {
-            // finish in fp32, round to fp16, stage, store
-            // staging ring of kStagingDepth buffers, ONE barrier per chunk: chunk i is written while stores i-1..i-3 drain
-            // (a TMA store takes ~1 us to release its smem source); before barrier i the issuer makes sure store
-            // i-(depth-1) is done, so after the barrier everybody knows the buffer of chunk i+1 is free
-            uint8_t* buf = staging + (half * kStagingDepth + (chunk_iter % kStagingDepth)) * kStagingBufBytes;
-  #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              __align__(16) __half o[8];
-              const __half* rh8 = reinterpret_cast<const __half*>(&rcur[g]);
-  #pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                float x = f[g * 8 + j];
-                if (!p.geglu) {
-                  x *= p.alpha;
-                  if (use_res) x = fmaf(p.beta, __half2float(rh8[j]), x);
-                  if (p.act == 1) x = silu(x);
-                }
-                o[j] = __float2half_rn(x);
-              }
-              *reinterpret_cast<uint4*>(buf + r * 64 + ((g ^ ((r >> 1) & 3)) << 4)) = *reinterpret_cast<const uint4*>(o);
-            }
-            fence_proxy_async();
-            if (issuer) tma_store_wait_read<kStagingDepth - 2>();
-            named_bar_sync(1 + half, 128);
-            if (issuer) {
+            } else {
+              // finish in fp32, round to fp16, store 8 columns at a time
               const int oc = p.geglu ? nbase / 2 : nbase;
-              tma_store_4d(&tmC, buf, oc, tw * p.bw, th * p.bh, tn * p.bn);
-              tma_store_commit();
+              const int ncols = p.geglu ? p.N / 2 : p.N;
+#pragma unroll
+              for (int g = 0; g < 4; ++g) {
+                if (oc + 8 * g >= ncols) continue;
+                __align__(16) __half o[8];
+                const __half* rh8 = reinterpret_cast<const __half*>(&rcur[g]);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                  float x = f[g * 8 + j];
+                  if (!p.geglu) {
+                    x *= p.alpha;
+                    if (use_res) x = fmaf(p.beta, __half2float(rh8[j]), x);
+                    if (p.act == 1) x = silu(x);
+                  }
+                  o[j] = __float2half_rn(x);
+                }
+                *reinterpret_cast<uint4*>(out_row + oc + 8 * g) = *reinterpret_cast<const uint4*>(o);
+              }
             }
-            ++chunk_iter;
           }
         }
-#pragma unroll
-        for (int g = 0; g < 4; ++g) rcur[g] = rnxt[g];
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (kTwoCta) mbar_arrive_remote(&tempty[as], 0); else mbar_arrive(&tempty[as]);
-      }
-      if (++as == 2) { as = 0; aphase ^= 1; }
     }
-    if (issuer) tma_store_wait_all();   // smem must stay valid until the last bulk store has read it
-  }
-
-  tc_fence_before();
-  if (kTwoCta) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    if (kTwoCta) tmem_dealloc_2sm(tmem_base, 512); else tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -655,11 +586,16 @@ static void pick_box(int W, int H, int NF, int* bw, int* bh, int* bn) {
   }
 }
 
+// tile widths the kernel is instantiated for (the wgmma N of one warpgroup). 160 divides the UNet's 320 / 640 / 1280
+// channels exactly; the GEGLU epilogue needs whole 64-column [value | gate] chunks.
+static const int kBlockNs[4] = {64, 128, 160, 256};
+
 static int pick_block_n(int N, int geglu, long long tiles_m, int num_sms) {
-  // candidates are multiples of 32 (GEGLU chunks) or 16; prefer few padded columns, then fewer waves
+  // prefer few padded columns, then fewer waves
   int best = 0;
   double best_cost = 1e30;
-  for (int bn = 256; bn >= 32; bn -= 32) {
+  for (int i = 3; i >= 0; --i) {
+    const int bn = kBlockNs[i];
     if (geglu && (bn % 64)) continue;
     const int tn = ceil_div(N, bn);
     const long long tiles = tiles_m * tn;
@@ -673,20 +609,20 @@ static int pick_block_n(int N, int geglu, long long tiles_m, int num_sms) {
 
 static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, int nmaps, ConvGemmParams& p,
                                  const __half* wt, long long ktot, const Epilogue& ep, int num_sms, const char** err) {
-  // kernel variants indexed [cta pair][epilogue]
-  typedef void (*KernelFn)(const AMaps, const CUtensorMap, const CUtensorMap, const ConvGemmParams);
-  static const KernelFn kernels[2][4] = {
-      {conv_gemm_kernel<false, kEpiGeneric>, conv_gemm_kernel<false, kEpiPlain>, conv_gemm_kernel<false, kEpiResidual>,
-       conv_gemm_kernel<false, kEpiGeglu>},
-      {conv_gemm_kernel<true, kEpiGeneric>, conv_gemm_kernel<true, kEpiPlain>, conv_gemm_kernel<true, kEpiResidual>,
-       conv_gemm_kernel<true, kEpiGeglu>}};
+  // kernel variants indexed [tile width][epilogue]
+  typedef void (*KernelFn)(const AMaps, const CUtensorMap, const ConvGemmParams);
+#define MVB_GEMM_ROW(BN) \
+  {conv_gemm_kernel<kEpiGeneric, BN>, conv_gemm_kernel<kEpiPlain, BN>, conv_gemm_kernel<kEpiResidual, BN>, \
+   conv_gemm_kernel<kEpiGeglu, BN>}
+  static const KernelFn kernels[4][4] = {MVB_GEMM_ROW(64), MVB_GEMM_ROW(128), MVB_GEMM_ROW(160), MVB_GEMM_ROW(256)};
+#undef MVB_GEMM_ROW
   // the opt-in is per device: key the "already set" state by the current device ordinal
   static bool attr_set_dev[64] = {};
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
   bool& attr_set = attr_set_dev[cur_dev & 63];
   if (!attr_set) {
-    for (int a = 0; a < 2; ++a)
+    for (int a = 0; a < 4; ++a)
       for (int b = 0; b < 4; ++b) {
         cudaError_t e = cudaFuncSetAttribute(reinterpret_cast<const void*>(kernels[a][b]),
                                              cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
@@ -696,51 +632,31 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   }
   const long long tiles_m = (long long)p.tiles_w * p.tiles_h * p.tiles_n;
   p.block_n = pick_block_n(p.N, ep.geglu, tiles_m, num_sms);
+  int bn_idx = 0;
+  while (kBlockNs[bn_idx] != p.block_n) ++bn_idx;
   p.tiles_nn = ceil_div(p.N, p.block_n);
   p.stage_bytes = kABytes + ((p.block_n * kBlockK * 2 + 1023) / 1024) * 1024;   // B tile rounded up to the swizzle period
   p.nstages = kRingBytes / p.stage_bytes;
   if (p.nstages > kMaxStages) p.nstages = kMaxStages;
-  static const int stage_cap = getenv("MVB_STAGES") ? atoi(getenv("MVB_STAGES")) : 0;   // experiment knob
-  if (stage_cap > 1 && p.nstages > stage_cap) p.nstages = stage_cap;
   p.out = ep.out; p.ldc = ep.ldc; p.bias = ep.bias; p.rowadd = ep.rowadd;
   p.rows_per_group = ep.rows_per_group > 0 ? ep.rows_per_group : 1;
   p.ld_rowadd = ep.ld_rowadd; p.res = ep.res; p.ld_res = ep.ld_res; p.alpha = ep.alpha; p.beta = ep.beta;
   p.geglu = ep.geglu; p.act = ep.act; p.out_f32 = ep.out_f32;
   if (ep.out_f32 && (ep.geglu || ep.res)) { *err = "conv_gemm: fp32 output excludes geglu/residual"; return cudaErrorInvalidValue; }
-  // CTA pairs when there is enough work for all 74 pairs (env MVB_TWOCTA=0/1 forces the choice for experiments)
-  static const int twocta_env = getenv("MVB_TWOCTA") ? atoi(getenv("MVB_TWOCTA")) : -1;
-  const long long pair_units = ((tiles_m + 1) / 2) * p.tiles_nn;
-  // pairs pay off when the mainloop dominates (K >= 1280: +5..9 % measured); short-K GEMMs are epilogue-bound and
-  // lose ~15 % to the pair-wide accumulator hand-off
-  bool two_cta = tiles_m >= 2 && pair_units >= (num_sms / 2) && (num_sms % 2 == 0) && ktot >= 1280;
-  if (twocta_env == 0) two_cta = false;
-  if (twocta_env == 1 && tiles_m >= 2 && (num_sms % 2 == 0)) two_cta = true;
+  if ((ep.ldc % (ep.out_f32 ? 4 : 8)) || (reinterpret_cast<uintptr_t>(ep.out) % 16)) {
+    *err = "conv_gemm: the output must be 16-byte aligned with a row stride of whole 16-byte vectors";
+    return cudaErrorInvalidValue;
+  }
   CUtensorMap tmB;
-  if (!encode_map_2d(&tmB, wt, (uint64_t)ktot, (uint64_t)p.N, (uint64_t)ktot, 64u,
-                     (uint32_t)(two_cta ? p.block_n / 2 : p.block_n))) {
+  if (!encode_map_2d(&tmB, wt, (uint64_t)ktot, (uint64_t)p.N, (uint64_t)ktot, 64u, (uint32_t)p.block_n)) {
     *err = "cuTensorMapEncodeTiled(B) failed";
     return cudaErrorInvalidValue;
   }
-  // output tensor map {cols, W, H, NF}: mirrors the A box, 32 columns x 128 pixels, 64-byte swizzle
-  CUtensorMap tmC = tmB;
-  p.tma_store = ep.out_f32 ? 0 : 1;
-  if (p.tma_store) {
-    const int ncols = ep.geglu ? p.N / 2 : p.N;
-    const uint64_t dims[4] = {(uint64_t)ncols, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.NF};
-    const uint64_t st[3] = {(uint64_t)ep.ldc, (uint64_t)ep.ldc * p.W, (uint64_t)ep.ldc * p.W * p.H};
-    const uint32_t box[4] = {32u, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-    if ((ep.ldc % 8) || !encode_map_4d_sw(&tmC, ep.out, dims, st, box, CU_TENSOR_MAP_SWIZZLE_64B)) {
-      *err = "cuTensorMapEncodeTiled(C) failed (output row stride must be a multiple of 8 elements)";
-      return cudaErrorInvalidValue;
-    }
-  }
   const long long num_tiles = tiles_m * p.tiles_nn;
-  int grid = (int)(num_tiles < num_sms ? num_tiles : num_sms);
-  if (two_cta) grid = (int)(2 * (pair_units < num_sms / 2 ? pair_units : num_sms / 2));
+  const int grid = (int)(num_tiles < num_sms ? num_tiles : num_sms);
   // epilogue variant: the fast ones need whole 32-column chunks and the common alpha / beta
-  static const int epi_env = getenv("MVB_EPI") ? atoi(getenv("MVB_EPI")) : -1;   // 0 forces the generic epilogue
   int epi = kEpiGeneric;
-  if (!ep.out_f32 && ep.act == 0 && epi_env != 0) {
+  if (!ep.out_f32 && ep.act == 0) {
     if (ep.geglu) { if (p.N % 64 == 0 && !ep.rowadd) epi = kEpiGeglu; }
     else if (p.N % 32 == 0) {
       if (ep.res && ep.beta == 1.f) epi = kEpiResidual;
@@ -749,26 +665,14 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   }
   static const bool trace = getenv("MVB_TRACE") != nullptr;
   if (trace)
-    fprintf(stderr, "MVB_TRACE gemm M=%lld N=%d K=%lld taps=%d block_n=%d tiles=%lld geglu=%d res=%d f32=%d cta2=%d epi=%d\n",
+    fprintf(stderr, "MVB_TRACE gemm M=%lld N=%d K=%lld taps=%d block_n=%d tiles=%lld geglu=%d res=%d f32=%d epi=%d\n",
             (long long)p.W * p.H * p.NF, p.N, ktot, p.ntaps, p.block_n, num_tiles, p.geglu, p.res != nullptr, p.out_f32,
-            (int)two_cta, epi);
+            epi);
   AMaps am;
   for (int i = 0; i < 4; ++i) am.m[i] = maps[i < nmaps ? i : 0];
   ProfScope prof(stream, KC_GEMM);
-  cudaError_t e;
-  {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(384);
-    cfg.dynamicSmemBytes = kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = two_cta ? 1 : 0;
-    e = cudaLaunchKernelEx(&cfg, kernels[two_cta ? 1 : 0][epi], am, tmB, tmC, p);
-  }
+  kernels[bn_idx][epi]<<<grid, 384, kSmemBytes, stream>>>(am, tmB, p);
+  cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) *err = "conv_gemm_kernel launch";
   return e;
 }

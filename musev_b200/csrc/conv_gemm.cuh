@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution / linear layer on tcgen05 tensor cores (sm_100a).
+// Implicit-GEMM convolution / linear layer on wgmma tensor cores (sm_90a).
 //
 //   out[m, n] = epilogue( sum_{tap, c} A[pixel(m) + tap, c] * Wt[n, tap*Cin + c] )
 //
@@ -41,7 +41,6 @@ struct ConvGemmParams {
   int geglu;  // packed columns are [16 value | 16 gate] chunks: out = value * gelu_erf(gate)
   int act;    // 0 none, 1 SiLU
   int out_f32;  // store fp32 instead of fp16 (embedding tables)
-  int tma_store;  // fp16 output leaves through smem staging + TMA store (coalesced), else direct 16-byte stores
 };
 
 struct ASource {

@@ -117,7 +117,7 @@ Engine::Engine(const mvb_config& cfg, int device, int kind) : cfg_(cfg), device_
   }
   cudaSetDevice(device);
   cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, device);
-  if (num_sms_ <= 0) num_sms_ = 148;
+  if (num_sms_ <= 0) num_sms_ = 132;
   slab_counting_ = true;
   slab_off_ = 0;
   build();                                   // pass 1: count bytes
@@ -533,7 +533,7 @@ int Engine::load_weight(const char* name, const void* ptr, int is_f32, const lon
   } else {
     if (numel != (long long)l.nsrc * l.ksrc) { err_ = std::string("bad shape for ") + name; return MVB_ERR_INVALID; }
     const long long total = (long long)l.rows_dst * l.kdst;
-    const int blocks = (int)((total + 255) / 256 < 148 * 32 ? (total + 255) / 256 : 148 * 32);
+    const int blocks = (int)((total + 255) / 256 < 132 * 32 ? (total + 255) / 256 : 132 * 32);
     if (is_f32)
       pack_matrix_kernel<float><<<blocks, 256>>>(l.dst, l.ld, l.rows_dst, l.kdst, (const float*)ptr, l.nsrc, l.ksrc,
                                                  l.rowmode, l.p0, l.p1, l.colmode, l.cin, l.taps);
@@ -1351,7 +1351,7 @@ bool Engine::run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s) {
     // diffusers Attention with one head of dim cm (attention_processor.py:1166-1250, `residual_connection=True`,
     // `rescale_output_factor=1`): GroupNorm(eps 1e-6) -> q, k, v (with bias) -> softmax(q k^T / sqrt(cm)) v -> to_out + x.
     // The head dim (512) is beyond the flash kernels' tile, and the problem is tiny (one 4096-token frame = 2 x 17 GFLOP),
-    // so it runs as two tcgen05 GEMMs per frame around a row-softmax: S = Q K^T with K as the "weight" operand, O = P V
+    // so it runs as two wgmma GEMMs per frame around a row-softmax: S = Q K^T with K as the "weight" operand, O = P V
     // with V^T as the weight operand (produced directly by a GEMM with the roles of W_v and the tokens swapped). The V
     // bias is added after P V: softmax rows sum to one, so P (V + 1 b^T) = P V + b^T.
     const int HW = Hc * Wc;

@@ -161,7 +161,7 @@ class Engine {
   bool run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
 
   mvb_config cfg_;
-  int device_ = 0, num_sms_ = 148;
+  int device_ = 0, num_sms_ = 132;
   int kind_ = 0;
   float ln_eps13_ = 0.f;       // LayerNorm eps of norm1 / norm3: 0 in the musev blocks (Q1), 1e-5 in the vanilla diffusers blocks
   int heads_ = 8;

@@ -1,5 +1,5 @@
 // HBM-bound kernels (see ops.cuh). Design rules: 128-bit loads/stores on the contiguous channel axis, fp32
-// statistics, grids sized to cover >= 2 waves of the 148 SMs where the tensor is large enough.
+// statistics, grids sized to cover >= 2 waves of the 132 SMs where the tensor is large enough.
 #include "ops.cuh"
 
 #include <math.h>
@@ -144,7 +144,7 @@ cudaError_t gn_stats(cudaStream_t s, const __half* x0, int C0, const __half* x1,
   if ((C0 % 8) || (C1 % 8) || (C % G) || ((C / G) % 2)) return cudaErrorInvalidValue;
   const int threads = 256;
   // ~8 resident blocks per SM (the kernel is latency-bound below that), at least ~32 pixels per block
-  int chunks = (8 * 148) / NF;          // rounded down: one full wave
+  int chunks = (8 * 132) / NF;          // rounded down: one full wave
   const int maxc = HW / 32 > 0 ? HW / 32 : 1;
   if (chunks > maxc) chunks = maxc;
   if (chunks > kGnMaxChunks) chunks = kGnMaxChunks;
@@ -386,7 +386,7 @@ cudaError_t gn_apply(cudaStream_t s, const __half* x0, int C0, const __half* x1,
   // ~4 waves of 6 resident blocks per SM (a 1.5-wave grid leaves half the machine idle for the second half), at least
   // 4 rows per thread so that the per-block prologue stays small
   const int rows_per_pass = threads / (vecs < threads ? vecs : threads) > 0 ? threads / (vecs < threads ? vecs : threads) : 1;
-  int ppb = (int)(((long long)HW * NF + 148 * 24 - 1) / (148 * 24));
+  int ppb = (int)(((long long)HW * NF + 132 * 24 - 1) / (132 * 24));
   if (ppb < 4 * rows_per_pass) ppb = 4 * rows_per_pass;
   if (ppb > HW) ppb = HW;
   int blocks = (HW + ppb - 1) / ppb;
@@ -405,7 +405,7 @@ cudaError_t gn_fused(cudaStream_t s, const __half* x0, int C0, const __half* x1,
   const int C = C0 + C1;
   if ((C0 % 8) || (C1 % 8) || (C % G) || ((C / G) % 2) || fps < 1 || (NF % fps) || G > 64) return cudaErrorInvalidValue;
   // same work decomposition as gn_stats / gn_apply
-  int chunks = (8 * 148) / NF;
+  int chunks = (8 * 132) / NF;
   const int maxc = HW / 32 > 0 ? HW / 32 : 1;
   if (chunks > maxc) chunks = maxc;
   if (chunks > kGnMaxChunks) chunks = kGnMaxChunks;
@@ -416,7 +416,7 @@ cudaError_t gn_fused(cudaStream_t s, const __half* x0, int C0, const __half* x1,
   if (threads < 64) threads = 256;
   const int cols = vecs < threads ? vecs : threads;
   const int rows_per_pass = threads / cols > 0 ? threads / cols : 1;
-  int ppb = (int)(((long long)HW * NF + 148 * 24 - 1) / (148 * 24));
+  int ppb = (int)(((long long)HW * NF + 132 * 24 - 1) / (132 * 24));
   if (ppb < 4 * rows_per_pass) ppb = 4 * rows_per_pass;
   if (ppb > HW) ppb = HW;
   const int pblocks = (HW + ppb - 1) / ppb;
@@ -585,7 +585,7 @@ cudaError_t layernorm(cudaStream_t s, const __half* x, long long M, int C, float
     const int L = C / 40;
     const long long groups = (M + 32 / L - 1) / (32 / L);
     long long blocks = (groups + 7) / 8;
-    if (blocks > 148 * 8) blocks = 148 * 8;   // 8 resident blocks per SM, grid-stride over row groups
+    if (blocks > 132 * 8) blocks = 132 * 8;   // 8 resident blocks per SM, grid-stride over row groups
     if (L == 8) layernorm40_kernel<8><<<(unsigned)blocks, 256, 0, s>>>(x, M, eps, gamma, beta, y);
     else if (L == 16) layernorm40_kernel<16><<<(unsigned)blocks, 256, 0, s>>>(x, M, eps, gamma, beta, y);
     else layernorm40_kernel<32><<<(unsigned)blocks, 256, 0, s>>>(x, M, eps, gamma, beta, y);
@@ -620,7 +620,7 @@ cudaError_t upsample2x(cudaStream_t s, const __half* x, int NF, int H, int W, in
   ProfScope prof(s, KC_OTHER);
   if (C % 8) return cudaErrorInvalidValue;
   const long long total = (long long)NF * 4 * H * W * (C / 8);
-  const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
   upsample2x_kernel<<<blocks, 256, 0, s>>>(x, H, W, C, y, total);
   return cudaGetLastError();
 }
@@ -640,7 +640,7 @@ cudaError_t add_tensors(cudaStream_t s, const __half* a, const __half* b, long l
   ProfScope prof(s, KC_OTHER);
   if (n % 8) return cudaErrorInvalidValue;
   const long long nv = n / 8;
-  const int blocks = (int)((nv + 255) / 256 < 148 * 16 ? (nv + 255) / 256 : 148 * 16);
+  const int blocks = (int)((nv + 255) / 256 < 132 * 16 ? (nv + 255) / 256 : 132 * 16);
   add_kernel<<<blocks, 256, 0, s>>>(a, b, nv, y);
   return cudaGetLastError();
 }
@@ -830,7 +830,7 @@ cudaError_t latent_pointwise(cudaStream_t s, const void* x, int is_f32, int N, i
   ProfScope prof(s, KC_OTHER);
   if (C > 8) return cudaErrorInvalidValue;
   const long long total = (long long)N * HW;
-  const int blocks = (int)((total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8);
+  const int blocks = (int)((total + 255) / 256 < 132 * 8 ? (total + 255) / 256 : 132 * 8);
   if (is_f32) latent_pointwise_kernel<float><<<blocks, 256, 0, s>>>((const float*)x, N, C, HW, w, b, in_scale, y);
   else latent_pointwise_kernel<__half><<<blocks, 256, 0, s>>>((const __half*)x, N, C, HW, w, b, in_scale, y);
   return cudaGetLastError();
@@ -936,8 +936,8 @@ cudaError_t tokens_to_ncthw_affine(cudaStream_t s, const __half* x, int ldx, int
 
 // ------------------------------------------------------------------------------------------------ temporal attention
 // ---- tensor-core version: one warp per (batch, pixel, head); T <= 32 frames padded to a 32x32 score tile.
-// S = Q K^T and O = P V run on mma.sync m16n8k16 (the problem is 32 x 32 x dp per warp: far too small for tcgen05's
-// 128-row tiles), so the kernel is left with its HBM traffic: q,k,v read once, o written once.
+// S = Q K^T and O = P V run on mma.sync m16n8k16 (the problem is 32 x 32 x dp per warp: far too small for wgmma's
+// 64-row warpgroup tiles), so the kernel is left with its HBM traffic: q,k,v read once, o written once.
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], const void* p) {
   const uint32_t a = static_cast<uint32_t>(__cvta_generic_to_shared(p));
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
@@ -1166,7 +1166,7 @@ cudaError_t fuse_cfg_ddim(cudaStream_t s, const float* eps_sum, const float* cou
                           float std_dev, const float* noise, float* eps_out, float* x0_out) {
   ProfScope prof(s, KC_OTHER);
   const long long n = (long long)B * C * T * HW;
-  const int blocks = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+  const int blocks = (int)((n + 255) / 256 < 132 * 8 ? (n + 255) / 256 : 132 * 8);
   if (is_f32)
     fuse_cfg_ddim_kernel<float><<<blocks, 256, 0, s>>>(eps_sum, counter, (const float*)latents_in, (float*)latents_out,
                                                        B, C, T, HW, cfg, guidance, alpha_t, alpha_prev, prediction_type,
@@ -1208,7 +1208,7 @@ cudaError_t fuse_cfg_affine(cudaStream_t s, const float* eps_sum, const float* c
                             float c_e, float c_n, const float* noise, float a_x, float a_e, float* aux_out, float* eps_out) {
   ProfScope prof(s, KC_OTHER);
   const long long n = (long long)B * C * T * HW;
-  const int blocks = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+  const int blocks = (int)((n + 255) / 256 < 132 * 8 ? (n + 255) / 256 : 132 * 8);
   if (is_f32)
     fuse_cfg_affine_kernel<float><<<blocks, 256, 0, s>>>(eps_sum, counter, (const float*)latents_in, (float*)latents_out, n, T,
                                                          HW, cfg, guidance, c_x, c_e, c_n, noise, a_x, a_e, aux_out, eps_out);
@@ -1237,7 +1237,7 @@ cudaError_t accumulate_window(cudaStream_t s, float* eps_sum, int B2, int C, int
                               int is_f32, int Tw, int src_t0, const int* frames_dev, int nframes) {
   ProfScope prof(s, KC_OTHER);
   const long long n = (long long)B2 * C * nframes * HW;
-  const int blocks = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+  const int blocks = (int)((n + 255) / 256 < 132 * 8 ? (n + 255) / 256 : 132 * 8);
   if (is_f32)
     accumulate_window_kernel<float><<<blocks, 256, 0, s>>>(eps_sum, B2, C, T, HW, (const float*)eps_win, Tw, src_t0,
                                                            frames_dev, nframes);

@@ -1,4 +1,4 @@
-"""Visual-Conditioned Parallel-Denoise loop on the B200 engine.
+"""Visual-Conditioned Parallel-Denoise loop on the CUDA engine.
 
 Mirrors the loop body of `MusevControlNetPipeline.__call__` (musev/pipelines/pipeline_controlnet.py:1846-2147):
 per step, every window -> UNet -> accumulate eps; overlap mean; CFG; scheduler.step. What changes:

@@ -7,7 +7,7 @@
   * `ImageProjModel`   the IP-Adapter image projection (`ip_adapter.ip_adapter.ImageProjModel`, a pip dependency of the
                        reference: requirements.txt:2; built at musev/models/ip_adapter_loader.py:89-93, called at
                        musev/pipelines/pipeline_controlnet.py:725,745): Linear(1024 -> 4 x 768) + LayerNorm(768), as one
-                       tcgen05 GEMM + one LayerNorm kernel through the op-level C ABI.
+                       wgmma GEMM + one LayerNorm kernel through the op-level C ABI.
 There is no CPU / PyTorch fallback.
 """
 from __future__ import annotations
@@ -42,12 +42,12 @@ def _lib():
 
 
 class ReferenceNet2D:
-    """B200 engine behind the call surface of `musev.models.referencenet.ReferenceNet2D` (need_block_embs=True,
+    """CUDA engine behind the call surface of `musev.models.referencenet.ReferenceNet2D` (need_block_embs=True,
     need_self_attn_block_embs=False -- the only configuration the released presets use, referencenet_loader.py:109-118)."""
 
     def __init__(self, config: ReferenceNetConfig, device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16):
         if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_100a) device; there is no CPU path")
+            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.cfg = config
         self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
         self.dtype = dtype
@@ -197,7 +197,7 @@ class ImageProjModel:
     def __init__(self, config: ImageProjConfig = ImageProjConfig(), device: Union[str, torch.device] = "cuda",
                  dtype: torch.dtype = torch.float16):
         if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_100a) device; there is no CPU path")
+            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         if config.clip_embeddings_dim % 64 or config.cross_attention_dim % 8:
             raise ValueError("clip_embeddings_dim must be a multiple of 64 and cross_attention_dim a multiple of 8")
         self.cfg = config

@@ -157,7 +157,7 @@ def _contiguous_index_range(idx, name) -> Tuple[int, int]:
 
 
 class UNet3DConditionModel:
-    """B200 engine behind the call surface of the reference model (musev/models/unet_3d_condition.py:179).
+    """CUDA engine behind the call surface of the reference model (musev/models/unet_3d_condition.py:179).
 
     Kept: `forward` signature and return type (:773-803, :1277-1280), `.config`, `.dtype`, `.device`,
     `.ip_adapter_cross_attn`, `.set_skip_temporal_layers` (:1639), `.to()`, `.eval()`, reference state-dict names.
@@ -165,7 +165,7 @@ class UNet3DConditionModel:
 
     def __init__(self, config: UNetConfig, device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16):
         if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_100a) device; there is no CPU path")
+            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.cfg = config
         self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
         self.dtype = dtype

@@ -53,14 +53,14 @@ class DecoderOutput:
 
 
 class AutoencoderKLDecoder:
-    """Decode half of `AutoencoderKL` on the B200 engine: `.decode(z)` (autoencoder_kl.py:275-302) and the pipeline-level
+    """Decode half of `AutoencoderKL` on the CUDA engine: `.decode(z)` (autoencoder_kl.py:275-302) and the pipeline-level
     `.decode_latents(latents)`; `.config.scaling_factor`, `.dtype`, `.device`, reference state-dict names (`decoder.*`,
     `post_quant_conv.*`; encoder / quant_conv entries of a full VAE state dict are ignored)."""
 
     def __init__(self, config: VAEConfig = VAEConfig(), device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16,
                  frames_per_call: int = 4):
         if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_100a) device; there is no CPU path")
+            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.cfg = config
         self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
         self.dtype = dtype

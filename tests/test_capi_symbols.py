@@ -1,4 +1,4 @@
-"""CPU test: the C-ABI library builds (nvcc cross-compiles sm_100a without a GPU), loads, and exports every function
+"""CPU test: the C-ABI library builds (nvcc cross-compiles sm_90a without a GPU), loads, and exports every function
 include/musev_b200.h declares. No compute call is made."""
 import ctypes
 import os
@@ -30,10 +30,10 @@ def test_library_loads_and_exports_every_symbol(built_lib):
     assert lib.mvb_version() >= 1
 
 
-def test_library_is_native_sm100a(built_lib):
+def test_library_is_native_sm90a(built_lib):
     sass = subprocess.run(["cuobjdump", "-sass", built_lib], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM"):          # tcgen05.mma / TMA / tcgen05.ld
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA", "UTMALDG", "SYNCS"):           # wgmma / TMA / mbarrier
         assert mnemonic in sass, mnemonic
 
 

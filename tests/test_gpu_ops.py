@@ -33,7 +33,7 @@ def _pad_heads(x, heads, d, dp, ones=False):
     return o.view(x.shape[0], heads * dp)
 
 
-# the last two shapes have >= 74 tile pairs: they run the CTA-pair (cta_group::2) variant, one with an odd tile count
+# the last two shapes fill more than one wave of tiles on the GPU, one with a ragged last tile
 @pytest.mark.parametrize("M,K,N", [(128, 64, 64), (100, 64, 48), (1000, 320, 320), (4096, 1280, 640), (2, 320, 1280),
                                    (40000, 128, 320), (149 * 128 + 37, 192, 64)])
 def test_linear(ops, M, K, N):
@@ -154,9 +154,7 @@ def test_temporal_attention(ops, B, T, HW, d):
 @pytest.mark.parametrize("variant", [0, 1, 2, 4])
 def test_spatial_attention(ops, NF, T, Nq, d, viscond, ones, variant):
     """Reference-only self attention: K/V = own frame (+) first frame of the batch (attention_processor.py:431-493).
-    variant 0 = default dispatch (ping-pong kernel with P in TMEM for padded head dims <= 64, the one-tile kernel above),
-    1 = the one-tile kernel everywhere, 2 = the split-KV kernel (padded head dims <= 64), 4 = the ping-pong kernel with two
-    threads per query row (padded head dims <= 64)."""
+    Every `variant` value is accepted by the op-level ABI and runs the same kernel; the result must not depend on it."""
     torch.manual_seed(8)
     heads, dp, M = 8, (d + 15) // 16 * 16, NF * Nq
     q, k, v = (torch.randn(M, heads * d, device=dev).half() for _ in range(3))

@@ -20,7 +20,7 @@ for K in (320, 640, 1280, 2560):
         e1.record(); torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / 10
         tiles = (M // 128)
-        waves = -(-tiles // 148)
+        waves = -(-tiles // 132)
         t_tile = ms * 1e3 / waves
         ingest = (128 + N) * K * 2 / 1024
         print(f"[sweep] K={K} N={N}: {ms*1e3:.1f} us  {2.0*M*N*K/ms/1e9:.0f} TF/s  per-tile {t_tile:.2f} us  ingest {ingest:.0f} KB/tile -> {ingest/t_tile*1.024:.0f} MB/s-per-us = GB/s per SM", flush=True)

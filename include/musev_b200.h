@@ -56,7 +56,9 @@ typedef struct mvb_conv_gemm_desc {
   int geglu;
   int act; /* 0 none, 1 SiLU */
   int out_f32; /* store fp32 (no residual / geglu) */
-  int stride2; /* 1: 3x3 stride-2 pad-1 conv of a contiguous [NF,H,W,c0] input (taps ignored) */
+  int stride2; /* 3x3 stride-2 conv of a contiguous [NF,H,W,c0] input with even H, W (taps ignored); 0: off,
+                  1: pad 1 on every side (UNet Downsample2D), 2: pad (0, 1, 0, 1) = right / bottom only
+                  (VAE encoder Downsample2D(padding=0), diffusers models/resnet.py:213-278) */
 } mvb_conv_gemm_desc;
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* desc, void* stream);
@@ -302,6 +304,27 @@ typedef struct mvb_vae_decode_args {
 int mvb_create_vae_decoder(const mvb_config* cfg, int device, mvb_handle** out);
 long long mvb_vae_decode_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args);
 int mvb_vae_decode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * VAE encode, before the denoise loop. Every pipeline call computes `vae.config.scaling_factor * vae.encode(x).latent_dist.mean`
+ * at three call sites of musev/pipelines/pipeline_controlnet.py: the vision-condition image
+ * (`prepare_condition_latents_and_index`, :978-981), the ReferenceNet input image (`get_referencenet_image_vae_emb`,
+ * :809-811) and, for video2video, every frame of the input video (`prepare_latents`, :348-368).
+ * Reference: diffusers `AutoencoderKL.encode` (models/autoencoder_kl.py:256-297: `Encoder.forward`, models/vae.py:133-175:
+ * conv_in, 4 DownEncoderBlock2D whose downsamplers pad (0, 1, 0, 1), UNetMidBlock2D with one single-head attention,
+ * GroupNorm + SiLU + conv_out; then quant_conv and `DiagonalGaussianDistribution`, vae.py:741-785).
+ * The handle is created from an `mvb_config` with in_channels = image channels, out_channels = latent channels, the VAE's
+ * block_out_channels, heads 1, norm_eps 1e-6; weights by the `AutoencoderKL.state_dict()` names `encoder.*` and `quant_conv.*`.
+ * It takes `mvb_vae_decode_args`, whose fields mean, for encode:
+ *   latents / latents_is_f32  the image [N, in_channels, h * 2^(num_blocks-1), w * 2^(num_blocks-1)] in [-1, 1], fp16 / fp32;
+ *   N, h, w                   frames (on the batch axis) and the LATENT size; h * w a multiple of 64 and at most 8192;
+ *   latent_scale              used with postprocess = 1 only (the VAE's scaling_factor);
+ *   out / out_is_f32          the output, fp16 / fp32;
+ *   postprocess               0: the raw moments [N, 2 * out_channels, h, w] (mean, then logvar unclamped: the clamp to
+ *                             [-30, 20] is DiagonalGaussianDistribution's), 1: latent_scale * mean as [N, out_channels, h, w]. */
+int mvb_create_vae_encoder(const mvb_config* cfg, int device, mvb_handle** out);
+long long mvb_vae_encode_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args);
+int mvb_vae_encode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

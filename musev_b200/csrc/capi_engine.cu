@@ -121,6 +121,34 @@ int mvb_vae_decode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspa
   return h->e->vae_decode(*args, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
+int mvb_create_vae_encoder(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out) return MVB_ERR_INVALID;
+  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->norm_num_groups < 1 || cfg->layers_per_block < 1) return MVB_ERR_INVALID;
+  for (int i = 0; i < cfg->num_blocks; ++i) {
+    const int c = cfg->block_out_channels[i];
+    if (c % 64 || c % cfg->norm_num_groups || (c / cfg->norm_num_groups) % 2) return MVB_ERR_INVALID;
+  }
+  // conv_in is an im2col of 9 * in_channels <= 64 columns; conv_out's 2 * out_channels moments fit its 16 padded columns
+  if (cfg->in_channels < 1 || cfg->in_channels > 7 || cfg->out_channels < 1 || cfg->out_channels > 8) return MVB_ERR_INVALID;
+  mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, 4);
+  if (!e) return MVB_ERR_STATE;
+  if (e->error()[0]) { delete e; return MVB_ERR_CUDA; }
+  mvb_handle* h = new (std::nothrow) mvb_handle{e};
+  if (!h) { delete e; return MVB_ERR_STATE; }
+  *out = h;
+  return MVB_OK;
+}
+
+long long mvb_vae_encode_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args) {
+  if (!h || !args) return -1;
+  return h->e->vae_encode_workspace_bytes(*args);
+}
+
+int mvb_vae_encode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes, void* stream) {
+  if (!h || !args) return MVB_ERR_INVALID;
+  return h->e->vae_encode(*args, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 void mvb_destroy(mvb_handle* h) {
   if (!h) return;
   delete h->e;

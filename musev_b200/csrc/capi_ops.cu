@@ -45,7 +45,7 @@ int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   const char* err = nullptr;
   if (d->stride2) {
     cudaError_t e2 = launch_conv_s2((cudaStream_t)stream, (const __half*)d->a0, d->c0, d->W, d->H, d->NF,
-                                    (const __half*)d->weight, d->N, ep, sm_count(), &err);
+                                    (const __half*)d->weight, d->N, ep, sm_count(), &err, d->stride2);
     if (e2 != cudaSuccess) return fail(err, e2);
     return MVB_OK;
   }

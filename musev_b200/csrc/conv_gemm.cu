@@ -710,9 +710,13 @@ cudaError_t launch_conv_gemm(cudaStream_t stream, const ASource& a0, const ASour
 }
 
 cudaError_t launch_conv_s2(cudaStream_t stream, const __half* x, int C, int W, int H, int NF, const __half* wt, int N,
-                           const Epilogue& ep, int num_sms, const char** err) {
+                           const Epilogue& ep, int num_sms, const char** err, int pad_mode) {
   if ((C % 64) || (N % 8) || (W % 2) || (H % 2)) {
     *err = "conv_s2: channels multiple of 64, even H and W";
+    return cudaErrorInvalidValue;
+  }
+  if (pad_mode != 1 && pad_mode != 2) {
+    *err = "conv_s2: pad mode must be 1 (pad 1 on every side) or 2 (pad (0, 1, 0, 1))";
     return cudaErrorInvalidValue;
   }
   const int Wo = W / 2, Ho = H / 2;
@@ -721,14 +725,18 @@ cudaError_t launch_conv_s2(cudaStream_t stream, const __half* x, int C, int W, i
   pick_box(Wo, Ho, NF, &p.bw, &p.bh, &p.bn);
   p.tiles_w = ceil_div(Wo, p.bw); p.tiles_h = ceil_div(Ho, p.bh); p.tiles_n = ceil_div(NF, p.bn);
   p.ntaps = 9;
+  // per kernel offset k: parity phase of the input row / column it reads and the offset within that phase
+  //   pad 1:         input 2y + k - 1: k=0 -> odd phase at y-1; k=1 -> even phase at y; k=2 -> odd phase at y
+  //   pad (0,1,0,1): input 2y + k:     k=0 -> even phase at y;  k=1 -> odd phase at y;  k=2 -> even phase at y+1
+  // out-of-range phase positions (y-1 = -1, y+1 = H/2) are outside the tensor map: TMA fills them with the zero pad
+  static const int8_t kPhase[2][3] = {{1, 0, 1}, {0, 1, 0}}, kOff[2][3] = {{-1, 0, 0}, {0, 0, 1}};
+  const int m = pad_mode - 1;
   for (int ky = 0; ky < 3; ++ky)
     for (int kx = 0; kx < 3; ++kx) {
       const int i = ky * 3 + kx;
-      // input row 2y + ky - 1: ky=0 -> odd phase at y-1; ky=1 -> even phase at y; ky=2 -> odd phase at y
-      const int py = (ky == 1) ? 0 : 1, px = (kx == 1) ? 0 : 1;
-      p.dy[i] = (ky == 0) ? -1 : 0;
-      p.dx[i] = (kx == 0) ? -1 : 0;
-      p.tap_src[i] = (int8_t)(py * 2 + px);
+      p.dy[i] = kOff[m][ky];
+      p.dx[i] = kOff[m][kx];
+      p.tap_src[i] = (int8_t)(kPhase[m][ky] * 2 + kPhase[m][kx]);
     }
   p.kb0 = C / 64; p.kb1 = 0; p.N = N;
   CUtensorMap maps[4];

@@ -69,11 +69,13 @@ cudaError_t launch_conv_gemm(cudaStream_t stream, const ASource& a0, const ASour
                              int ntaps, const int8_t* dy, const int8_t* dx, const __half* wt, int N,
                              const Epilogue& ep, int num_sms, const char** err);
 
-// 3x3 / stride 2 / pad 1 convolution (Downsample2D, diffusers models/resnet.py:247-278) on [NF, H, W, C] with even
-// H, W: the four (row, column) parity phases of the input are four strided TMA views; every tap reads one of them
-// at offset 0 or -1, so the same kernel runs it without an im2col pass. Output image is H/2 x W/2.
+// 3x3 / stride 2 convolution (Downsample2D, diffusers models/resnet.py:213-278) on [NF, H, W, C] with even H, W: the
+// four (row, column) parity phases of the input are four strided TMA views; every tap reads one of them at a fixed
+// offset, so the same kernel runs it without an im2col pass. Output image is H/2 x W/2.
+// pad_mode 1: pad 1 on every side (the UNet's downsamplers, offsets -1 / 0);
+// pad_mode 2: F.pad(x, (0, 1, 0, 1)) then pad 0 (the VAE encoder's `padding=0` downsamplers, offsets 0 / +1).
 cudaError_t launch_conv_s2(cudaStream_t stream, const __half* x, int C, int W, int H, int NF, const __half* wt, int N,
-                           const Epilogue& ep, int num_sms, const char** err);
+                           const Epilogue& ep, int num_sms, const char** err, int pad_mode);
 
 // Encoded tensor maps are memoized process-wide (conv_gemm.cu): hits / misses since the library was loaded.
 void tensor_map_cache_stats(unsigned long long* hits, unsigned long long* misses);

@@ -110,7 +110,7 @@ Engine::Engine(const mvb_config& cfg, int device, int kind) : cfg_(cfg), device_
     // musev/models/unet_2d_blocks.py -> musev BasicTransformerBlock and inherits the eps = 0 quirk (Q1)
     ln_eps13_ = kind_ == 1 ? 1e-5f : 0.f;
   }
-  if (kind_ == 3) {
+  if (kind_ == 3 || kind_ == 4) {
     cfg_.need_transformer_in = cfg_.use_anivv1_cfg = cfg_.resnet_2d_skip_time_act = cfg_.keep_vision_condtion = 0;
     cfg_.need_refer_emb = cfg_.ip_adapter_cross_attn = cfg_.need_t2i_ip_adapter = 0;
     heads_ = 1;
@@ -314,7 +314,57 @@ void Engine::build_refer(const std::string& p, ReferAttn& r, int C) {
 void Engine::build() {
   if (kind_ == 1 || kind_ == 2) build_controlnet();
   else if (kind_ == 3) build_vae();
+  else if (kind_ == 4) build_vae_encoder();
   else build_unet();
+}
+
+// UNetMidBlock2D of either VAE half (diffusers unet_2d_blocks.py; vae.py:113-122 / 236-245): resnet, one single-head
+// attention of dim C (GroupNorm + biased q/k/v/out), resnet; weights under `<p>.mid_block.*`
+void Engine::build_vae_mid(const std::string& p, int C) {
+  const std::string m = p + ".mid_block.";
+  build_resnet(m + "resnets.0", mid_res_[0], C, C, false);
+  vae_attn_norm_ = make_norm(m + "attentions.0.group_norm", C);
+  reg_linear(m + "attentions.0.to_q", vae_q_, C, C, true);
+  reg_linear(m + "attentions.0.to_k", vae_k_, C, C, true);
+  reg_linear(m + "attentions.0.to_v", vae_v_, C, C, true);
+  reg_linear(m + "attentions.0.to_out.0", vae_o_, C, C, true);
+  build_resnet(m + "resnets.1", mid_res_[1], C, C, false);
+}
+
+// AutoencoderKL encoder half: Encoder.__init__ + quant_conv (diffusers models/vae.py:65-131, autoencoder_kl.py:101):
+// conv_in, one DownEncoderBlock2D per entry of block_out_channels (layers_per_block resnets each, a pad-(0,1,0,1) stride-2
+// conv downsampler except on the last), UNetMidBlock2D, GroupNorm + SiLU + conv_out (2 x latent channels), quant_conv.
+// in_channels = image channels, out_channels = latent channels (the decoder's convention mirrored).
+void Engine::build_vae_encoder() {
+  const mvb_config& c = cfg_;
+  const int nb = c.num_blocks, c0 = c.block_out_channels[0], cm = c.block_out_channels[nb - 1];
+  const int zc2 = 2 * c.out_channels;
+  temb_total_ = femb_total_ = 0;
+  conv_in_ = make_mat(c0, 64, true);
+  reg_mat("encoder.conv_in.weight", conv_in_, 0, c0, 0, 0, 0, c0, c.in_channels * 9, 1, c.in_channels, 9);
+  reg_vec("encoder.conv_in.bias", conv_in_.bias, c0, c0);
+  down_.resize(nb);
+  int ch = c0;
+  for (int i = 0; i < nb; ++i) {
+    const int prev = ch;
+    ch = c.block_out_channels[i];
+    Block& b = down_[i];
+    b.layers.resize(c.layers_per_block);
+    const std::string p = "encoder.down_blocks." + std::to_string(i);
+    for (int j = 0; j < c.layers_per_block; ++j)
+      build_resnet(p + ".resnets." + std::to_string(j), b.layers[j].res, j == 0 ? prev : ch, ch, false);
+    b.has_sampler = i != nb - 1;
+    if (b.has_sampler) reg_conv(p + ".downsamplers.0.conv", b.sampler, ch, ch, 9);
+  }
+  build_vae_mid("encoder", cm);
+  norm_out_ = make_norm("encoder.conv_norm_out", cm);
+  conv_out_ = make_mat(16, 9 * cm, true);
+  reg_mat("encoder.conv_out.weight", conv_out_, 0, 16, 0, 0, 0, zc2, 9 * cm, 1, cm, 9);
+  reg_vec("encoder.conv_out.bias", conv_out_.bias, 16, zc2);
+  vae_pq_w_ = slab<float>((size_t)zc2 * zc2);
+  vae_pq_b_ = slab<float>(zc2);
+  reg_vec("quant_conv.weight", vae_pq_w_, zc2 * zc2, zc2 * zc2);
+  reg_vec("quant_conv.bias", vae_pq_b_, zc2, zc2);
 }
 
 // AutoencoderKL decoder half: post_quant_conv + Decoder.__init__ (diffusers models/autoencoder_kl.py:102-104, vae.py:201-263):
@@ -332,13 +382,7 @@ void Engine::build_vae() {
   conv_in_ = make_mat(cm, 64, true);
   reg_mat("decoder.conv_in.weight", conv_in_, 0, cm, 0, 0, 0, cm, zc * 9, 1, zc, 9);
   reg_vec("decoder.conv_in.bias", conv_in_.bias, cm, cm);
-  build_resnet("decoder.mid_block.resnets.0", mid_res_[0], cm, cm, false);
-  vae_attn_norm_ = make_norm("decoder.mid_block.attentions.0.group_norm", cm);
-  reg_linear("decoder.mid_block.attentions.0.to_q", vae_q_, cm, cm, true);
-  reg_linear("decoder.mid_block.attentions.0.to_k", vae_k_, cm, cm, true);
-  reg_linear("decoder.mid_block.attentions.0.to_v", vae_v_, cm, cm, true);
-  reg_linear("decoder.mid_block.attentions.0.to_out.0", vae_o_, cm, cm, true);
-  build_resnet("decoder.mid_block.resnets.1", mid_res_[1], cm, cm, false);
+  build_vae_mid("decoder", cm);
   up_.resize(nb);
   int ch = cm;
   for (int i = 0; i < nb; ++i) {
@@ -930,6 +974,51 @@ struct Engine::Fwd {
     }
     return tok;
   }
+  // UNetMidBlock2D of the VAE (unet_2d_blocks.py: resnet, Attention, resnet; Engine::build_vae_mid), C channels
+  __half* vae_mid(__half* x, int C, int Hd, int Wd) {
+    const int HW = Hd * Wd;
+    const long long M0 = (long long)NF * HW;
+    x = resnet(E->mid_res_[0], x, C, nullptr, 0, Hd, Wd);
+    tap("mid.resnets.0", x, M0, C);
+    {
+      // diffusers Attention with one head of dim C (attention_processor.py:1166-1250, `residual_connection=True`,
+      // `rescale_output_factor=1`): GroupNorm(eps 1e-6) -> q, k, v (with bias) -> softmax(q k^T / sqrt(C)) v -> to_out + x.
+      // The head dim (512) is beyond the flash kernels' tile, and the problem is tiny (one 4096-token frame = 2 x 17 GFLOP),
+      // so it runs as two wgmma GEMMs per frame around a row-softmax: S = Q K^T with K as the "weight" operand, O = P V
+      // with V^T as the weight operand (produced directly by a GEMM with the roles of W_v and the tokens swapped). The V
+      // bias is added after P V: softmax rows sum to one, so P (V + 1 b^T) = P V + b^T.
+      __half* out = alloc_h(M0, C);
+      const size_t mk = mark();
+      __half* nbuf = alloc_h(M0, C);
+      gn(x, C, nullptr, 0, HW, 1, E->cfg_.norm_eps, E->vae_attn_norm_, 0, nbuf);
+      __half* q = alloc_h(M0, C);
+      __half* k = alloc_h(M0, C);
+      { Epilogue ep; ep.out = q; ep.ldc = C; gemm(nbuf, M0, C, E->vae_q_, ep); }
+      { Epilogue ep; ep.out = k; ep.ldc = C; gemm(nbuf, M0, C, E->vae_k_, ep); }
+      __half* vt = alloc_h((long long)NF * C, HW);         // per frame: V^T [C, HW]
+      __half* sc = alloc_h(HW, HW);                         // one frame's scores / probabilities
+      __half* ao = alloc_h(M0, C);
+      for (int n = 0; n < NF; ++n) {
+        Mat tok; tok.w = nbuf + (long long)n * HW * C; tok.N = HW; tok.K = C; tok.bias = nullptr;
+        { Epilogue ep; ep.out = vt + (long long)n * C * HW; ep.ldc = HW; gemm(E->vae_v_.w, C, C, tok, ep, false); }
+        Mat km; km.w = k + (long long)n * HW * C; km.N = HW; km.K = C; km.bias = nullptr;
+        { Epilogue ep; ep.out = sc; ep.ldc = HW; gemm(q + (long long)n * HW * C, HW, C, km, ep, false); }
+        if (!dry && ok) {
+          cudaError_t e = softmax_rows(s, sc, HW, HW, HW, 1.f / sqrtf((float)C));
+          if (e != cudaSuccess) fail("softmax_rows", e);
+        }
+        Mat vm; vm.w = vt + (long long)n * C * HW; vm.N = C; vm.K = HW; vm.bias = E->vae_v_.bias;
+        { Epilogue ep; ep.out = ao + (long long)n * HW * C; ep.ldc = C; gemm(sc, HW, HW, vm, ep, true); }
+      }
+      { Epilogue ep; ep.out = out; ep.ldc = C; ep.res = x; ep.ld_res = C; gemm(ao, M0, C, E->vae_o_, ep); }
+      release(mk);
+      x = out;
+    }
+    tap("mid.attentions.0", x, M0, C);
+    x = resnet(E->mid_res_[1], x, C, nullptr, 0, Hd, Wd);
+    tap("mid", x, M0, C);
+    return x;
+  }
 };
 
 bool Engine::run(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
@@ -1082,7 +1171,7 @@ bool Engine::run(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
       if (!ar.dry && f.ok) {
         Epilogue ep; ep.out = y; ep.ldc = ch; ep.bias = blk.sampler.bias;
         const char* err = nullptr;
-        cudaError_t e = launch_conv_s2(s, x, ch, Wc, Hc, NF, blk.sampler.w, ch, ep, num_sms_, &err);
+        cudaError_t e = launch_conv_s2(s, x, ch, Wc, Hc, NF, blk.sampler.w, ch, ep, num_sms_, &err, 1);
         if (e != cudaSuccess) f.fail(err, e);
       }
       x = y; Hc /= 2; Wc /= 2;
@@ -1271,7 +1360,7 @@ bool Engine::run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_
       if (!ar.dry && f.ok) {
         Epilogue ep; ep.out = y; ep.ldc = ch; ep.bias = blk.sampler.bias;
         const char* err = nullptr;
-        cudaError_t e = launch_conv_s2(s, x, ch, Wc, Hc, NF, blk.sampler.w, ch, ep, num_sms_, &err);
+        cudaError_t e = launch_conv_s2(s, x, ch, Wc, Hc, NF, blk.sampler.w, ch, ep, num_sms_, &err, 1);
         if (e != cudaSuccess) f.fail(err, e);
       }
       x = y; Hc /= 2; Wc /= 2;
@@ -1344,47 +1433,7 @@ bool Engine::run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s) {
     f.release(mk);
   }
   f.tap("conv_in", x, M0, cm);
-  // ---- mid block (unet_2d_blocks.py UNetMidBlock2D: resnet, Attention, resnet)
-  x = f.resnet(mid_res_[0], x, cm, nullptr, 0, Hc, Wc);
-  f.tap("mid.resnets.0", x, M0, cm);
-  {
-    // diffusers Attention with one head of dim cm (attention_processor.py:1166-1250, `residual_connection=True`,
-    // `rescale_output_factor=1`): GroupNorm(eps 1e-6) -> q, k, v (with bias) -> softmax(q k^T / sqrt(cm)) v -> to_out + x.
-    // The head dim (512) is beyond the flash kernels' tile, and the problem is tiny (one 4096-token frame = 2 x 17 GFLOP),
-    // so it runs as two wgmma GEMMs per frame around a row-softmax: S = Q K^T with K as the "weight" operand, O = P V
-    // with V^T as the weight operand (produced directly by a GEMM with the roles of W_v and the tokens swapped). The V
-    // bias is added after P V: softmax rows sum to one, so P (V + 1 b^T) = P V + b^T.
-    const int HW = Hc * Wc;
-    __half* out = f.alloc_h(M0, cm);
-    const size_t mk = f.mark();
-    __half* nbuf = f.alloc_h(M0, cm);
-    f.gn(x, cm, nullptr, 0, HW, 1, c.norm_eps, vae_attn_norm_, 0, nbuf);
-    __half* q = f.alloc_h(M0, cm);
-    __half* k = f.alloc_h(M0, cm);
-    { Epilogue ep; ep.out = q; ep.ldc = cm; f.gemm(nbuf, M0, cm, vae_q_, ep); }
-    { Epilogue ep; ep.out = k; ep.ldc = cm; f.gemm(nbuf, M0, cm, vae_k_, ep); }
-    __half* vt = f.alloc_h((long long)NF * cm, HW);         // per frame: V^T [cm, HW]
-    __half* sc = f.alloc_h(HW, HW);                           // one frame's scores / probabilities
-    __half* ao = f.alloc_h(M0, cm);
-    for (int n = 0; n < NF; ++n) {
-      Mat tok; tok.w = nbuf + (long long)n * HW * cm; tok.N = HW; tok.K = cm; tok.bias = nullptr;
-      { Epilogue ep; ep.out = vt + (long long)n * cm * HW; ep.ldc = HW; f.gemm(vae_v_.w, cm, cm, tok, ep, false); }
-      Mat km; km.w = k + (long long)n * HW * cm; km.N = HW; km.K = cm; km.bias = nullptr;
-      { Epilogue ep; ep.out = sc; ep.ldc = HW; f.gemm(q + (long long)n * HW * cm, HW, cm, km, ep, false); }
-      if (!ar.dry && f.ok) {
-        cudaError_t e = softmax_rows(s, sc, HW, HW, HW, 1.f / sqrtf((float)cm));
-        if (e != cudaSuccess) f.fail("softmax_rows", e);
-      }
-      Mat vm; vm.w = vt + (long long)n * cm * HW; vm.N = cm; vm.K = HW; vm.bias = vae_v_.bias;
-      { Epilogue ep; ep.out = ao + (long long)n * HW * cm; ep.ldc = cm; f.gemm(sc, HW, HW, vm, ep, true); }
-    }
-    { Epilogue ep; ep.out = out; ep.ldc = cm; ep.res = x; ep.ld_res = cm; f.gemm(ao, M0, cm, vae_o_, ep); }
-    f.release(mk);
-    x = out;
-  }
-  f.tap("mid.attentions.0", x, M0, cm);
-  x = f.resnet(mid_res_[1], x, cm, nullptr, 0, Hc, Wc);
-  f.tap("mid", x, M0, cm);
+  x = f.vae_mid(x, cm, Hc, Wc);
   // ---- up blocks (unet_2d_blocks.py UpDecoderBlock2D)
   int ch = cm;
   for (int i = 0; i < nb; ++i) {
@@ -1422,6 +1471,105 @@ bool Engine::run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s) {
     if (e != cudaSuccess) f.fail("vae output", e);
   }
   return f.ok;
+}
+
+static const char* vae_encode_shape_error(const mvb_vae_decode_args& a) {
+  if (a.N < 1 || a.h < 1 || a.w < 1) return "vae encode: bad shape";
+  if (((long long)a.h * a.w) % 64 || (long long)a.h * a.w > 8192)
+    return "vae: latent h*w must be a multiple of 64 and at most 8192 (mid-block attention runs as GEMMs over the tokens)";
+  if (a.postprocess != 0 && a.postprocess != 1) return "vae encode: postprocess must be 0 (moments) or 1 (scaled mean)";
+  return nullptr;
+}
+
+// AutoencoderKL.encode (diffusers models/autoencoder_kl.py:256-297) = Encoder.forward (models/vae.py:133-175) + quant_conv,
+// frames on the batch axis, channels-last activations like run_vae. a.latents is the image [N, C, h*2^(nb-1), w*2^(nb-1)].
+bool Engine::run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s) {
+  const mvb_config& c = cfg_;
+  const int nb = c.num_blocks, c0 = c.block_out_channels[0], cm = c.block_out_channels[nb - 1];
+  const int NF = a.N, zc2 = 2 * c.out_channels, f = 1 << (nb - 1);
+  if (const char* bad = vae_encode_shape_error(a)) { err_ = bad; return false; }
+  mvb_unet_args ua{};
+  ua.B = NF; ua.T = 1; ua.H = a.h * f; ua.W = a.w * f;
+  Fwd fw;
+  fw.E = this; fw.ar = &ar; fw.s = s; fw.dry = ar.dry; fw.a = &ua;
+  fw.B = NF; fw.T = 1; fw.H = ua.H; fw.W = ua.W; fw.NF = NF;
+  fw.heads = 1;
+  fw.skip_temporal = true;
+  fw.temb_table = nullptr; fw.femb_table = nullptr; fw.enc = nullptr; fw.clip = nullptr;
+  if (!ar.dry) taps_.clear();
+  fw.gn_part = fw.alloc_f((long long)NF * (kGnMaxChunks + 1) * c.norm_num_groups * 2);
+  int Hc = ua.H, Wc = ua.W;
+  // ---- conv_in (vae.py:136): im2col of the C-channel image (9 C of 64 columns) + one GEMM
+  __half* x = fw.alloc_h((long long)NF * Hc * Wc, c0);
+  {
+    const long long M = (long long)NF * Hc * Wc;
+    const size_t mk = fw.mark();
+    __half* A = fw.alloc_h(M, 64);
+    if (!ar.dry && fw.ok) {
+      cudaError_t e = im2col_latent(s, a.latents, a.latents_is_f32, NF, c.in_channels, 1, Hc, Wc, A);
+      if (e != cudaSuccess) fw.fail("vae encode input", e);
+    }
+    Epilogue ep; ep.out = x; ep.ldc = c0;
+    fw.gemm(A, M, 64, conv_in_, ep);
+    fw.release(mk);
+  }
+  fw.tap("conv_in", x, (long long)NF * Hc * Wc, c0);
+  // ---- down blocks (unet_2d_blocks.py DownEncoderBlock2D; Downsample2D(padding=0) pads (0, 1, 0, 1), resnet.py:213-278)
+  int ch = c0;
+  for (int i = 0; i < nb; ++i) {
+    Block& blk = down_[i];
+    for (size_t j = 0; j < blk.layers.size(); ++j) {
+      x = fw.resnet(blk.layers[j].res, x, ch, nullptr, 0, Hc, Wc);
+      ch = blk.layers[j].res.C;
+    }
+    if (blk.has_sampler) {
+      __half* y = fw.alloc_h((long long)NF * (Hc / 2) * (Wc / 2), ch);
+      if (!ar.dry && fw.ok) {
+        Epilogue ep; ep.out = y; ep.ldc = ch; ep.bias = blk.sampler.bias;
+        const char* err = nullptr;
+        cudaError_t e = launch_conv_s2(s, x, ch, Wc, Hc, NF, blk.sampler.w, ch, ep, num_sms_, &err, 2);
+        if (e != cudaSuccess) fw.fail(err, e);
+      }
+      x = y; Hc /= 2; Wc /= 2;
+    }
+    fw.tap("down_blocks." + std::to_string(i), x, (long long)NF * Hc * Wc, ch);
+  }
+  x = fw.vae_mid(x, cm, Hc, Wc);
+  // ---- out (vae.py:170-173) + quant_conv (autoencoder_kl.py:284): conv_out stores fp32 so the moments are not rounded
+  // to fp16 before quant_conv
+  const long long M = (long long)NF * Hc * Wc;
+  __half* hn = fw.alloc_h(M, cm);
+  fw.gn(x, cm, nullptr, 0, Hc * Wc, 1, c.norm_eps, norm_out_, 1, hn);
+  float* o32 = fw.alloc_f(M * 16);
+  { Epilogue ep; ep.out = (__half*)o32; ep.ldc = 16; ep.out_f32 = 1; fw.conv3x3(hn, cm, nullptr, 0, NF, Hc, Wc, conv_out_, ep); }
+  if (!ar.dry && fw.ok) {
+    cudaError_t e = vae_moments(s, o32, 16, NF, zc2, Hc * Wc, vae_pq_w_, vae_pq_b_, a.postprocess, a.latent_scale, a.out,
+                                a.out_is_f32);
+    if (e != cudaSuccess) fw.fail("vae encode output", e);
+  }
+  return fw.ok;
+}
+
+long long Engine::vae_encode_workspace_bytes(const mvb_vae_decode_args& a) {
+  if (kind_ != 4) { err_ = "not a VAE encoder handle"; return -1; }
+  Arena ar;
+  ar.dry = true;
+  if (!run_vae_encode(a, ar, nullptr)) return -1;
+  return (long long)ar.peak + 4096;
+}
+
+int Engine::vae_encode(const mvb_vae_decode_args& a, void* workspace, long long wbytes, cudaStream_t stream) {
+  if (kind_ != 4) { err_ = "not a VAE encoder handle"; return MVB_ERR_STATE; }
+  if (!finalized_) { err_ = "mvb_finalize has not been called (or weights are missing)"; return MVB_ERR_STATE; }
+  if (!a.latents || !a.out || !workspace) { err_ = "null pointer argument"; return MVB_ERR_INVALID; }
+  if (const char* bad = vae_encode_shape_error(a)) { err_ = bad; return MVB_ERR_INVALID; }
+  cudaSetDevice(device_);
+  Arena ar;
+  ar.dry = false;
+  ar.base = (char*)workspace;
+  ar.cap = (size_t)wbytes;
+  if (!run_vae_encode(a, ar, stream)) return MVB_ERR_CUDA;
+  return MVB_OK;
 }
 
 long long Engine::vae_workspace_bytes(const mvb_vae_decode_args& a) {

@@ -115,7 +115,7 @@ class Engine {
  public:
   // kind 0: UNet3DConditionModel; kind 1: ControlNet encoder (diffusers models/controlnet.py);
   // kind 2: ReferenceNet2D encoder + mid block (musev/models/referencenet.py);
-  // kind 3: AutoencoderKL decoder (diffusers models/autoencoder_kl.py, vae.py)
+  // kind 3: AutoencoderKL decoder (diffusers models/autoencoder_kl.py, vae.py); kind 4: AutoencoderKL encoder (same files)
   explicit Engine(const mvb_config& cfg, int device, int kind = 0);
   ~Engine();
   int load_weight(const char* name, const void* dev_ptr, int is_f32, const long long* shape, int ndim);
@@ -125,6 +125,8 @@ class Engine {
   int forward(const mvb_unet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long vae_workspace_bytes(const mvb_vae_decode_args& a);
   int vae_decode(const mvb_vae_decode_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
+  long long vae_encode_workspace_bytes(const mvb_vae_decode_args& a);
+  int vae_encode(const mvb_vae_decode_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long controlnet_workspace_bytes(const mvb_controlnet_args& a);
   int controlnet_forward(const mvb_controlnet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   int kind() const { return kind_; }
@@ -139,6 +141,8 @@ class Engine {
   void build_unet();
   void build_controlnet();
   void build_vae();
+  void build_vae_encoder();
+  void build_vae_mid(const std::string& p, int C);
   template <typename T> T* slab(size_t n);
   Mat make_mat(int N, int K, bool bias);
   Norm make_norm(const std::string& p, int C);
@@ -159,6 +163,7 @@ class Engine {
   bool run(const mvb_unet_args& a, Arena& ar, cudaStream_t s);
   bool run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_t s);
   bool run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
+  bool run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
 
   mvb_config cfg_;
   int device_ = 0, num_sms_ = 132;
@@ -197,7 +202,8 @@ class Engine {
   float* fidx_dev_ = nullptr;    // device float[64] scratch for timestep / frame index values
   Mat zero_convs_[MVB_CONTROLNET_MAX_OUT];   // ControlNet: controlnet_down_blocks.* then controlnet_mid_block
   int n_zero_convs_ = 0;
-  // VAE decoder: post_quant_conv (fp32 [C, C] + bias), single-head mid-block attention (q/k/v/out with bias, GroupNorm)
+  // VAE: post_quant_conv (decoder) / quant_conv (encoder), fp32 [C, C] + bias; the mid block's resnets are mid_res_ and
+  // its single-head attention is q/k/v/out with bias after a GroupNorm (build_vae_mid, Fwd::vae_mid)
   float* vae_pq_w_ = nullptr;
   float* vae_pq_b_ = nullptr;
   Norm vae_attn_norm_;

@@ -836,6 +836,41 @@ cudaError_t latent_pointwise(cudaStream_t s, const void* x, int is_f32, int N, i
   return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------------ VAE encoder output
+// quant_conv (AutoencoderKL.encode, diffusers models/autoencoder_kl.py:284): a 1x1 convolution with bias over the C2 = 2 zc
+// moment channels, fp32 throughout. x: conv_out's fp32 tokens [N*HW, ldx]; moments m = W x + b.
+//   postprocess 0: y = m as [N, C2, HW] (mean | logvar; the logvar clamp belongs to DiagonalGaussianDistribution);
+//   postprocess 1: y = scale * mean as [N, C2 / 2, HW], the `scaling_factor * latent_dist.mean` of the pipeline.
+template <typename TOut>
+__global__ void vae_moments_kernel(const float* __restrict__ x, int ldx, int N, int C2, int HW, const float* __restrict__ w,
+                                   const float* __restrict__ b, int postprocess, float scale, TOut* __restrict__ y) {
+  const long long total = (long long)N * HW;
+  const int cout = postprocess ? C2 / 2 : C2;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long n = i / HW, p = i % HW;
+    float v[16];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) v[k] = k < C2 ? x[i * ldx + k] : 0.f;
+    for (int c = 0; c < cout; ++c) {
+      float acc = b[c];
+#pragma unroll
+      for (int k = 0; k < 16; ++k)
+        if (k < C2) acc = fmaf(w[c * C2 + k], v[k], acc);
+      y[(n * cout + c) * HW + p] = (TOut)(postprocess ? scale * acc : acc);
+    }
+  }
+}
+cudaError_t vae_moments(cudaStream_t s, const float* x, int ldx, int N, int C2, int HW, const float* w, const float* b,
+                        int postprocess, float scale, void* y, int is_f32) {
+  ProfScope prof(s, KC_OTHER);
+  if (C2 > 16 || C2 > ldx || (C2 % 2)) return cudaErrorInvalidValue;
+  const long long total = (long long)N * HW;
+  const int blocks = (int)((total + 255) / 256 < 132 * 8 ? (total + 255) / 256 : 132 * 8);
+  if (is_f32) vae_moments_kernel<float><<<blocks, 256, 0, s>>>(x, ldx, N, C2, HW, w, b, postprocess, scale, (float*)y);
+  else vae_moments_kernel<__half><<<blocks, 256, 0, s>>>(x, ldx, N, C2, HW, w, b, postprocess, scale, (__half*)y);
+  return cudaGetLastError();
+}
+
 // In-place row softmax of an fp16 score matrix [M, N] (N % 8 == 0), fp32 statistics: p = exp(scale (s - max)) / sum. One
 // warp per row, the row held in registers for N <= 8192 (three passes over registers, one read + one write of HBM).
 __global__ void __launch_bounds__(256)

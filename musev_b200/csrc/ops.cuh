@@ -54,6 +54,10 @@ cudaError_t latent_pointwise(cudaStream_t s, const void* x, int is_f32, int N, i
 cudaError_t softmax_rows(cudaStream_t s, __half* x, long long M, int N, long long ld, float scale);
 cudaError_t tokens_to_ncthw_affine(cudaStream_t s, const __half* x, int ldx, int B, int C, int T, int HW, void* y, int is_f32,
                                    float alpha, float beta, float lo, float hi);
+// VAE encoder output: quant_conv (C2 x C2 fp32 1x1 conv + bias, C2 <= 16) on conv_out's fp32 tokens [N*HW, ldx] -> NCHW
+// moments [N, C2, HW] (postprocess 0) or scale * mean [N, C2/2, HW] (postprocess 1), fp16 or fp32
+cudaError_t vae_moments(cudaStream_t s, const float* x, int ldx, int N, int C2, int HW, const float* w, const float* b,
+                        int postprocess, float scale, void* y, int is_f32);
 // temporal self-attention over the frame axis (musev/models/temporal_transformer.py:241-273 -> SDPA):
 // qkv [B, T, HW, 3*heads*dp] (q | k | v, head-padded), out [B, T, HW, heads*d].
 cudaError_t temporal_attention(cudaStream_t s, const __half* qkv, int ld, int B, int T, int HW, int heads, int d,

@@ -3,7 +3,8 @@
 Counts 2*M*N*K for every conv / linear the REFERENCE executes and 4*BH*Nq*Nk*d for every attention call -- true,
 unpadded dimensions; the dead CFG recompute (Q3) and the no-op AdaIN (Q2) are excluded. For the baseline shape
 (B=2, T=16+1, 64x64) this reproduces the numbers measured on the reference with hooks: 48.336 TFLOP (`musev`),
-54.153 TFLOP (`musev_referencenet`).
+54.153 TFLOP (`musev_referencenet`). `vae_encoder_flops` / `vae_decoder_flops` count the two VAE halves the same way
+(equal to torch's FlopCounterMode on the oracles, tests/test_vae_encoder_host.py).
 """
 from __future__ import annotations
 
@@ -139,3 +140,84 @@ def unet_forward_flops(cfg: UNetConfig, B: int, T: int, H: int, W: int, n_text: 
     f["gemm"] = f["conv"] + f["linear"]
     f["total"] = f["gemm"] + f["attention"]
     return f
+
+
+def _vae_mid_flops(conv, lin, attn, NF: int, hw: int, cm: int) -> None:
+    """UNetMidBlock2D of the VAE: two resnets and one single-head attention of dim cm over the hw tokens of a frame."""
+    for _ in range(2):
+        conv(NF * hw, cm, cm, 9); conv(NF * hw, cm, cm, 9)
+    for _ in range(4):                       # q, k, v, to_out
+        lin(NF * hw, cm, cm)
+    attn(NF, hw, hw, cm)
+
+
+def _vae_counters():
+    f = {"conv": 0.0, "linear": 0.0, "attention": 0.0}
+
+    def conv(M, cin, cout, taps):
+        f["conv"] += 2.0 * M * cout * cin * taps
+
+    def lin(M, K, N):
+        f["linear"] += 2.0 * M * N * K
+
+    def attn(bh, nq, nk, d):
+        f["attention"] += 4.0 * bh * nq * nk * d
+
+    return f, conv, lin, attn
+
+
+def _vae_total(f: Dict[str, float]) -> Dict[str, float]:
+    f["gemm"] = f["conv"] + f["linear"]
+    f["total"] = f["gemm"] + f["attention"]
+    return f
+
+
+def vae_encoder_flops(cfg, N: int, h: int, w: int) -> Dict[str, float]:
+    """`AutoencoderKL.encode` of N images of (h * 2^(nb-1)) x (w * 2^(nb-1)) pixels (h, w = latent size; VAEConfig `cfg`):
+    Encoder.forward + quant_conv (diffusers models/vae.py:133-175, autoencoder_kl.py:284). SD-1.5 at 64x64 latents
+    (one 512x512 image): 1.117 TFLOP."""
+    f, conv, lin, attn = _vae_counters()
+    boc, nb = cfg.block_out_channels, len(cfg.block_out_channels)
+    H, W = h * 2 ** (nb - 1), w * 2 ** (nb - 1)
+    conv(N * H * W, cfg.in_channels, boc[0], 9)
+    ch = boc[0]
+    for i in range(nb):
+        prev, ch = ch, boc[i]
+        for j in range(cfg.layers_per_block):
+            cin = prev if j == 0 else ch
+            conv(N * H * W, cin, ch, 9); conv(N * H * W, ch, ch, 9)
+            if cin != ch:
+                conv(N * H * W, cin, ch, 1)
+        if i != nb - 1:
+            H, W = H // 2, W // 2
+            conv(N * H * W, ch, ch, 9)
+    _vae_mid_flops(conv, lin, attn, N, H * W, boc[-1])
+    zc2 = 2 * cfg.latent_channels
+    conv(N * H * W, boc[-1], zc2, 9)
+    conv(N * H * W, zc2, zc2, 1)
+    return _vae_total(f)
+
+
+def vae_decoder_flops(cfg, N: int, h: int, w: int) -> Dict[str, float]:
+    """`AutoencoderKL.decode` of N latents of h x w (VAEConfig `cfg`): post_quant_conv + Decoder.forward (diffusers
+    models/autoencoder_kl.py:283, models/vae.py:265-316). SD-1.5 at 64x64 latents (one 512x512 image): 2.515 TFLOP."""
+    f, conv, lin, attn = _vae_counters()
+    boc, nb = cfg.block_out_channels, len(cfg.block_out_channels)
+    zc, cm = cfg.latent_channels, boc[-1]
+    H, W = h, w
+    conv(N * H * W, zc, zc, 1)
+    conv(N * H * W, zc, cm, 9)
+    _vae_mid_flops(conv, lin, attn, N, H * W, cm)
+    ch = cm
+    for i in range(nb):
+        prev, ch = ch, boc[nb - 1 - i]
+        for j in range(cfg.layers_per_block + 1):
+            cin = prev if j == 0 else ch
+            conv(N * H * W, cin, ch, 9); conv(N * H * W, ch, ch, 9)
+            if cin != ch:
+                conv(N * H * W, cin, ch, 1)
+        if i != nb - 1:
+            H, W = H * 2, W * 2
+            conv(N * H * W, ch, ch, 9)
+    conv(N * H * W, boc[0], cfg.out_channels, 9)
+    return _vae_total(f)

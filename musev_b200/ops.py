@@ -41,7 +41,7 @@ def conv_gemm(
     act: int = 0,
     out: Optional[torch.Tensor] = None,
     out_f32: bool = False,
-    stride2: bool = False,
+    stride2: int = 0,                      # 3x3 stride-2 conv: 1 (or True) pad 1 on every side, 2 pad (0, 1, 0, 1)
 ) -> torch.Tensor:
     assert a0.dtype == torch.float16 and weight.dtype == torch.float16 and a0.dim() == 4
     assert a0.stride(3) == 1 and weight.is_contiguous()

@@ -346,11 +346,12 @@ def image_proj_param_shapes(cfg: ImageProjConfig) -> "OrderedDict[str, Tuple[int
     return out
 
 
-# ------------------------------------------------------------------------------------------------ VAE decoder (8f-3)
+# ------------------------------------------------------------------------------------------------ VAE (8f-3)
 @dataclass
 class VAEConfig:
-    """SD-1.5 `vae/config.json` as `AutoencoderKL.__init__` takes it (diffusers models/autoencoder_kl.py:65-118); only the
-    decoder half (+ post_quant_conv) is built."""
+    """SD-1.5 `vae/config.json` as `AutoencoderKL.__init__` takes it (diffusers models/autoencoder_kl.py:65-118). Both halves
+    are built: the encoder (+ quant_conv, `vae_encoder_param_shapes`) and the decoder (+ post_quant_conv,
+    `vae_decoder_param_shapes`)."""
     in_channels: int = 3
     out_channels: int = 3
     latent_channels: int = 4
@@ -360,44 +361,49 @@ class VAEConfig:
     scaling_factor: float = 0.18215
 
 
+def _vae_resnet(out, p, cin, c):
+    out[f"{p}.norm1.weight"] = (cin,)
+    out[f"{p}.norm1.bias"] = (cin,)
+    out[f"{p}.conv1.weight"] = (c, cin, 3, 3)
+    out[f"{p}.conv1.bias"] = (c,)
+    out[f"{p}.norm2.weight"] = (c,)
+    out[f"{p}.norm2.bias"] = (c,)
+    out[f"{p}.conv2.weight"] = (c, c, 3, 3)
+    out[f"{p}.conv2.bias"] = (c,)
+    if cin != c:
+        out[f"{p}.conv_shortcut.weight"] = (c, cin, 1, 1)
+        out[f"{p}.conv_shortcut.bias"] = (c,)
+
+
+def _vae_mid(out, p, cm):
+    """UNetMidBlock2D of either half: resnet, single-head Attention (GroupNorm, biased q/k/v/out), resnet."""
+    _vae_resnet(out, f"{p}.mid_block.resnets.0", cm, cm)
+    a = f"{p}.mid_block.attentions.0"
+    out[f"{a}.group_norm.weight"] = (cm,)
+    out[f"{a}.group_norm.bias"] = (cm,)
+    for n in ("to_q", "to_k", "to_v", "to_out.0"):
+        out[f"{a}.{n}.weight"] = (cm, cm)
+        out[f"{a}.{n}.bias"] = (cm,)
+    _vae_resnet(out, f"{p}.mid_block.resnets.1", cm, cm)
+
+
 def vae_decoder_param_shapes(cfg: VAEConfig) -> "OrderedDict[str, Tuple[int, ...]]":
     """name -> shape of the `post_quant_conv.*` and `decoder.*` entries of the reference `AutoencoderKL.state_dict()`
     (diffusers models/vae.py:201-263; 138 tensors at SD-1.5 size)."""
     out: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
     boc = cfg.block_out_channels
     zc, cm = cfg.latent_channels, boc[-1]
-
-    def resnet(p, cin, c):
-        out[f"{p}.norm1.weight"] = (cin,)
-        out[f"{p}.norm1.bias"] = (cin,)
-        out[f"{p}.conv1.weight"] = (c, cin, 3, 3)
-        out[f"{p}.conv1.bias"] = (c,)
-        out[f"{p}.norm2.weight"] = (c,)
-        out[f"{p}.norm2.bias"] = (c,)
-        out[f"{p}.conv2.weight"] = (c, c, 3, 3)
-        out[f"{p}.conv2.bias"] = (c,)
-        if cin != c:
-            out[f"{p}.conv_shortcut.weight"] = (c, cin, 1, 1)
-            out[f"{p}.conv_shortcut.bias"] = (c,)
-
     out["post_quant_conv.weight"] = (zc, zc, 1, 1)
     out["post_quant_conv.bias"] = (zc,)
     out["decoder.conv_in.weight"] = (cm, zc, 3, 3)
     out["decoder.conv_in.bias"] = (cm,)
-    resnet("decoder.mid_block.resnets.0", cm, cm)
-    a = "decoder.mid_block.attentions.0"
-    out[f"{a}.group_norm.weight"] = (cm,)
-    out[f"{a}.group_norm.bias"] = (cm,)
-    for n in ("to_q", "to_k", "to_v", "to_out.0"):
-        out[f"{a}.{n}.weight"] = (cm, cm)
-        out[f"{a}.{n}.bias"] = (cm,)
-    resnet("decoder.mid_block.resnets.1", cm, cm)
+    _vae_mid(out, "decoder", cm)
     ch = cm
     nb = len(boc)
     for i in range(nb):
         prev, ch = ch, boc[nb - 1 - i]
         for j in range(cfg.layers_per_block + 1):
-            resnet(f"decoder.up_blocks.{i}.resnets.{j}", prev if j == 0 else ch, ch)
+            _vae_resnet(out, f"decoder.up_blocks.{i}.resnets.{j}", prev if j == 0 else ch, ch)
         if i != nb - 1:
             out[f"decoder.up_blocks.{i}.upsamplers.0.conv.weight"] = (ch, ch, 3, 3)
             out[f"decoder.up_blocks.{i}.upsamplers.0.conv.bias"] = (ch,)
@@ -405,4 +411,31 @@ def vae_decoder_param_shapes(cfg: VAEConfig) -> "OrderedDict[str, Tuple[int, ...
     out["decoder.conv_norm_out.bias"] = (boc[0],)
     out["decoder.conv_out.weight"] = (cfg.out_channels, boc[0], 3, 3)
     out["decoder.conv_out.bias"] = (cfg.out_channels,)
+    return out
+
+
+def vae_encoder_param_shapes(cfg: VAEConfig) -> "OrderedDict[str, Tuple[int, ...]]":
+    """name -> shape of the `encoder.*` and `quant_conv.*` entries of the reference `AutoencoderKL.state_dict()`
+    (diffusers models/vae.py:65-131, autoencoder_kl.py:101; 108 tensors at SD-1.5 size)."""
+    out: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    boc = cfg.block_out_channels
+    zc2, cm = 2 * cfg.latent_channels, boc[-1]
+    out["encoder.conv_in.weight"] = (boc[0], cfg.in_channels, 3, 3)
+    out["encoder.conv_in.bias"] = (boc[0],)
+    ch = boc[0]
+    nb = len(boc)
+    for i in range(nb):
+        prev, ch = ch, boc[i]
+        for j in range(cfg.layers_per_block):
+            _vae_resnet(out, f"encoder.down_blocks.{i}.resnets.{j}", prev if j == 0 else ch, ch)
+        if i != nb - 1:
+            out[f"encoder.down_blocks.{i}.downsamplers.0.conv.weight"] = (ch, ch, 3, 3)
+            out[f"encoder.down_blocks.{i}.downsamplers.0.conv.bias"] = (ch,)
+    _vae_mid(out, "encoder", cm)
+    out["encoder.conv_norm_out.weight"] = (cm,)
+    out["encoder.conv_norm_out.bias"] = (cm,)
+    out["encoder.conv_out.weight"] = (zc2, cm, 3, 3)
+    out["encoder.conv_out.bias"] = (zc2,)
+    out["quant_conv.weight"] = (zc2, zc2, 1, 1)
+    out["quant_conv.bias"] = (zc2,)
     return out

@@ -16,7 +16,7 @@ import torch
 
 from .schema import (ControlNetConfig, ImageProjConfig, ReferenceNetConfig, UNetConfig, VAEConfig, controlnet_param_shapes,
                      image_proj_param_shapes, refer_emb_shapes, referencenet_param_shapes, unet_param_shapes,
-                     vae_decoder_param_shapes)
+                     vae_decoder_param_shapes, vae_encoder_param_shapes)
 
 _BRANCH_OUT = ("conv2.weight", "proj_out.weight", "to_out.0.weight", "ff.net.2.weight", "conv4.3.weight")
 # the ControlNet's zero-initialised convolutions (controlnet.py:97-99,425-444) are drawn non-zero for the same reason
@@ -30,7 +30,8 @@ def _gen(seed: int, name: str) -> torch.Generator:
 
 
 def make_state_dict(cfg, seed: int = 0, dtype: torch.dtype = torch.float32) -> "OrderedDict[str, torch.Tensor]":
-    """Seeded weights for a `UNetConfig` (denoiser) or a `ControlNetConfig` (ControlNet encoder)."""
+    """Seeded weights for a `UNetConfig` (denoiser), a `ControlNetConfig` (ControlNet encoder), a `ReferenceNetConfig`, an
+    `ImageProjConfig` or a `VAEConfig` (the full `AutoencoderKL`: encoder + quant_conv, decoder + post_quant_conv)."""
     sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
     if isinstance(cfg, ReferenceNetConfig):
         shapes = referencenet_param_shapes(cfg)
@@ -39,7 +40,7 @@ def make_state_dict(cfg, seed: int = 0, dtype: torch.dtype = torch.float32) -> "
     elif isinstance(cfg, ImageProjConfig):
         shapes = image_proj_param_shapes(cfg)
     elif isinstance(cfg, VAEConfig):
-        shapes = vae_decoder_param_shapes(cfg)
+        shapes = OrderedDict(list(vae_encoder_param_shapes(cfg).items()) + list(vae_decoder_param_shapes(cfg).items()))
     else:
         shapes = unet_param_shapes(cfg)
     for name, shape in shapes.items():
@@ -115,3 +116,8 @@ def make_referencenet_inputs(cfg: ReferenceNetConfig, batch: int, n_ref: int, h:
         "encoder_hidden_states": r("rn_tokens", batch * n_ref, n_tokens, cfg.cross_attention_dim),
         "num_frames": n_ref,
     }
+
+
+def make_vae_images(frames: int, H: int, W: int, seed: int = 2469, channels: int = 3) -> torch.Tensor:
+    """Seeded images in [-1, 1], what `prepare_image` hands to `vae.encode`: [frames, channels, H, W] fp32."""
+    return torch.rand(frames, channels, H, W, generator=torch.Generator().manual_seed(seed)) * 2 - 1

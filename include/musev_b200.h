@@ -232,6 +232,22 @@ const char* mvb_handle_error(mvb_handle* h);
 /* Debug aid for bisecting parity: layer outputs of the last forward, fp16 [rows, C] inside the caller's workspace. */
 int mvb_debug_num_taps(mvb_handle* h);
 int mvb_debug_tap(mvb_handle* h, int i, char* name, int name_cap, const void** ptr, long long* rows, int* C);
+/* LoRA merge into the packed weights of a UNet handle, after mvb_finalize. Replaces the in-place
+ * `curr_layer.weight.data += adding_weight` of musev/utils/model_util.py:update_pipeline_lora_model (:153-262) and, with
+ * subtract = 1, the `layer.weight.data -= added_weight` of unload_lora (:468-475). For each i:
+ *   up[i].name            the target, a reference weight name (`down_blocks.0.attentions.0.proj_in.weight`); a target may
+ *                         appear once per call;
+ *   up[i] / down[i]       the kohya `lora_up` [N, r] / `lora_down` [r, K] factors on the handle's device, fp16 or fp32;
+ *                         4-D for convolutions: up [N, r, 1, 1], down [r, Cin, kh, kw] (1x1 or the conv's own kernel);
+ *                         1 <= r <= 256; down[i].name is not read;
+ *   scale[i]              strength * alpha / r (1 without alpha) times the 0 / 1 block weight of LORA_BLOCK_WEIGHT_MAP.
+ * delta16 = fp16(scale * (up @ down)) with the rank summed in a fixed order, W16 = fp16(W16 +- delta16): an unload repeats
+ * the apply's delta16 bit for bit. Every entry is validated before anything is written; synchronous. */
+int mvb_unet_merge_lora(mvb_handle* h, const mvb_named_tensor* up, const mvb_named_tensor* down, const float* scale, int n,
+                        int subtract);
+/* Debug aid (no reference equivalent): copies the packed matrix / convolution weight `name` back into the reference layout
+ * as fp16 (`dst_f16`: device buffer of the reference tensor's element count). Synchronous. */
+int mvb_debug_read_weight(mvb_handle* h, const char* name, void* dst_f16);
 
 
 /* ---------------------------------------------------------------------------------------------------------

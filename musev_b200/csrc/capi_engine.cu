@@ -166,6 +166,17 @@ int mvb_load_weights(mvb_handle* h, const mvb_named_tensor* tensors, int n) {
 }
 
 int mvb_finalize(mvb_handle* h) { return h ? h->e->finalize() : MVB_ERR_INVALID; }
+
+int mvb_unet_merge_lora(mvb_handle* h, const mvb_named_tensor* up, const mvb_named_tensor* down, const float* scale, int n,
+                        int subtract) {
+  if (!h) return MVB_ERR_INVALID;
+  return h->e->merge_lora(up, down, scale, n, subtract);
+}
+
+int mvb_debug_read_weight(mvb_handle* h, const char* name, void* dst_f16) {
+  if (!h) return MVB_ERR_INVALID;
+  return h->e->read_weight(name, dst_f16);
+}
 int mvb_num_params(mvb_handle* h) { return h ? h->e->num_params() : 0; }
 
 long long mvb_workspace_bytes(mvb_handle* h, const mvb_unet_args* args) {

@@ -121,6 +121,11 @@ class Engine {
   int load_weight(const char* name, const void* dev_ptr, int is_f32, const long long* shape, int ndim);
   int load_weights(const mvb_named_tensor* tensors, int n);
   int finalize();
+  // LoRA merge into the packed weights (csrc/lora.cu; musev/utils/model_util.py:108-262,468-475). up[i].name names the
+  // target by its reference weight name; subtract = 1 removes a previous merge. UNet handles only, after finalize.
+  int merge_lora(const mvb_named_tensor* up, const mvb_named_tensor* down, const float* scale, int n, int subtract);
+  // Packed matrix / convolution weight -> fp16 in the reference layout (device pointer, nsrc x ksrc elements)
+  int read_weight(const char* name, void* dst_f16);
   long long workspace_bytes(const mvb_unet_args& a);
   int forward(const mvb_unet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long vae_workspace_bytes(const mvb_vae_decode_args& a);

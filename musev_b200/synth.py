@@ -118,6 +118,67 @@ def make_referencenet_inputs(cfg: ReferenceNetConfig, batch: int, n_ref: int, h:
     }
 
 
+def make_lora_state_dict(cfg: UNetConfig, targets, rank: int = 4, seed: int = 0, amp: float = 0.5,
+                         no_alpha=(), f32=(), text_targets=(), prefix: str = "lora_unet") -> "OrderedDict[str, torch.Tensor]":
+    """A seeded kohya-style LoRA on the UNet weights `targets` (reference names; matrices, 1x1 and kxk convolutions).
+
+    Every factor is drawn from its own generator (seed, kohya key), like `make_state_dict`. Factors are fp16 unless the
+    target is in `f32`; `alpha` = rank / 2 except for targets in `no_alpha`, which get no `.alpha` key. kxk convolutions
+    get the LoCon factorisation up [N, r, 1, 1], down [r, Cin, kh, kw]. `amp` sets |scale * up @ down| relative to the
+    weight's own draw. `text_targets` is a list of (kohya name after `lora_te_`, out, in) linear layers of a text encoder."""
+    shapes = unet_param_shapes(cfg)
+    sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+
+    def add(mod, up_shape, down_shape, fan_in, dtype, alpha):
+        g = _gen(seed, mod + ".lora_down.weight")
+        down = torch.randn(down_shape, generator=g) / fan_in ** 0.5
+        up = torch.randn(up_shape, generator=_gen(seed, mod + ".lora_up.weight")) * (amp / rank ** 0.5)
+        if alpha:
+            up = up * 2.0      # alpha / rank = 1 / 2
+        sd[mod + ".lora_down.weight"] = down.to(dtype)
+        sd[mod + ".lora_up.weight"] = up.to(dtype)
+        if alpha:
+            sd[mod + ".alpha"] = torch.tensor(rank / 2.0, dtype=dtype)
+
+    for name in targets:
+        shape = shapes[name]
+        if len(shape) not in (2, 4):
+            raise ValueError(f"{name}: LoRA factors exist for 2-D and 4-D weights only, not {shape}")
+        mod = f"{prefix}_" + name[:-7].replace(".", "_")
+        dtype = torch.float32 if name in f32 else torch.float16
+        fan_in = 1
+        for s in shape[1:]:
+            fan_in *= s
+        if len(shape) == 2:
+            add(mod, (shape[0], rank), (rank, shape[1]), fan_in, dtype, name not in no_alpha)
+        else:
+            add(mod, (shape[0], rank, 1, 1), (rank,) + tuple(shape[1:]), fan_in, dtype, name not in no_alpha)
+    for mod, n_out, n_in in text_targets:
+        add("lora_te_" + mod, (n_out, rank), (rank, n_in), n_in, torch.float16, True)
+    return sd
+
+
+def make_text_encoder(width: int = 64, seed: int = 0) -> torch.nn.Module:
+    """A stand-in for `pipeline.text_encoder` with CLIP's module path to one attention: `text_model.encoder.layers.0.
+    self_attn.{q,k,v,out}_proj`, fp16 seeded linears. The LoRA key of its k_proj is `lora_te_text_model_encoder_layers_0_
+    self_attn_k_proj`."""
+    nn = torch.nn
+    attn = nn.Module()
+    for p in ("q_proj", "k_proj", "v_proj", "out_proj"):
+        lin = nn.Linear(width, width, bias=False)
+        lin.weight.data = torch.randn(width, width, generator=_gen(seed, "te." + p)).div(width ** 0.5).half()
+        setattr(attn, p, lin)
+    layer = nn.Module()
+    layer.self_attn = attn
+    enc = nn.Module()
+    enc.layers = nn.ModuleList([layer])
+    tm = nn.Module()
+    tm.encoder = enc
+    root = nn.Module()
+    root.text_model = tm
+    return root
+
+
 def make_vae_images(frames: int, H: int, W: int, seed: int = 2469, channels: int = 3) -> torch.Tensor:
     """Seeded images in [-1, 1], what `prepare_image` hands to `vae.encode`: [frames, channels, H, W] fp32."""
     return torch.rand(frames, channels, H, W, generator=torch.Generator().manual_seed(seed)) * 2 - 1

@@ -123,6 +123,11 @@ def _lib():
         l.mvb_debug_tap.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.POINTER(C.c_void_p),
                                     C.POINTER(C.c_longlong), C.POINTER(C.c_int)]
         l.mvb_debug_tap.restype = C.c_int
+        l.mvb_unet_merge_lora.argtypes = [C.c_void_p, C.POINTER(MvbNamedTensor), C.POINTER(MvbNamedTensor),
+                                          C.POINTER(C.c_float), C.c_int, C.c_int]
+        l.mvb_unet_merge_lora.restype = C.c_int
+        l.mvb_debug_read_weight.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
+        l.mvb_debug_read_weight.restype = C.c_int
         _declared = True
     return l
 
@@ -134,6 +139,14 @@ class UNet3DConditionOutput:
 
     def __getitem__(self, i):
         return (self.sample,)[i]
+
+
+def _named(name: str, t: torch.Tensor) -> MvbNamedTensor:
+    e = MvbNamedTensor()
+    e.name, e.device_ptr, e.is_f32, e.ndim = name.encode(), t.data_ptr(), _is_f32(t), t.dim()
+    for i, v in enumerate(t.shape):
+        e.shape[i] = v
+    return e
 
 
 def _is_f32(t: torch.Tensor) -> int:
@@ -385,6 +398,38 @@ class UNet3DConditionModel:
         return UNet3DConditionOutput(sample=out)
 
     __call__ = forward
+
+    # ------------------------------------------------------------------ LoRA (musev_b200/lora.py is the public surface)
+    def _merge_lora(self, targets: Sequence[str], ups: Sequence[torch.Tensor], downs: Sequence[torch.Tensor],
+                    scales: Sequence[float], subtract: bool = False) -> None:
+        """W16 = fp16(W16 +- fp16(scale * (up @ down))) for every target (reference weight names), one `mvb_unet_merge_lora`
+        call. The factors must be contiguous fp16 / fp32 tensors on this model's device."""
+        n = len(targets)
+        if not (len(ups) == len(downs) == len(scales) == n):
+            raise ValueError("targets, ups, downs and scales differ in length")
+        for t in list(ups) + list(downs):
+            if t.device != self.device or not t.is_contiguous():
+                raise ValueError(f"LoRA factors must be contiguous tensors on {self.device}")
+        up_arr = (MvbNamedTensor * max(n, 1))(*[_named(nm, u) for nm, u in zip(targets, ups)])
+        down_arr = (MvbNamedTensor * max(n, 1))(*[_named(nm, d) for nm, d in zip(targets, downs)])
+        sc = (C.c_float * max(n, 1))(*[float(s) for s in scales])
+        torch.cuda.current_stream(self.device).synchronize()      # the factors may still be in flight
+        l = _lib()
+        rc = l.mvb_unet_merge_lora(self._h, up_arr, down_arr, sc, n, int(bool(subtract)))
+        if rc != 0:
+            raise _capi.MvbError(f"mvb_unet_merge_lora ({rc}): {l.mvb_handle_error(self._h).decode()}")
+
+    def debug_weight(self, name: str) -> torch.Tensor:
+        """The packed matrix / convolution weight `name` read back into its reference shape, fp16 on the device."""
+        shape = unet_param_shapes(self.cfg).get(name)
+        if shape is None or len(shape) < 2:
+            raise ValueError(f"{name} is not a matrix or convolution weight of this UNet")
+        out = torch.empty(shape, dtype=torch.float16, device=self.device)
+        l = _lib()
+        rc = l.mvb_debug_read_weight(self._h, name.encode(), out.data_ptr())
+        if rc != 0:
+            raise _capi.MvbError(f"mvb_debug_read_weight ({rc}): {l.mvb_handle_error(self._h).decode()}")
+        return out
 
     # ------------------------------------------------------------------ debug
     def debug_taps(self) -> Dict[str, torch.Tensor]:

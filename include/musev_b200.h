@@ -63,6 +63,13 @@ typedef struct mvb_conv_gemm_desc {
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* desc, void* stream);
 
+/* Small-channel 3x3 convolution (pad 1, stride 1 / 2) + bias + optional SiLU on mma.sync tensor cores, the kernel of the
+ * PoseGuider's image-resolution layers (musev/models/controlnet.py:334-350). out: channels-last fp16 [NF, H/s, W/s, cout],
+ * cout 16 / 32 / 64 / 128. in_nchw = 1: x is an NCHW image [NF, cin <= 3, H, W] (fp16, or fp32 with x_is_f32) and weight
+ * is [cout, 32] with column tap * cin + c; in_nchw = 0: x is channels-last fp16 [NF, H, W, cin], cin 16 / 32, and weight
+ * is [cout, 9 cin] (tap-major, as above). act: 0 none, 1 SiLU. */
+int mvb_op_small_conv(const void* x, int x_is_f32, int in_nchw, int cin, int H, int W, int NF, int stride, const void* weight,
+                      const float* bias, int cout, int act, void* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Op level: flash attention on wgmma (spatial self / reference / cross attention of the transformer blocks).
@@ -202,6 +209,8 @@ typedef struct mvb_unet_args {
   const void* mid_residual; int residual_is_f32;
   int skip_temporal_layers;
   void* out; int out_is_f32;                   /* [B, out_channels, T, H, W] */
+  const void* pose_guider_emb; int pose_is_f32; /* [(B T), block_out_channels[0], H, W] added to conv_in's output
+                                                   (unet_3d_condition.py:1011-1016); NULL = none (since mvb_version 2) */
 } mvb_unet_args;
 
 /* Reference: UNet3DConditionModel.__init__ (unet_3d_condition.py:213-610). */
@@ -341,6 +350,29 @@ int mvb_vae_decode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspa
 int mvb_create_vae_encoder(const mvb_config* cfg, int device, mvb_handle** out);
 long long mvb_vae_encode_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args);
 int mvb_vae_encode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * PoseGuider, once per pipeline call before the denoise loop (pose-guided video2video, MooreAnimateAnyone's pose guider).
+ * Reference: `musev.models.controlnet.PoseGuider` (musev/models/controlnet.py:326-371): conv_in, then per block i a
+ * stride-1 conv boc[i] -> boc[i] and a stride-2 conv boc[i] -> boc[i+1], SiLU after each, and conv_out (all 3x3, pad 1),
+ * run on `control_image` by musev/pipelines/pipeline_controlnet.py:1774-1783; its output is `pose_guider_emb` of every
+ * UNet call (mvb_unet_args.pose_guider_emb).
+ * The handle is created from an `mvb_config` with in_channels = conditioning channels (1..3), out_channels = embedding
+ * channels, num_blocks / block_out_channels (<= 4); other fields are ignored. Layers reading 16 or 32 channels run on a
+ * small-channel tensor-core kernel; other channel counts are padded to a multiple of 64 and must then be at most 128 where
+ * they are the output of a 16 / 32-channel layer. Weights by the `PoseGuider.state_dict()` names `conv_in.*`,
+ * `blocks.{i}.*`, `conv_out.*`. It takes `mvb_vae_decode_args`, whose fields mean, for the pose guider:
+ *   latents / latents_is_f32  the image [N, in_channels, h * 2^(num_blocks-1), w * 2^(num_blocks-1)], NCHW fp16 / fp32
+ *                             (frames on the batch axis), read directly by conv_in;
+ *   N, h, w                   frames and the OUTPUT size (H/8 x W/8 for four blocks);
+ *   latent_scale              ignored;
+ *   out / out_is_f32          the embedding [N, out_channels, h, w], fp16 / fp32;
+ *   postprocess               must be 0.
+ * Sizes the kernels cannot take are rejected before any launch (negative return, mvb_handle_error). */
+int mvb_create_pose_guider(const mvb_config* cfg, int device, mvb_handle** out);
+long long mvb_pose_guider_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args);
+int mvb_pose_guider_forward(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes,
+                            void* stream);
 
 #ifdef __cplusplus
 }

@@ -61,6 +61,9 @@ def _declare(l: C.CDLL) -> None:
     l.mvb_version.restype = C.c_int
     l.mvb_op_conv_gemm.argtypes = [C.POINTER(ConvGemmDesc), C.c_void_p]
     l.mvb_op_conv_gemm.restype = C.c_int
+    l.mvb_op_small_conv.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                    C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    l.mvb_op_small_conv.restype = C.c_int
     l.mvb_op_attention.argtypes = [C.POINTER(AttentionDesc), C.c_void_p]
     l.mvb_op_attention.restype = C.c_int
     l.mvb_debug_attention_trace.argtypes = [C.c_void_p]

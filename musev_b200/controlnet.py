@@ -7,6 +7,9 @@ scaling run inside libmusevb200.so (`mvb_controlnet_forward`, musev_b200/csrc/en
 call and passes `controlnet_cond_latents` on every step (pipeline_controlnet.py:1258), so it stays a handful of torch
 convolutions here, outside the per-step path.
 
+`PoseGuider` (musev/models/controlnet.py:326-399) is the pose-guided video2video encoder: eight 3x3 convolutions run once per
+pipeline call on the pose images (`mvb_pose_guider_forward`, `Engine::run_pose_guider`); its output is the UNet's
+`pose_guider_emb`.
 """
 from __future__ import annotations
 
@@ -19,8 +22,9 @@ import torch
 import torch.nn.functional as F
 
 from . import _capi
-from .schema import ControlNetConfig, controlnet_param_shapes
+from .schema import ControlNetConfig, PoseGuiderConfig, controlnet_param_shapes, pose_guider_param_shapes
 from .unet import MvbConfig, _is_f32, _lib as _unet_lib, load_weights_batched
+from .vae import MvbVaeDecodeArgs
 
 MAX_OUT = 13
 
@@ -53,6 +57,12 @@ def _lib():
         l.mvb_controlnet_workspace_bytes.restype = C.c_longlong
         l.mvb_controlnet_forward.argtypes = [C.c_void_p, C.POINTER(MvbControlnetArgs), C.c_void_p, C.c_longlong, C.c_void_p]
         l.mvb_controlnet_forward.restype = C.c_int
+        l.mvb_create_pose_guider.argtypes = [C.POINTER(MvbConfig), C.c_int, C.POINTER(C.c_void_p)]
+        l.mvb_create_pose_guider.restype = C.c_int
+        l.mvb_pose_guider_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(MvbVaeDecodeArgs)]
+        l.mvb_pose_guider_workspace_bytes.restype = C.c_longlong
+        l.mvb_pose_guider_forward.argtypes = [C.c_void_p, C.POINTER(MvbVaeDecodeArgs), C.c_void_p, C.c_longlong, C.c_void_p]
+        l.mvb_pose_guider_forward.restype = C.c_int
         _declared = True
     return l
 
@@ -237,5 +247,153 @@ class ControlNetModel:
         if not return_dict:
             return (down, mid)
         return ControlNetOutput(down_block_res_samples=down, mid_block_res_sample=mid)
+
+    __call__ = forward
+
+
+def check_pose_guider_state_dict(cfg: PoseGuiderConfig, state_dict: Dict[str, torch.Tensor], strict: bool = True):
+    """(name, tensor) pairs to load and the unexpected keys of a PoseGuider state dict. A missing key raises KeyError naming
+    it, whatever `strict` says; a wrong shape raises RuntimeError; unexpected keys raise only when `strict`."""
+    expected = pose_guider_param_shapes(cfg)
+    missing = [k for k in expected if k not in state_dict]
+    if missing:
+        more = f" (and {len(missing) - 1} more)" if len(missing) > 1 else ""
+        raise KeyError(f"PoseGuider state dict is missing {missing[0]!r}{more}; the engine has no initialiser for it")
+    unexpected = [k for k in state_dict if k not in expected]
+    if strict and unexpected:
+        raise RuntimeError(f"Error(s) in loading state_dict: unexpected {unexpected[:5]}")
+    todo = []
+    for name, shape in expected.items():
+        t = state_dict[name]
+        if tuple(t.shape) != tuple(shape):
+            raise RuntimeError(f"size mismatch for {name}: {tuple(t.shape)} vs {tuple(shape)}")
+        todo.append((name, t))
+    return todo, unexpected
+
+
+class PoseGuider:
+    """CUDA engine behind the call surface of `musev.models.controlnet.PoseGuider` (musev/models/controlnet.py:326-399).
+
+    Kept: the constructor arguments, `from_pretrained(path, conditioning_embedding_channels, conditioning_channels,
+    block_out_channels)`, `forward(conditioning [b, c, t, H, W]) -> [b, emb, t, H/8, W/8]`, `.to()`, `.eval()` and the
+    reference state-dict names. Frames run in chunks of `frames_per_call` (bounds the activation workspace, like the VAE).
+    Departure: the reference loads with `strict=False` and keeps its initialiser's values for a missing key; the engine
+    has no initialiser, so a missing key raises, naming it. Unexpected keys are ignored when `strict=False`."""
+
+    def __init__(self, conditioning_embedding_channels: int, conditioning_channels: int = 3,
+                 block_out_channels: Tuple[int, ...] = (16, 32, 64, 128), device: Union[str, torch.device] = "cuda",
+                 dtype: torch.dtype = torch.float16, frames_per_call: int = 8):
+        if not torch.cuda.is_available():
+            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
+        self.cfg = PoseGuiderConfig(int(conditioning_embedding_channels), int(conditioning_channels), tuple(block_out_channels))
+        self.config = SimpleNamespace(**asdict(self.cfg))
+        self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
+        self.dtype = dtype
+        self.frames_per_call = int(frames_per_call)
+        self._ws: Optional[torch.Tensor] = None
+        self._h = C.c_void_p()
+        self._loaded = False
+        c = MvbConfig()
+        c.in_channels, c.out_channels = self.cfg.conditioning_channels, self.cfg.conditioning_embedding_channels
+        c.num_blocks = len(self.cfg.block_out_channels)
+        if not 1 <= c.num_blocks <= 4:
+            raise ValueError(f"block_out_channels must have 1..4 entries, got {self.cfg.block_out_channels}")
+        for i, v in enumerate(self.cfg.block_out_channels):
+            c.block_out_channels[i] = v
+        rc = _lib().mvb_create_pose_guider(C.byref(c), self.device.index or 0, C.byref(self._h))
+        if rc != 0:
+            raise _capi.MvbError(f"mvb_create_pose_guider failed ({rc}): unsupported channel counts {self.cfg} "
+                                 "or out of device memory")
+
+    @classmethod
+    def from_pretrained(cls, pretrained_model_path, conditioning_embedding_channels: int, conditioning_channels: int = 3,
+                        block_out_channels: Tuple[int, ...] = (16, 32, 64, 128), device="cuda", dtype=torch.float16):
+        """controlnet.py:373-399: a `torch.load`-able state dict file; loaded with `strict=False` (see the class notes)."""
+        state_dict = torch.load(pretrained_model_path, map_location="cpu")
+        m = cls(conditioning_embedding_channels, conditioning_channels, block_out_channels, device=device, dtype=dtype)
+        m.load_state_dict(state_dict, strict=False)
+        return m
+
+    def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = True):
+        todo, unexpected = check_pose_guider_state_dict(self.cfg, state_dict, strict)
+        load_weights_batched(self._h, todo, self.device)
+        l = _lib()
+        rc = l.mvb_finalize(self._h)
+        if rc != 0:
+            raise _capi.MvbError(f"mvb_finalize: {l.mvb_handle_error(self._h).decode()}")
+        self._loaded = True
+        return SimpleNamespace(missing_keys=[], unexpected_keys=unexpected)
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) and self._h.value:
+                _lib().mvb_destroy(self._h)
+                self._h = C.c_void_p()
+        except Exception:
+            pass
+
+    def eval(self):
+        return self
+
+    def to(self, *args, **kwargs):
+        for a in list(args) + list(kwargs.values()):
+            if isinstance(a, torch.dtype):
+                if a not in (torch.float16, torch.float32):
+                    raise ValueError("musev_b200 computes in fp16 with fp32 accumulation; I/O dtype is fp16 or fp32")
+                self.dtype = a
+            elif isinstance(a, (str, torch.device)) and torch.device(a).type != "cuda":
+                raise RuntimeError("musev_b200 has no CPU path")
+        return self
+
+    @torch.no_grad()
+    def embed_frames(self, images: torch.Tensor, out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+        """images [N, c, H, W] (fp16 / fp32, frames on the batch axis) -> [N, emb, H / 2^(nb-1), W / 2^(nb-1)]."""
+        if not self._loaded:
+            raise RuntimeError("weights not loaded: call load_state_dict first")
+        f = 2 ** (len(self.cfg.block_out_channels) - 1)
+        if images.dim() != 4 or images.shape[1] != self.cfg.conditioning_channels:
+            raise ValueError(f"conditioning must have {self.cfg.conditioning_channels} channels, got {tuple(images.shape)}")
+        N, _, H, W = images.shape
+        if N < 1 or H < f or W < f or H % f or W % f:
+            raise ValueError(f"image size {H}x{W} must be a positive multiple of {f} (the pose guider downsamples {f}x)")
+        x = images.to(self.device)
+        if x.dtype not in (torch.float16, torch.float32):
+            x = x.float()
+        x = x.contiguous()
+        h, w = H // f, W // f
+        out = torch.empty((N, self.cfg.conditioning_embedding_channels, h, w), dtype=out_dtype or self.dtype, device=self.device)
+        l = _lib()
+        step = max(1, self.frames_per_call)
+        for n0 in range(0, N, step):
+            n1 = min(N, n0 + step)
+            xc, oc = x[n0:n1], out[n0:n1]
+            a = MvbVaeDecodeArgs()
+            a.latents, a.latents_is_f32 = xc.data_ptr(), _is_f32(xc)
+            a.N, a.h, a.w = n1 - n0, h, w
+            a.latent_scale = 1.0
+            a.out, a.out_is_f32 = oc.data_ptr(), _is_f32(oc)
+            a.postprocess = 0
+            need = l.mvb_pose_guider_workspace_bytes(self._h, C.byref(a))
+            if need < 0:
+                raise _capi.MvbError(f"mvb_pose_guider_workspace_bytes: {l.mvb_handle_error(self._h).decode()}")
+            if self._ws is None or self._ws.numel() < need:
+                self._ws = None
+                self._ws = torch.empty(int(need), dtype=torch.uint8, device=self.device)
+            rc = l.mvb_pose_guider_forward(self._h, C.byref(a), self._ws.data_ptr(), self._ws.numel(),
+                                           torch.cuda.current_stream(self.device).cuda_stream)
+            if rc != 0:
+                raise _capi.MvbError(f"mvb_pose_guider_forward ({rc}): {l.mvb_handle_error(self._h).decode()}")
+        self._keep = x
+        return out
+
+    @torch.no_grad()
+    def forward(self, conditioning: torch.Tensor) -> torch.Tensor:
+        """PoseGuider.forward (controlnet.py:361-371): conditioning [b, c, t, H, W] -> [b, emb, t, H/8, W/8] (four blocks)."""
+        if conditioning.dim() != 5:
+            raise ValueError(f"conditioning must be [b, c, t, H, W], got {tuple(conditioning.shape)}")
+        b, c, t, H, W = conditioning.shape
+        x = conditioning.permute(0, 2, 1, 3, 4).reshape(b * t, c, H, W)                    # InflatedConv3d, :308-316
+        e = self.embed_frames(x)
+        return e.view(b, t, *e.shape[1:]).permute(0, 2, 1, 3, 4).contiguous()
 
     __call__ = forward

@@ -149,6 +149,47 @@ int mvb_vae_encode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspa
   return h->e->vae_encode(*args, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
+// The layer split of Engine::build_pose_guider: conv_in and every layer reading 16 / 32 channels run on the small-channel
+// kernel, whose output is at most 128 (padded) channels.
+static bool pose_guider_config_ok(const mvb_config* cfg) {
+  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->in_channels < 1 || cfg->in_channels > 3) return false;
+  if (cfg->out_channels < 1 || cfg->out_channels > 4096) return false;
+  const int nb = cfg->num_blocks;
+  for (int i = 0; i < nb; ++i)
+    if (cfg->block_out_channels[i] < 1 || cfg->block_out_channels[i] > 4096) return false;
+  auto small = [](int cin) { return cin == 16 || cin == 32; };
+  if (mvb::cond_channels_padded(cfg->block_out_channels[0]) > 128) return false;                           // conv_in
+  for (int i = 0; i + 1 < nb; ++i) {
+    const int c = cfg->block_out_channels[i], n = cfg->block_out_channels[i + 1];
+    if (small(c) && mvb::cond_channels_padded(n) > 128) return false;                                       // blocks.2i+1
+  }
+  if (small(cfg->block_out_channels[nb - 1]) && cfg->out_channels > 128) return false;                      // conv_out
+  return true;
+}
+
+int mvb_create_pose_guider(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out) return MVB_ERR_INVALID;
+  if (!pose_guider_config_ok(cfg)) return MVB_ERR_INVALID;
+  mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, 5);
+  if (!e) return MVB_ERR_STATE;
+  if (e->error()[0]) { delete e; return MVB_ERR_CUDA; }
+  mvb_handle* h = new (std::nothrow) mvb_handle{e};
+  if (!h) { delete e; return MVB_ERR_STATE; }
+  *out = h;
+  return MVB_OK;
+}
+
+long long mvb_pose_guider_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args) {
+  if (!h || !args) return -1;
+  return h->e->pose_guider_workspace_bytes(*args);
+}
+
+int mvb_pose_guider_forward(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes,
+                            void* stream) {
+  if (!h || !args) return MVB_ERR_INVALID;
+  return h->e->pose_guider_forward(*args, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 void mvb_destroy(mvb_handle* h) {
   if (!h) return;
   delete h->e;

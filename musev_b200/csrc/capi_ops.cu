@@ -6,6 +6,7 @@
 
 #include "../../include/musev_b200.h"
 #include "attention.cuh"
+#include "cond_embed.cuh"
 #include "conv_gemm.cuh"
 #include "ops.cuh"
 
@@ -32,7 +33,7 @@ extern "C" {
 
 const char* mvb_last_error(void) { return g_err; }
 
-int mvb_version(void) { return 1; }
+int mvb_version(void) { return 2; }   // 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   if (!d || !d->a0 || !d->weight || !d->out) return fail("mvb_op_conv_gemm: null pointer", cudaSuccess);
@@ -55,6 +56,13 @@ int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   return MVB_OK;
 }
 
+int mvb_op_small_conv(const void* x, int x_is_f32, int in_nchw, int cin, int H, int W, int NF, int stride, const void* weight,
+                      const float* bias, int cout, int act, void* out, void* stream) {
+  const char* err = nullptr;
+  cudaError_t e = launch_small_conv((cudaStream_t)stream, x, x_is_f32, in_nchw, cin, H, W, NF, stride, (const __half*)weight,
+                                    bias, cout, act, (__half*)out, sm_count(), &err);
+  return e == cudaSuccess ? MVB_OK : fail(err, e);
+}
 
 int mvb_op_attention(const mvb_attention_desc* d, void* stream) {
   if (!d || !d->q || !d->out || !d->k[0] || !d->v[0]) return fail("mvb_op_attention: null pointer", cudaSuccess);

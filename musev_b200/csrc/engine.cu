@@ -8,6 +8,7 @@
 #include <string.h>
 
 #include "attention.cuh"
+#include "cond_embed.cuh"
 #include "conv_gemm.cuh"
 #include "ops.cuh"
 
@@ -18,7 +19,8 @@ static inline int pad16(int d) { return (d + 15) / 16 * 16; }
 // ---------------------------------------------------------------------------------------------- packing kernels
 template <typename TSrc>
 __global__ void pack_matrix_kernel(__half* __restrict__ dst, long long ld, int rows_dst, int kdst, const TSrc* __restrict__ src,
-                                   int nsrc, int ksrc, int rowmode, int p0, int p1, int colmode, int cin, int taps) {
+                                   int nsrc, int ksrc, int rowmode, int p0, int p1, int colmode, int cin, int taps,
+                                   int cin_dst) {
   const long long total = (long long)rows_dst * kdst;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int r = (int)(i / kdst), kk = (int)(i % kdst);
@@ -32,7 +34,8 @@ __global__ void pack_matrix_kernel(__half* __restrict__ dst, long long ld, int r
     }
     int scol = kk;
     if (colmode == 1) {
-      if (kk < cin * taps) { const int tap = kk / cin, c = kk % cin; scol = c * taps + tap; } else scol = -1;
+      const int cd = cin_dst > cin ? cin_dst : cin;
+      if (kk < cd * taps) { const int tap = kk / cd, c = kk % cd; scol = c < cin ? c * taps + tap : -1; } else scol = -1;
     } else if (kk >= ksrc) scol = -1;
     float v = 0.f;
     if (srow >= 0 && srow < nsrc && scol >= 0) v = (float)src[(long long)srow * ksrc + scol];
@@ -62,6 +65,7 @@ struct PackDesc {
   long long ld;
   int rows_dst, kdst, nsrc, ksrc, rowmode, p0, p1, colmode, cin, taps;
   int is_vec, vn, vmode, is_f32;
+  int cin_dst;
 };
 __device__ __forceinline__ float pack_src(const void* src, long long i, int is_f32) {
   return is_f32 ? reinterpret_cast<const float*>(src)[i] : __half2float(reinterpret_cast<const __half*>(src)[i]);
@@ -91,7 +95,8 @@ __global__ void pack_batch_kernel(const PackDesc* __restrict__ descs) {
     }
     int scol = kk;
     if (d.colmode == 1) {
-      if (kk < d.cin * d.taps) { const int tap = kk / d.cin, c = kk % d.cin; scol = c * d.taps + tap; } else scol = -1;
+      const int cd = d.cin_dst > d.cin ? d.cin_dst : d.cin;
+      if (kk < cd * d.taps) { const int tap = kk / cd, c = kk % cd; scol = c < d.cin ? c * d.taps + tap : -1; } else scol = -1;
     } else if (kk >= d.ksrc) scol = -1;
     float v = 0.f;
     if (srow >= 0 && srow < d.nsrc && scol >= 0) v = pack_src(d.src, (long long)srow * d.ksrc + scol, d.is_f32);
@@ -315,6 +320,7 @@ void Engine::build() {
   if (kind_ == 1 || kind_ == 2) build_controlnet();
   else if (kind_ == 3) build_vae();
   else if (kind_ == 4) build_vae_encoder();
+  else if (kind_ == 5) build_pose_guider();
   else build_unet();
 }
 
@@ -365,6 +371,36 @@ void Engine::build_vae_encoder() {
   vae_pq_b_ = slab<float>(zc2);
   reg_vec("quant_conv.weight", vae_pq_w_, zc2 * zc2, zc2 * zc2);
   reg_vec("quant_conv.bias", vae_pq_b_, zc2, zc2);
+}
+
+// PoseGuider.__init__ (musev/models/controlnet.py:326-359): conv_in (in_channels -> boc[0]), per block i < nb - 1 a stride-1
+// conv boc[i] -> boc[i] and a stride-2 conv boc[i] -> boc[i + 1], conv_out (boc[-1] -> out_channels); SiLU after all but
+// conv_out. Layers reading 16 / 32 channels (and conv_in, which reads the image) run on the small-channel kernel; the
+// others on conv_gemm / conv_s2 with their input channels padded to a multiple of 64.
+void Engine::build_pose_guider() {
+  const mvb_config& c = cfg_;
+  const int nb = c.num_blocks;
+  pg_.clear();
+  auto add = [&](const std::string& p, int cin, int cout, int stride, bool image, bool act) {
+    CondConv L;
+    L.cin = cin; L.cout = cout; L.stride = stride; L.act = act;
+    L.small = image || cin == 16 || cin == 32;
+    L.cin_p = image ? cin : cond_channels_padded(cin);
+    L.cout_p = act ? cond_channels_padded(cout) : (cout + 7) / 8 * 8;
+    if (L.small) L.cout_p = L.cout_p <= 16 ? 16 : L.cout_p <= 32 ? 32 : L.cout_p <= 64 ? 64 : 128;   // kernel widths
+    const int K = image ? 32 : 9 * L.cin_p;
+    L.m = make_mat(L.cout_p, K, true);
+    reg_mat(p + ".weight", L.m, 0, cout, 0, 0, 0, cout, cin * 9, 1, cin, 9);
+    if (!image) loaders_[p + ".weight"].cin_dst = L.cin_p;
+    reg_vec(p + ".bias", L.m.bias, L.cout_p, cout);
+    pg_.push_back(L);
+  };
+  add("conv_in", c.in_channels, c.block_out_channels[0], 1, true, true);
+  for (int i = 0; i + 1 < nb; ++i) {
+    add("blocks." + std::to_string(2 * i), c.block_out_channels[i], c.block_out_channels[i], 1, false, true);
+    add("blocks." + std::to_string(2 * i + 1), c.block_out_channels[i], c.block_out_channels[i + 1], 2, false, true);
+  }
+  add("conv_out", c.block_out_channels[nb - 1], c.out_channels, 1, false, false);
 }
 
 // AutoencoderKL decoder half: post_quant_conv + Decoder.__init__ (diffusers models/autoencoder_kl.py:102-104, vae.py:201-263):
@@ -580,10 +616,10 @@ int Engine::load_weight(const char* name, const void* ptr, int is_f32, const lon
     const int blocks = (int)((total + 255) / 256 < 132 * 32 ? (total + 255) / 256 : 132 * 32);
     if (is_f32)
       pack_matrix_kernel<float><<<blocks, 256>>>(l.dst, l.ld, l.rows_dst, l.kdst, (const float*)ptr, l.nsrc, l.ksrc,
-                                                 l.rowmode, l.p0, l.p1, l.colmode, l.cin, l.taps);
+                                                 l.rowmode, l.p0, l.p1, l.colmode, l.cin, l.taps, l.cin_dst);
     else
       pack_matrix_kernel<__half><<<blocks, 256>>>(l.dst, l.ld, l.rows_dst, l.kdst, (const __half*)ptr, l.nsrc, l.ksrc,
-                                                  l.rowmode, l.p0, l.p1, l.colmode, l.cin, l.taps);
+                                                  l.rowmode, l.p0, l.p1, l.colmode, l.cin, l.taps, l.cin_dst);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { err_ = std::string("pack kernel: ") + cudaGetErrorString(e); return MVB_ERR_CUDA; }
@@ -625,6 +661,7 @@ int Engine::load_weights(const mvb_named_tensor* ts, int n) {
       if (numel != (long long)l.nsrc * l.ksrc) { err_ = std::string("bad shape for ") + t.name; return MVB_ERR_INVALID; }
       d.dst = l.dst; d.ld = l.ld; d.rows_dst = l.rows_dst; d.kdst = l.kdst; d.nsrc = l.nsrc; d.ksrc = l.ksrc;
       d.rowmode = l.rowmode; d.p0 = l.p0; d.p1 = l.p1; d.colmode = l.colmode; d.cin = l.cin; d.taps = l.taps;
+      d.cin_dst = l.cin_dst;
     }
     descs.push_back(d);
     touched.push_back(&l);
@@ -1121,6 +1158,14 @@ bool Engine::run(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
       if (e != cudaSuccess) f.fail("im2col_latent", e);
     }
     Epilogue ep; ep.out = x; ep.ldc = c0;
+    if (a.pose_guider_emb) {   // sample = conv_in(sample) + pose_guider_emb (:1011-1016), added in the GEMM epilogue
+      __half* pose = f.alloc_h(M, c0);
+      if (!ar.dry && f.ok) {
+        cudaError_t e = ncthw_to_tokens(s, a.pose_guider_emb, a.pose_is_f32, NF, c0, 1, Hc * Wc, pose, c0, 1.f);
+        if (e != cudaSuccess) f.fail("pose_guider_emb convert", e);
+      }
+      ep.res = pose; ep.ld_res = c0;
+    }
     f.gemm(A, M, 64, conv_in_, ep);
     f.release(mk);
   }
@@ -1569,6 +1614,97 @@ int Engine::vae_encode(const mvb_vae_decode_args& a, void* workspace, long long 
   ar.base = (char*)workspace;
   ar.cap = (size_t)wbytes;
   if (!run_vae_encode(a, ar, stream)) return MVB_ERR_CUDA;
+  return MVB_OK;
+}
+
+static const char* pose_guider_shape_error(const mvb_vae_decode_args& a, int nb) {
+  if (a.N < 1 || a.h < 1 || a.w < 1) return "pose guider: bad shape (N, h, w must be positive)";
+  if (a.postprocess != 0) return "pose guider: postprocess must be 0";
+  const long long H = (long long)a.h << (nb - 1), W = (long long)a.w << (nb - 1);
+  if (H > 8192 || W > 8192 || (long long)a.N * H * W > (1LL << 24))
+    return "pose guider: image too large (at most 8192 pixels a side and 2^24 pixels per call; split the frames)";
+  return nullptr;
+}
+
+// PoseGuider.forward (musev/models/controlnet.py:361-371) on frames-on-the-batch-axis images: a.latents = image
+// [N, in_channels, h 2^(nb-1), w 2^(nb-1)] (NCHW, read directly by conv_in), a.out = [N, out_channels, h, w].
+// Activations are channels-last fp16 in two ping-pong buffers.
+bool Engine::run_pose_guider(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s) {
+  const mvb_config& c = cfg_;
+  const int nb = c.num_blocks, NF = a.N;
+  if (const char* bad = pose_guider_shape_error(a, nb)) { err_ = bad; return false; }
+  int Hc = a.h << (nb - 1), Wc = a.w << (nb - 1);
+  size_t most = 0;
+  {
+    int hh = Hc, ww = Wc;
+    for (const CondConv& L : pg_) {
+      hh /= L.stride; ww /= L.stride;
+      const size_t b = (size_t)NF * hh * ww * L.cout_p * sizeof(__half);
+      if (b > most) most = b;
+    }
+  }
+  __half* buf[2] = {(__half*)ar.alloc(most), (__half*)ar.alloc(most)};
+  if (!buf[0] || !buf[1]) { err_ = "workspace too small"; return false; }
+  if (!ar.dry) taps_.clear();
+  const void* x = a.latents;
+  int cur = 0;
+  for (size_t i = 0; i < pg_.size(); ++i) {
+    const CondConv& L = pg_[i];
+    __half* y = buf[cur];
+    const int Ho = Hc / L.stride, Wo = Wc / L.stride;
+    if (!ar.dry) {
+      const char* err = nullptr;
+      cudaError_t e;
+      if (L.small) {
+        e = launch_small_conv(s, x, i == 0 ? a.latents_is_f32 : 0, i == 0, i == 0 ? L.cin : L.cin_p, Hc, Wc, NF, L.stride,
+                              L.m.w, L.m.bias, L.cout_p, L.act ? 1 : 0, y, num_sms_, &err);
+      } else {
+        Epilogue ep; ep.out = y; ep.ldc = L.cout_p; ep.bias = L.m.bias; ep.act = L.act ? 1 : 0;
+        const __half* xh = (const __half*)x;
+        if (L.stride == 2) {
+          e = launch_conv_s2(s, xh, L.cin_p, Wc, Hc, NF, L.m.w, L.cout_p, ep, num_sms_, &err, 1);
+        } else {
+          static const int8_t dy[9] = {-1, -1, -1, 0, 0, 0, 1, 1, 1}, dx[9] = {-1, 0, 1, -1, 0, 1, -1, 0, 1};
+          ASource a0{xh, L.cin_p, (long long)L.cin_p, (long long)L.cin_p * Wc, (long long)L.cin_p * Wc * Hc};
+          e = launch_conv_gemm(s, a0, nullptr, Wc, Hc, NF, 9, dy, dx, L.m.w, L.cout_p, ep, num_sms_, &err);
+        }
+      }
+      if (e != cudaSuccess) {
+        err_ = std::string(i == 0 ? "conv_in" : i + 1 == pg_.size() ? "conv_out" : "blocks." + std::to_string(i - 1)) +
+               ": " + (err ? err : "launch failed") + " (" + cudaGetErrorString(e) + ")";
+        return false;
+      }
+      taps_.push_back({i == 0 ? "conv_in" : i + 1 == pg_.size() ? "conv_out" : "blocks." + std::to_string(i - 1), y,
+                       (long long)NF * Ho * Wo, L.cout_p});
+    }
+    x = y; cur ^= 1; Hc = Ho; Wc = Wo;
+  }
+  if (!ar.dry) {
+    cudaError_t e = tokens_to_ncthw(s, (const __half*)x, pg_.back().cout_p, NF, c.out_channels, 1, Hc * Wc, a.out, a.out_is_f32);
+    if (e != cudaSuccess) { err_ = std::string("pose guider output: ") + cudaGetErrorString(e); return false; }
+  }
+  return true;
+}
+
+long long Engine::pose_guider_workspace_bytes(const mvb_vae_decode_args& a) {
+  if (kind_ != 5) { err_ = "not a PoseGuider handle"; return -1; }
+  Arena ar;
+  ar.dry = true;
+  if (!run_pose_guider(a, ar, nullptr)) return -1;
+  return (long long)ar.peak + 4096;
+}
+
+int Engine::pose_guider_forward(const mvb_vae_decode_args& a, void* workspace, long long wbytes, cudaStream_t stream) {
+  if (kind_ != 5) { err_ = "not a PoseGuider handle"; return MVB_ERR_STATE; }
+  if (!finalized_) { err_ = "mvb_finalize has not been called (or weights are missing)"; return MVB_ERR_STATE; }
+  if (!a.latents || !a.out || !workspace) { err_ = "null pointer argument"; return MVB_ERR_INVALID; }
+  if (const char* bad = pose_guider_shape_error(a, cfg_.num_blocks)) { err_ = bad; return MVB_ERR_INVALID; }
+  cudaSetDevice(device_);
+  Arena ar;
+  ar.dry = false;
+  ar.base = (char*)workspace;
+  ar.cap = (size_t)wbytes;
+  if (!run_pose_guider(a, ar, stream)) return MVB_ERR_CUDA;
   return MVB_OK;
 }
 

@@ -88,6 +88,7 @@ struct Loader {
   int p0 = 0, p1 = 0;
   int colmode = 0;  // 0 identity (zero fill beyond Ksrc), 1 conv [N, Cin, taps] -> (tap, c)
   int cin = 0, taps = 1;
+  int cin_dst = 0;  // colmode 1: destination channel stride per tap when > cin (the padding columns stay zero)
   int nsrc = 0, ksrc = 0;
   // LK_VEC
   float* vdst = nullptr;
@@ -96,6 +97,15 @@ struct Loader {
   // LK_ABS_SCALAR
   float* host_scalar = nullptr;
   bool loaded = false;
+};
+
+// One 3x3 convolution of a conditioning-embedding stack (PoseGuider). Channel counts other than 16 / 32 are padded to a
+// multiple of 64 with zero weight rows / columns and zero bias, so a padded channel is SiLU(0) = 0 and stays exact.
+struct CondConv {
+  Mat m;                 // packed [cout_p, K]: K = 32 (image conv_in), 9 cin_p otherwise; column tap * cin_p + c
+  int cin = 0, cin_p = 0, cout = 0, cout_p = 0, stride = 1;
+  bool small = false;    // cond_embed.cu small-channel kernel (cin 16 / 32 or the image conv_in); else conv_gemm / conv_s2
+  bool act = true;       // SiLU after every conv except conv_out
 };
 
 struct Arena {
@@ -115,7 +125,8 @@ class Engine {
  public:
   // kind 0: UNet3DConditionModel; kind 1: ControlNet encoder (diffusers models/controlnet.py);
   // kind 2: ReferenceNet2D encoder + mid block (musev/models/referencenet.py);
-  // kind 3: AutoencoderKL decoder (diffusers models/autoencoder_kl.py, vae.py); kind 4: AutoencoderKL encoder (same files)
+  // kind 3: AutoencoderKL decoder (diffusers models/autoencoder_kl.py, vae.py); kind 4: AutoencoderKL encoder (same files);
+  // kind 5: PoseGuider (musev/models/controlnet.py:326-371)
   explicit Engine(const mvb_config& cfg, int device, int kind = 0);
   ~Engine();
   int load_weight(const char* name, const void* dev_ptr, int is_f32, const long long* shape, int ndim);
@@ -132,6 +143,8 @@ class Engine {
   int vae_decode(const mvb_vae_decode_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long vae_encode_workspace_bytes(const mvb_vae_decode_args& a);
   int vae_encode(const mvb_vae_decode_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
+  long long pose_guider_workspace_bytes(const mvb_vae_decode_args& a);
+  int pose_guider_forward(const mvb_vae_decode_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long controlnet_workspace_bytes(const mvb_controlnet_args& a);
   int controlnet_forward(const mvb_controlnet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   int kind() const { return kind_; }
@@ -148,6 +161,7 @@ class Engine {
   void build_vae();
   void build_vae_encoder();
   void build_vae_mid(const std::string& p, int C);
+  void build_pose_guider();
   template <typename T> T* slab(size_t n);
   Mat make_mat(int N, int K, bool bias);
   Norm make_norm(const std::string& p, int C);
@@ -169,6 +183,7 @@ class Engine {
   bool run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_t s);
   bool run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
   bool run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
+  bool run_pose_guider(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
 
   mvb_config cfg_;
   int device_ = 0, num_sms_ = 132;
@@ -213,6 +228,10 @@ class Engine {
   float* vae_pq_b_ = nullptr;
   Norm vae_attn_norm_;
   Mat vae_q_, vae_k_, vae_v_, vae_o_;
+  std::vector<CondConv> pg_;   // PoseGuider: conv_in, blocks.0 .. blocks.{2 (num_blocks - 1) - 1}, conv_out
 };
+
+// Channel count a PoseGuider activation is stored with: 16 / 32 as is (small-channel kernel), others padded to 64k.
+inline int cond_channels_padded(int c) { return (c == 16 || c == 32) ? c : (c + 63) / 64 * 64; }
 
 }  // namespace mvb

@@ -221,3 +221,15 @@ def vae_decoder_flops(cfg, N: int, h: int, w: int) -> Dict[str, float]:
             conv(N * H * W, ch, ch, 9)
     conv(N * H * W, boc[0], cfg.out_channels, 9)
     return _vae_total(f)
+
+
+def pose_guider_flops(cfg, N: int, H: int, W: int) -> Dict[str, float]:
+    """`PoseGuider.forward` on N images of H x W (PoseGuiderConfig `cfg`; musev/models/controlnet.py:361-371), 2 M N K per
+    3x3 convolution over the reference's channel counts (padding channels are not counted). (16, 32, 96, 256) -> 320 at
+    512 x 512: 14.72 GFLOP per frame."""
+    from .schema import pose_guider_layers
+    f, conv, _, _ = _vae_counters()
+    for _, cin, cout, stride in pose_guider_layers(cfg):
+        H, W = (H - 1) // stride + 1, (W - 1) // stride + 1
+        conv(N * H * W, cin, cout, 9)
+    return _vae_total(f)

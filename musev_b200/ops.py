@@ -82,6 +82,22 @@ def conv_gemm(
     return out
 
 
+def small_conv(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], stride: int = 1, act: bool = True,
+               nchw: bool = False) -> torch.Tensor:
+    """3x3 conv (pad 1) + bias + SiLU on the small-channel kernel. x: channels-last fp16 [NF, H, W, cin] (cin 16 / 32) or,
+    with nchw, an image [NF, cin <= 3, H, W] fp16 / fp32; weight: packed fp16 [cout, 9 cin] (nchw: [cout, 32]), column
+    tap * cin + c. Returns channels-last fp16 [NF, H / stride, W / stride, cout]."""
+    if nchw:
+        NF, cin, H, W = x.shape
+    else:
+        NF, H, W, cin = x.shape
+    cout = weight.shape[0]
+    out = torch.empty(NF, (H - 1) // stride + 1, (W - 1) // stride + 1, cout, dtype=torch.float16, device=x.device)
+    _capi.check(_capi.lib().mvb_op_small_conv(_ptr(x), int(x.dtype == torch.float32), int(nchw), cin, H, W, NF, stride,
+                                              _ptr(weight), _ptr(bias), cout, int(act), _ptr(out), _stream()))
+    return out
+
+
 def attention(q, segs, NF, Nq, heads, d, dp, scale, out=None, out_scale=1.0, accumulate=False, v_ones_col=False, variant=0):
     """q: [NF*Nq, >=heads*dp] fp16 (row stride taken from the tensor); segs: list of dicts
     {k, v, nk, fdiv, fmul, fadd} with k/v [rows, >=heads*dp] views sharing a row stride."""

@@ -65,6 +65,7 @@ class ParallelDenoiser:
         noise_type: str = "random",                    # or "video_fusion" (pipeline_controlnet.py:1690-1696)
         w_ind_noise: float = 0.5,
         cfg_split: bool = False,                       # pair the ranks: each rank of a pair runs ONE half of the CFG batch
+        pose_guider_emb: Optional[torch.Tensor] = None,  # [2B, C0, n_vc + T, h, w], vision-condition frames first
     ) -> DenoiseOutput:
         if guidance_scale <= 1.0:
             # the reference's CFG-off branch feeds the wrong vis-cond tensor (pipeline_controlnet.py:1922-1926, Q14)
@@ -73,6 +74,13 @@ class ParallelDenoiser:
         dev = latents.device
         B, C, T, h, w = latents.shape
         n_vc = condition_latents.shape[2]
+        if pose_guider_emb is not None:
+            # the PoseGuider output (pipeline_controlnet.py:1774-1783, UNet :2066), on the frame axis of make_controlnet_fn's
+            # controlnet_latents; every window gets its own frames (see DESIGN.md section 5)
+            pg = pose_guider_emb
+            if pg.dim() != 5 or pg.shape[0] != 2 * B or tuple(pg.shape[2:]) != (n_vc + T, h, w):
+                raise ValueError(f"pose_guider_emb must be [2B, C0, n_vc + T, h, w] = [{2 * B}, C0, {n_vc + T}, {h}, {w}], "
+                                 f"got {tuple(pg.shape)}")
         sch = self.scheduler
         sch.set_timesteps(num_inference_steps, device="cpu")
         contexts = [c[0] for c in prepare_global_context(context_schedule, num_inference_steps, T, context_frames,
@@ -150,6 +158,15 @@ class ParallelDenoiser:
                 else:
                     model_in = torch.cat([cond2, torch.cat([lat_c] * 2)], dim=2)    # :1908-1946
                 kw = dict(unet_kwargs)
+                if pose_guider_emb is not None:
+                    # vision-condition frames + this window's frames (duplicates included), (b t) c h w like model_in
+                    ctx = torch.tensor(list(range(n_vc)) + [ci + n_vc for ci in c], dtype=torch.long,
+                                       device=pose_guider_emb.device)
+                    pe = pose_guider_emb.index_select(2, ctx)
+                    if cfg_split:
+                        pe = pe[rows]
+                    nb, c0, tc = pe.shape[:3]
+                    kw["pose_guider_emb"] = pe.permute(0, 2, 1, 3, 4).reshape(nb * tc, c0, h, w)
                 if controlnet_fn is not None:
                     if cfg_split:      # the callback gets this rank's half of the CFG batch and which rows it is
                         down_res, mid_res = controlnet_fn(c, model_in, t, i, rows)

@@ -439,3 +439,34 @@ def vae_encoder_param_shapes(cfg: VAEConfig) -> "OrderedDict[str, Tuple[int, ...
     out["quant_conv.weight"] = (zc2, zc2, 1, 1)
     out["quant_conv.bias"] = (zc2,)
     return out
+
+
+# ------------------------------------------------------------------------------------------------ PoseGuider
+@dataclass
+class PoseGuiderConfig:
+    """Constructor arguments of `musev.models.controlnet.PoseGuider` (musev/models/controlnet.py:326-359). The class default
+    is (16, 32, 64, 128); scripts/inference/video2video.py:1024-1030 builds (16, 32, 96, 256) -> 320."""
+    conditioning_embedding_channels: int = 320
+    conditioning_channels: int = 3
+    block_out_channels: Tuple[int, ...] = (16, 32, 64, 128)
+
+
+def pose_guider_layers(cfg: PoseGuiderConfig):
+    """(name, cin, cout, stride) of the PoseGuider's 3x3 convolutions in forward order; SiLU follows all but conv_out."""
+    boc = cfg.block_out_channels
+    out = [("conv_in", cfg.conditioning_channels, boc[0], 1)]
+    for i in range(len(boc) - 1):
+        out.append((f"blocks.{2 * i}", boc[i], boc[i], 1))
+        out.append((f"blocks.{2 * i + 1}", boc[i], boc[i + 1], 2))
+    out.append(("conv_out", boc[-1], cfg.conditioning_embedding_channels, 1))
+    return out
+
+
+def pose_guider_param_shapes(cfg: PoseGuiderConfig) -> "OrderedDict[str, Tuple[int, ...]]":
+    """name -> shape of the reference `PoseGuider.state_dict()`: a weight and a bias per convolution, 4 len(block_out_channels)
+    tensors."""
+    out: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    for name, cin, cout, _ in pose_guider_layers(cfg):
+        out[f"{name}.weight"] = (cout, cin, 3, 3)
+        out[f"{name}.bias"] = (cout,)
+    return out

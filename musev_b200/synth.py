@@ -14,9 +14,9 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from .schema import (ControlNetConfig, ImageProjConfig, ReferenceNetConfig, UNetConfig, VAEConfig, controlnet_param_shapes,
-                     image_proj_param_shapes, refer_emb_shapes, referencenet_param_shapes, unet_param_shapes,
-                     vae_decoder_param_shapes, vae_encoder_param_shapes)
+from .schema import (ControlNetConfig, ImageProjConfig, PoseGuiderConfig, ReferenceNetConfig, UNetConfig, VAEConfig,
+                     controlnet_param_shapes, image_proj_param_shapes, pose_guider_param_shapes, refer_emb_shapes,
+                     referencenet_param_shapes, unet_param_shapes, vae_decoder_param_shapes, vae_encoder_param_shapes)
 
 _BRANCH_OUT = ("conv2.weight", "proj_out.weight", "to_out.0.weight", "ff.net.2.weight", "conv4.3.weight")
 # the ControlNet's zero-initialised convolutions (controlnet.py:97-99,425-444) are drawn non-zero for the same reason
@@ -182,3 +182,35 @@ def make_text_encoder(width: int = 64, seed: int = 0) -> torch.nn.Module:
 def make_vae_images(frames: int, H: int, W: int, seed: int = 2469, channels: int = 3) -> torch.Tensor:
     """Seeded images in [-1, 1], what `prepare_image` hands to `vae.encode`: [frames, channels, H, W] fp32."""
     return torch.rand(frames, channels, H, W, generator=torch.Generator().manual_seed(seed)) * 2 - 1
+
+
+def make_pose_guider_state_dict(cfg: PoseGuiderConfig, seed: int = 0, dtype: torch.dtype = torch.float32,
+                                bias_scale: float = 0.05) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded weights for a `PoseGuider` (musev/models/controlnet.py:326-359), one generator per name as in `make_state_dict`.
+    Every convolution is drawn with unit gain (std 1 / sqrt(fan_in)) and biases with std `bias_scale`. The reference
+    zero-initialises `conv_out` (`zero_module`, :352-359); it is drawn non-zero here, otherwise every output is zero and a
+    parity test could not see anything."""
+    sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+    for name, shape in pose_guider_param_shapes(cfg).items():
+        g = _gen(seed, "pose_guider." + name)
+        if len(shape) == 1:
+            t = torch.randn(shape, generator=g) * bias_scale
+        else:
+            t = torch.randn(shape, generator=g) / (shape[1] * 9) ** 0.5
+        sd[name] = t.to(dtype)
+    return sd
+
+
+def make_pose_images(frames: int, H: int, W: int, seed: int = 1717, channels: int = 3) -> torch.Tensor:
+    """Seeded condition images in [0, 1] (what the pipeline's control-image processor hands the pose guider): [frames,
+    channels, H, W] fp32, smooth enough that the stride-2 layers see structure rather than white noise."""
+    g = torch.Generator().manual_seed(seed)
+    lo = torch.rand(frames, channels, max(1, H // 8), max(1, W // 8), generator=g)
+    hi = torch.rand(frames, channels, H, W, generator=g)
+    up = torch.nn.functional.interpolate(lo, size=(H, W), mode="bilinear", align_corners=False)
+    return (0.75 * up + 0.25 * hi).clamp(0, 1)
+
+
+def make_pose_guider_emb(frames: int, channels: int, h: int, w: int, seed: int = 5151, scale: float = 0.5) -> torch.Tensor:
+    """A seeded stand-in for the UNet's `pose_guider_emb`: [(b t), channels, h, w] fp32."""
+    return torch.randn(frames, channels, h, w, generator=torch.Generator().manual_seed(seed)) * scale

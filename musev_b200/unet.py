@@ -50,6 +50,7 @@ class MvbUnetArgs(C.Structure):
         ("mid_residual", C.c_void_p), ("residual_is_f32", C.c_int),
         ("skip_temporal_layers", C.c_int),
         ("out", C.c_void_p), ("out_is_f32", C.c_int),
+        ("pose_guider_emb", C.c_void_p), ("pose_is_f32", C.c_int),
     ]
 
 
@@ -155,6 +156,16 @@ def _is_f32(t: torch.Tensor) -> int:
     if t.dtype == torch.float16:
         return 0
     raise ValueError(f"musev_b200 takes float16 or float32 tensors, got {t.dtype}")
+
+
+def check_pose_guider_emb(emb: torch.Tensor, B: int, T: int, c0: int, H: int, W: int) -> None:
+    """`pose_guider_emb` is added to conv_in's output (unet_3d_condition.py:1011-1016): (b t) c h w over every frame of the
+    sample, vision-condition frames included, fp16 or fp32. Raises ValueError otherwise."""
+    want = (B * T, c0, H, W)
+    if tuple(emb.shape) != want:
+        raise ValueError(f"pose_guider_emb must be (b t) c h w = {want}, got {tuple(emb.shape)}")
+    if emb.dtype not in (torch.float16, torch.float32):
+        raise ValueError(f"pose_guider_emb must be float16 or float32, got {emb.dtype}")
 
 
 def _contiguous_index_range(idx, name) -> Tuple[int, int]:
@@ -305,8 +316,7 @@ class UNet3DConditionModel:
             raise RuntimeError("weights not loaded: call load_state_dict first")
         for name, v in (("class_labels", class_labels), ("timestep_cond", timestep_cond), ("attention_mask", attention_mask),
                         ("frame_index", frame_index), ("refer_self_attn_emb", refer_self_attn_emb),
-                        ("face_emb", face_emb), ("ip_adapter_face_emb", ip_adapter_face_emb),
-                        ("pose_guider_emb", pose_guider_emb)):
+                        ("face_emb", face_emb), ("ip_adapter_face_emb", ip_adapter_face_emb)):
             if v is not None:
                 raise NotImplementedError(f"musev_b200: `{name}` is not used by the released presets and is not supported")
         if skip_temporal_layers is not None:
@@ -376,6 +386,11 @@ class UNet3DConditionModel:
             keep.append(mres)
             a.residual_is_f32 = _is_f32(mres)
             a.mid_residual = mres.data_ptr()
+        if pose_guider_emb is not None:
+            check_pose_guider_emb(pose_guider_emb, B, T, self.cfg.block_out_channels[0], H, W)
+            pose = pose_guider_emb.to(dev).contiguous()
+            keep.append(pose)
+            a.pose_guider_emb, a.pose_is_f32 = pose.data_ptr(), _is_f32(pose)
         a.skip_temporal_layers = int(self.skip_temporal_layers)
         out = torch.empty((B, self.cfg.out_channels, T, H, W), dtype=sample.dtype, device=dev)
         a.out, a.out_is_f32 = out.data_ptr(), _is_f32(out)

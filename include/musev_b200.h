@@ -217,7 +217,8 @@ typedef struct mvb_unet_args {
 int mvb_create(const mvb_config* cfg, int device, mvb_handle** out);
 void mvb_destroy(mvb_handle* h);
 /* Reference: from_pretrained_2d / load_state_dict (unet_3d_condition.py:1284-1637): feed every tensor of the
- * reference state_dict by its reference name; the library packs it into its kernel layout on the device. */
+ * reference state_dict by its reference name; the library packs it into its kernel layout on the device. Synchronous, like
+ * mvb_load_weights below (one entry of it): the source may be freed on return. */
 int mvb_load_weight(mvb_handle* h, const char* name, const void* device_ptr, int is_f32, const long long* shape, int ndim);
 /* Batched form (the `mvb_load_weights(h, const mvb_named_tensor*, n)` of SURVEY.md 8b): every entry is validated, then the
  * whole batch is packed by one kernel launch; synchronous (the sources may be freed on return). Entries not in a batch can

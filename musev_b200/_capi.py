@@ -1,8 +1,15 @@
-"""ctypes binding of include/musev_b200.h. There is no fallback: if the library is missing, loading raises."""
+"""ctypes binding of include/musev_b200.h. There is no fallback: if the library is missing, loading raises.
+
+Also the host side every whole-model wrapper shares (`EngineModel`): one engine handle, its weights by reference names,
+the workspace and the launch."""
 from __future__ import annotations
 
 import ctypes as C
 import os
+from types import SimpleNamespace
+from typing import Dict, Iterable, Optional, Sequence, Tuple
+
+import torch
 
 from .build import LIB_PATH
 
@@ -43,6 +50,71 @@ class AttentionDesc(C.Structure):
     ]
 
 
+class MvbConfig(C.Structure):
+    _fields_ = [
+        ("in_channels", C.c_int), ("out_channels", C.c_int), ("num_blocks", C.c_int),
+        ("block_out_channels", C.c_int * 4), ("layers_per_block", C.c_int), ("heads", C.c_int),
+        ("cross_attention_dim", C.c_int), ("norm_num_groups", C.c_int), ("norm_eps", C.c_float),
+        ("need_transformer_in", C.c_int), ("use_anivv1_cfg", C.c_int), ("resnet_2d_skip_time_act", C.c_int),
+        ("keep_vision_condtion", C.c_int), ("need_refer_emb", C.c_int), ("ip_adapter_cross_attn", C.c_int),
+        ("need_t2i_ip_adapter", C.c_int),
+    ]
+
+
+MAX_REFER = 16
+
+
+class MvbUnetArgs(C.Structure):
+    _fields_ = [
+        ("sample", C.c_void_p), ("sample_is_f32", C.c_int),
+        ("B", C.c_int), ("T", C.c_int), ("H", C.c_int), ("W", C.c_int),
+        ("timestep", C.c_float),
+        ("encoder_hidden_states", C.c_void_p), ("ehs_is_f32", C.c_int), ("n_text", C.c_int),
+        ("has_sample_index", C.c_int),
+        ("n_vis_cond", C.c_int), ("vis_cond_first", C.c_int),
+        ("sample_frame_rate", C.c_float),
+        ("vision_clip_emb", C.c_void_p), ("clip_is_f32", C.c_int), ("n_clip", C.c_int), ("ip_adapter_scale", C.c_float),
+        ("n_refer", C.c_int),
+        ("refer_embs", C.c_void_p * MAX_REFER), ("refer_t", C.c_int * MAX_REFER), ("refer_h", C.c_int * MAX_REFER),
+        ("refer_w", C.c_int * MAX_REFER),
+        ("mid_refer_emb", C.c_void_p), ("mid_refer_t", C.c_int), ("mid_refer_h", C.c_int), ("mid_refer_w", C.c_int),
+        ("refer_is_f32", C.c_int),
+        ("n_down_residuals", C.c_int), ("down_residuals", C.c_void_p * MAX_REFER),
+        ("mid_residual", C.c_void_p), ("residual_is_f32", C.c_int),
+        ("skip_temporal_layers", C.c_int),
+        ("out", C.c_void_p), ("out_is_f32", C.c_int),
+        ("pose_guider_emb", C.c_void_p), ("pose_is_f32", C.c_int),
+    ]
+
+
+class MvbNamedTensor(C.Structure):
+    _fields_ = [("name", C.c_char_p), ("device_ptr", C.c_void_p), ("is_f32", C.c_int), ("ndim", C.c_int),
+                ("shape", C.c_longlong * 5)]
+
+
+MAX_OUT = 13
+
+
+class MvbControlnetArgs(C.Structure):
+    _fields_ = [
+        ("sample", C.c_void_p), ("sample_is_f32", C.c_int),
+        ("NF", C.c_int), ("H", C.c_int), ("W", C.c_int),
+        ("timestep", C.c_float),
+        ("encoder_hidden_states", C.c_void_p), ("ehs_is_f32", C.c_int), ("n_text", C.c_int),
+        ("cond_latents", C.c_void_p), ("cond_is_f32", C.c_int),
+        ("n_out", C.c_int),
+        ("scales", C.c_float * MAX_OUT),
+        ("outs", C.c_void_p * MAX_OUT),
+        ("out_is_f32", C.c_int),
+        ("out_frames", C.c_int),
+    ]
+
+
+class MvbVaeDecodeArgs(C.Structure):
+    _fields_ = [("latents", C.c_void_p), ("latents_is_f32", C.c_int), ("N", C.c_int), ("h", C.c_int), ("w", C.c_int),
+                ("latent_scale", C.c_float), ("out", C.c_void_p), ("out_is_f32", C.c_int), ("postprocess", C.c_int)]
+
+
 def lib() -> C.CDLL:
     """Load libmusevb200.so (built in-tree by musev_b200.build). Raises if it is not there."""
     global _lib
@@ -51,13 +123,18 @@ def lib() -> C.CDLL:
             raise MvbError(
                 f"{LIB_PATH} not found: build it with `python -m musev_b200.build` "
                 "(musev_b200 has no CPU or PyTorch fallback)")
-        _lib = C.CDLL(LIB_PATH)
-        _lib.mvb_last_error.restype = C.c_char_p
-        _declare(_lib)
+        l = C.CDLL(LIB_PATH)
+        _declare(l)
+        _lib = l
     return _lib
 
 
 def _declare(l: C.CDLL) -> None:
+    def fn(name, restype, *argtypes):
+        f = getattr(l, name)
+        f.restype, f.argtypes = restype, list(argtypes)
+
+    l.mvb_last_error.restype = C.c_char_p
     l.mvb_version.restype = C.c_int
     l.mvb_op_conv_gemm.argtypes = [C.POINTER(ConvGemmDesc), C.c_void_p]
     l.mvb_op_conv_gemm.restype = C.c_int
@@ -100,6 +177,29 @@ def _declare(l: C.CDLL) -> None:
     l.mvb_profile_enable.restype = None
     l.mvb_profile_collect.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_longlong)]
     l.mvb_profile_collect.restype = C.c_int
+    # whole-model handles
+    H, I, LL, P = C.c_void_p, C.c_int, C.c_longlong, C.POINTER
+    for create in ("mvb_create", "mvb_create_controlnet", "mvb_create_referencenet", "mvb_create_vae_decoder",
+                   "mvb_create_vae_encoder", "mvb_create_pose_guider"):
+        fn(create, I, P(MvbConfig), I, P(C.c_void_p))
+    fn("mvb_destroy", None, H)
+    fn("mvb_load_weight", I, H, C.c_char_p, C.c_void_p, I, P(LL), I)
+    fn("mvb_load_weights", I, H, P(MvbNamedTensor), I)
+    fn("mvb_finalize", I, H)
+    fn("mvb_num_params", I, H)
+    fn("mvb_handle_error", C.c_char_p, H)
+    fn("mvb_debug_num_taps", I, H)
+    fn("mvb_debug_tap", I, H, I, C.c_char_p, I, P(C.c_void_p), P(LL), P(I))
+    fn("mvb_unet_merge_lora", I, H, P(MvbNamedTensor), P(MvbNamedTensor), P(C.c_float), I, I)
+    fn("mvb_debug_read_weight", I, H, C.c_char_p, C.c_void_p)
+    for ws, run, args in (("mvb_workspace_bytes", "mvb_unet_forward", MvbUnetArgs),
+                          ("mvb_controlnet_workspace_bytes", "mvb_controlnet_forward", MvbControlnetArgs),
+                          ("mvb_referencenet_workspace_bytes", "mvb_referencenet_forward", MvbControlnetArgs),
+                          ("mvb_vae_decode_workspace_bytes", "mvb_vae_decode", MvbVaeDecodeArgs),
+                          ("mvb_vae_encode_workspace_bytes", "mvb_vae_encode", MvbVaeDecodeArgs),
+                          ("mvb_pose_guider_workspace_bytes", "mvb_pose_guider_forward", MvbVaeDecodeArgs)):
+        fn(ws, LL, H, P(args))
+        fn(run, I, H, P(args), C.c_void_p, LL, C.c_void_p)
 
 
 def check(rc: int) -> None:
@@ -130,3 +230,188 @@ def profile_collect():
     n = (C.c_longlong * 6)()
     check(lib().mvb_profile_collect(ms, n))
     return {c: dict(ms=ms[i], launches=int(n[i])) for i, c in enumerate(CATEGORIES)}
+
+
+def _is_f32(t: torch.Tensor) -> int:
+    if t.dtype == torch.float32:
+        return 1
+    if t.dtype == torch.float16:
+        return 0
+    raise ValueError(f"musev_b200 takes float16 or float32 tensors, got {t.dtype}")
+
+
+def _named(name: str, t: torch.Tensor) -> MvbNamedTensor:
+    e = MvbNamedTensor()
+    e.name, e.device_ptr, e.is_f32, e.ndim = name.encode(), t.data_ptr(), _is_f32(t), t.dim()
+    for i, v in enumerate(t.shape):
+        e.shape[i] = v
+    return e
+
+
+PACK_BATCH_BYTES = 512 << 20     # source bytes staged on the device per mvb_load_weights call
+
+
+def load_weights_batched(handle, named_tensors: Iterable[Tuple[str, torch.Tensor]], device) -> None:
+    """Feeds (name, tensor) pairs to `mvb_load_weights` in batches of ~PACK_BATCH_BYTES: one host->device staging copy
+    per tensor, ONE packing kernel per batch."""
+    l = lib()
+    batch, keep, nbytes = [], [], 0
+
+    def flush():
+        nonlocal batch, keep, nbytes
+        if not batch:
+            return
+        arr = (MvbNamedTensor * len(batch))(*batch)
+        rc = l.mvb_load_weights(handle, arr, len(batch))
+        if rc != 0:
+            raise MvbError(f"mvb_load_weights: {l.mvb_handle_error(handle).decode()}")
+        batch, keep, nbytes = [], [], 0
+
+    for name, t in named_tensors:
+        if t.dtype not in (torch.float16, torch.float32):
+            t = t.float()
+        t = t.to(device).contiguous()
+        batch.append(_named(name, t))
+        keep.append(t)
+        nbytes += t.numel() * t.element_size()
+        if nbytes >= PACK_BATCH_BYTES:
+            torch.cuda.current_stream(device).synchronize()
+            flush()
+    torch.cuda.current_stream(device).synchronize()
+    flush()
+
+
+def make_config(in_channels: int, out_channels: int, block_out_channels: Sequence[int], layers_per_block: int = 0,
+                heads: int = 0, cross_attention_dim: int = 0, norm_num_groups: int = 0, norm_eps: float = 0.0,
+                **switches) -> MvbConfig:
+    """An `mvb_config`; `switches` are the int flags of the UNet (`need_transformer_in`, ...)."""
+    c = MvbConfig()
+    c.in_channels, c.out_channels, c.num_blocks = in_channels, out_channels, len(block_out_channels)
+    for i, v in enumerate(block_out_channels):
+        c.block_out_channels[i] = v
+    c.layers_per_block, c.heads = layers_per_block, heads
+    c.cross_attention_dim, c.norm_num_groups, c.norm_eps = cross_attention_dim, norm_num_groups, norm_eps
+    for k, v in switches.items():
+        setattr(c, k, int(v))
+    return c
+
+
+class EngineModel:
+    """One engine handle behind a reference model's call surface: creation, weights by reference state-dict names,
+    `.eval()`, `.to()`, and the grow-only workspace every call runs in. A subclass names its C entry points and
+    gives the expected parameter shapes."""
+
+    _create = ""              # mvb_create_* of the model kind
+    _workspace = ""           # its *_workspace_bytes
+    _forward = ""             # its forward
+    _ignored: Tuple[str, ...] = ()   # state-dict prefixes of other models, skipped by load_state_dict
+
+    def __init__(self, config: MvbConfig, device, dtype: torch.dtype, unsupported: str = "unsupported configuration"):
+        if not torch.cuda.is_available():
+            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
+        self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
+        self.dtype = dtype
+        self._ws: Optional[torch.Tensor] = None
+        self._h = C.c_void_p()
+        self._loaded = False
+        rc = getattr(lib(), self._create)(C.byref(config), self.device.index or 0, C.byref(self._h))
+        if rc != 0:
+            raise MvbError(f"{self._create} failed ({rc}): {unsupported} or out of device memory")
+
+    def _error(self) -> str:
+        return lib().mvb_handle_error(self._h).decode()
+
+    def _param_shapes(self) -> Dict[str, Tuple[int, ...]]:
+        raise NotImplementedError
+
+    def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = True):
+        """Checks names and shapes against the schema, then packs the tensors on the device in batches (peak extra memory
+        = one ~512 MB staging batch)."""
+        expected = self._param_shapes()
+        missing = [k for k in expected if k not in state_dict]
+        unexpected = [k for k in state_dict if k not in expected and not k.startswith(self._ignored)]
+        if strict and (missing or unexpected):
+            raise RuntimeError(f"Error(s) in loading state_dict: missing {missing[:5]} unexpected {unexpected[:5]}")
+        todo = []
+        for name, shape in expected.items():
+            if name not in state_dict:
+                continue
+            t = state_dict[name]
+            if tuple(t.shape) != tuple(shape):
+                raise RuntimeError(f"size mismatch for {name}: {tuple(t.shape)} vs {tuple(shape)}")
+            todo.append((name, t))
+        self._load(todo)
+        return SimpleNamespace(missing_keys=missing, unexpected_keys=unexpected)
+
+    def _load(self, todo: Sequence[Tuple[str, torch.Tensor]]) -> None:
+        load_weights_batched(self._h, todo, self.device)
+        if lib().mvb_finalize(self._h) != 0:
+            raise MvbError(f"mvb_finalize: {self._error()}")
+        self._loaded = True
+
+    def _check_loaded(self) -> None:
+        if not self._loaded:
+            raise RuntimeError("weights not loaded: call load_state_dict first")
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) and self._h.value:
+                lib().mvb_destroy(self._h)
+                self._h = C.c_void_p()
+        except Exception:
+            pass
+
+    def eval(self):
+        return self
+
+    def to(self, *args, **kwargs):
+        for a in list(args) + list(kwargs.values()):
+            if isinstance(a, torch.dtype):
+                if a not in (torch.float16, torch.float32):
+                    raise ValueError("musev_b200 computes in fp16 with fp32 accumulation; I/O dtype is fp16 or fp32")
+                self.dtype = a
+            elif isinstance(a, (str, torch.device)) and torch.device(a).type != "cuda":
+                raise RuntimeError("musev_b200 has no CPU path")
+        return self
+
+    def _launch(self, args: C.Structure) -> None:
+        """One forward on the current stream of the model's device, in the handle's workspace (grown when too small)."""
+        l = lib()
+        need = getattr(l, self._workspace)(self._h, C.byref(args))
+        if need < 0:
+            raise MvbError(f"{self._workspace}: {self._error()}")
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = None
+            self._ws = torch.empty(int(need), dtype=torch.uint8, device=self.device)
+        rc = getattr(l, self._forward)(self._h, C.byref(args), self._ws.data_ptr(), self._ws.numel(),
+                                       torch.cuda.current_stream(self.device).cuda_stream)
+        if rc != 0:
+            raise MvbError(f"{self._forward} ({rc}): {self._error()}")
+
+    def _launch_frames(self, x: torch.Tensor, out: torch.Tensor, h: int, w: int, latent_scale: float,
+                       postprocess: int) -> torch.Tensor:
+        """Runs an `mvb_vae_decode_args` model on x [N, ...] -> out [N, ...] in chunks of `frames_per_call` frames (bounds
+        the activation workspace); h, w = the size the model's entry point documents."""
+        step = max(1, self.frames_per_call)
+        for n0 in range(0, x.shape[0], step):
+            xc, oc = x[n0:n0 + step], out[n0:n0 + step]
+            a = MvbVaeDecodeArgs()
+            a.latents, a.latents_is_f32 = xc.data_ptr(), _is_f32(xc)
+            a.N, a.h, a.w = xc.shape[0], h, w
+            a.latent_scale = float(latent_scale)
+            a.out, a.out_is_f32 = oc.data_ptr(), _is_f32(oc)
+            a.postprocess = int(postprocess)
+            self._launch(a)
+        self._keep = x   # the input must outlive the asynchronous launches
+        return out
+
+    def debug_weight(self, name: str) -> torch.Tensor:
+        """The packed matrix / convolution weight `name` read back into its reference shape, fp16 on the device."""
+        shape = self._param_shapes().get(name)
+        if shape is None or len(shape) < 2:
+            raise ValueError(f"{name} is not a matrix or convolution weight of this model")
+        out = torch.empty(shape, dtype=torch.float16, device=self.device)
+        rc = lib().mvb_debug_read_weight(self._h, name.encode(), out.data_ptr())
+        if rc != 0:
+            raise MvbError(f"mvb_debug_read_weight ({rc}): {self._error()}")
+        return out

@@ -13,7 +13,6 @@ pipeline call on the pose images (`mvb_pose_guider_forward`, `Engine::run_pose_g
 """
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import asdict
 from types import SimpleNamespace
 from typing import Any, Dict, List, Optional, Tuple, Union
@@ -21,80 +20,29 @@ from typing import Any, Dict, List, Optional, Tuple, Union
 import torch
 import torch.nn.functional as F
 
-from . import _capi
+from ._capi import EngineModel, MvbControlnetArgs, _is_f32, make_config
+# Names callers imported from this module before the binding moved to _capi; they are the binding's own objects.
+from ._capi import lib as _lib  # noqa: F401
 from .schema import ControlNetConfig, PoseGuiderConfig, controlnet_param_shapes, pose_guider_param_shapes
-from .unet import MvbConfig, _is_f32, _lib as _unet_lib, load_weights_batched
-from .vae import MvbVaeDecodeArgs
-
-MAX_OUT = 13
-
-
-class MvbControlnetArgs(C.Structure):
-    _fields_ = [
-        ("sample", C.c_void_p), ("sample_is_f32", C.c_int),
-        ("NF", C.c_int), ("H", C.c_int), ("W", C.c_int),
-        ("timestep", C.c_float),
-        ("encoder_hidden_states", C.c_void_p), ("ehs_is_f32", C.c_int), ("n_text", C.c_int),
-        ("cond_latents", C.c_void_p), ("cond_is_f32", C.c_int),
-        ("n_out", C.c_int),
-        ("scales", C.c_float * MAX_OUT),
-        ("outs", C.c_void_p * MAX_OUT),
-        ("out_is_f32", C.c_int),
-        ("out_frames", C.c_int),
-    ]
-
-
-_declared = False
-
-
-def _lib():
-    global _declared
-    l = _unet_lib()
-    if not _declared:
-        l.mvb_create_controlnet.argtypes = [C.POINTER(MvbConfig), C.c_int, C.POINTER(C.c_void_p)]
-        l.mvb_create_controlnet.restype = C.c_int
-        l.mvb_controlnet_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(MvbControlnetArgs)]
-        l.mvb_controlnet_workspace_bytes.restype = C.c_longlong
-        l.mvb_controlnet_forward.argtypes = [C.c_void_p, C.POINTER(MvbControlnetArgs), C.c_void_p, C.c_longlong, C.c_void_p]
-        l.mvb_controlnet_forward.restype = C.c_int
-        l.mvb_create_pose_guider.argtypes = [C.POINTER(MvbConfig), C.c_int, C.POINTER(C.c_void_p)]
-        l.mvb_create_pose_guider.restype = C.c_int
-        l.mvb_pose_guider_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(MvbVaeDecodeArgs)]
-        l.mvb_pose_guider_workspace_bytes.restype = C.c_longlong
-        l.mvb_pose_guider_forward.argtypes = [C.c_void_p, C.POINTER(MvbVaeDecodeArgs), C.c_void_p, C.c_longlong, C.c_void_p]
-        l.mvb_pose_guider_forward.restype = C.c_int
-        _declared = True
-    return l
 
 
 class ControlNetOutput(SimpleNamespace):
     """diffusers models/controlnet.py:46-61."""
 
 
-class ControlNetModel:
+class ControlNetModel(EngineModel):
     """CUDA engine behind the call surface of diffusers `ControlNetModel` (models/controlnet.py:114)."""
 
+    _create, _workspace, _forward = "mvb_create_controlnet", "mvb_controlnet_workspace_bytes", "mvb_controlnet_forward"
+    _COND = "controlnet_cond_embedding."
+
     def __init__(self, config: ControlNetConfig, device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16):
-        if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.cfg = config
-        self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
-        self.dtype = dtype
         self.config = SimpleNamespace(**asdict(config), global_pool_conditions=False)
-        self._ws: Optional[torch.Tensor] = None
-        self._h = C.c_void_p()
-        self._loaded = False
         self._cond_w: Dict[str, torch.Tensor] = {}
-        c = MvbConfig()
-        c.in_channels, c.out_channels = config.in_channels, config.in_channels
-        c.num_blocks = len(config.block_out_channels)
-        for i, v in enumerate(config.block_out_channels):
-            c.block_out_channels[i] = v
-        c.layers_per_block, c.heads = config.layers_per_block, config.attention_head_dim
-        c.cross_attention_dim, c.norm_num_groups, c.norm_eps = config.cross_attention_dim, config.norm_num_groups, config.norm_eps
-        rc = _lib().mvb_create_controlnet(C.byref(c), self.device.index or 0, C.byref(self._h))
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_create_controlnet failed ({rc}): unsupported configuration or out of device memory")
+        c = make_config(config.in_channels, config.in_channels, config.block_out_channels, config.layers_per_block,
+                        config.attention_head_dim, config.cross_attention_dim, config.norm_num_groups, config.norm_eps)
+        super().__init__(c, device, dtype)
         # residual map geometry: (channels, downscale) of the 12 + 1 outputs (controlnet.py:788-823)
         self._maps: List[Tuple[int, int]] = [(config.block_out_channels[0], 1)]
         ds = 1
@@ -114,51 +62,13 @@ class ControlNetModel:
         m.load_state_dict(state_dict)
         return m
 
-    def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = True):
-        expected = controlnet_param_shapes(self.cfg)
-        missing = [k for k in expected if k not in state_dict]
-        unexpected = [k for k in state_dict if k not in expected]
-        if strict and (missing or unexpected):
-            raise RuntimeError(f"Error(s) in loading state_dict: missing {missing[:5]} unexpected {unexpected[:5]}")
-        l = _lib()
-        todo = []
-        for name, shape in expected.items():
-            if name not in state_dict:
-                continue
-            t = state_dict[name]
-            if tuple(t.shape) != tuple(shape):
-                raise RuntimeError(f"size mismatch for {name}: {tuple(t.shape)} vs {tuple(shape)}")
-            if name.startswith("controlnet_cond_embedding."):
-                self._cond_w[name] = t.to(self.device, self.dtype).contiguous()
-                continue
-            todo.append((name, t))
-        load_weights_batched(self._h, todo, self.device)
-        rc = l.mvb_finalize(self._h)
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_finalize: {l.mvb_handle_error(self._h).decode()}")
-        self._loaded = True
-        return SimpleNamespace(missing_keys=missing, unexpected_keys=unexpected)
+    def _param_shapes(self):
+        return controlnet_param_shapes(self.cfg)
 
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) and self._h.value:
-                _lib().mvb_destroy(self._h)
-                self._h = C.c_void_p()
-        except Exception:
-            pass
-
-    def eval(self):
-        return self
-
-    def to(self, *args, **kwargs):
-        for a in list(args) + list(kwargs.values()):
-            if isinstance(a, torch.dtype):
-                if a not in (torch.float16, torch.float32):
-                    raise ValueError("musev_b200 computes in fp16 with fp32 accumulation; I/O dtype is fp16 or fp32")
-                self.dtype = a
-            elif isinstance(a, (str, torch.device)) and torch.device(a).type != "cuda":
-                raise RuntimeError("musev_b200 has no CPU path")
-        return self
+    def _load(self, todo):
+        # the conditioning embedding stays a torch conv stack (module docstring); the engine takes the rest
+        self._cond_w.update({n: t.to(self.device, self.dtype).contiguous() for n, t in todo if n.startswith(self._COND)})
+        super()._load([(n, t) for n, t in todo if not n.startswith(self._COND)])
 
     # ------------------------------------------------------------------ one-shot conditioning embedding
     @torch.no_grad()
@@ -192,8 +102,7 @@ class ControlNetModel:
         controlnet_cond_latents: Optional[torch.Tensor] = None,
     ):
         """Reference: ControlNetModel.forward, diffusers models/controlnet.py:645-852."""
-        if not self._loaded:
-            raise RuntimeError("weights not loaded: call load_state_dict first")
+        self._check_loaded()
         for name, v in (("class_labels", class_labels), ("timestep_cond", timestep_cond), ("attention_mask", attention_mask),
                         ("added_cond_kwargs", added_cond_kwargs)):
             if v is not None:
@@ -232,17 +141,7 @@ class ControlNetModel:
             a.scales[k] = scales[k]
             a.outs[k] = outs[k].data_ptr()
         a.out_is_f32 = _is_f32(outs[0])
-        l = _lib()
-        need = l.mvb_controlnet_workspace_bytes(self._h, C.byref(a))
-        if need < 0:
-            raise _capi.MvbError(f"mvb_controlnet_workspace_bytes: {l.mvb_handle_error(self._h).decode()}")
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = None
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        rc = l.mvb_controlnet_forward(self._h, C.byref(a), self._ws.data_ptr(), self._ws.numel(),
-                                      torch.cuda.current_stream().cuda_stream)
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_controlnet_forward: {l.mvb_handle_error(self._h).decode()}")
+        self._launch(a)
         down, mid = outs[:-1], outs[-1]
         if not return_dict:
             return (down, mid)
@@ -271,7 +170,7 @@ def check_pose_guider_state_dict(cfg: PoseGuiderConfig, state_dict: Dict[str, to
     return todo, unexpected
 
 
-class PoseGuider:
+class PoseGuider(EngineModel):
     """CUDA engine behind the call surface of `musev.models.controlnet.PoseGuider` (musev/models/controlnet.py:326-399).
 
     Kept: the constructor arguments, `from_pretrained(path, conditioning_embedding_channels, conditioning_channels,
@@ -280,30 +179,18 @@ class PoseGuider:
     Departure: the reference loads with `strict=False` and keeps its initialiser's values for a missing key; the engine
     has no initialiser, so a missing key raises, naming it. Unexpected keys are ignored when `strict=False`."""
 
+    _create, _workspace, _forward = "mvb_create_pose_guider", "mvb_pose_guider_workspace_bytes", "mvb_pose_guider_forward"
+
     def __init__(self, conditioning_embedding_channels: int, conditioning_channels: int = 3,
                  block_out_channels: Tuple[int, ...] = (16, 32, 64, 128), device: Union[str, torch.device] = "cuda",
                  dtype: torch.dtype = torch.float16, frames_per_call: int = 8):
-        if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.cfg = PoseGuiderConfig(int(conditioning_embedding_channels), int(conditioning_channels), tuple(block_out_channels))
         self.config = SimpleNamespace(**asdict(self.cfg))
-        self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
-        self.dtype = dtype
         self.frames_per_call = int(frames_per_call)
-        self._ws: Optional[torch.Tensor] = None
-        self._h = C.c_void_p()
-        self._loaded = False
-        c = MvbConfig()
-        c.in_channels, c.out_channels = self.cfg.conditioning_channels, self.cfg.conditioning_embedding_channels
-        c.num_blocks = len(self.cfg.block_out_channels)
-        if not 1 <= c.num_blocks <= 4:
+        if not 1 <= len(self.cfg.block_out_channels) <= 4:
             raise ValueError(f"block_out_channels must have 1..4 entries, got {self.cfg.block_out_channels}")
-        for i, v in enumerate(self.cfg.block_out_channels):
-            c.block_out_channels[i] = v
-        rc = _lib().mvb_create_pose_guider(C.byref(c), self.device.index or 0, C.byref(self._h))
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_create_pose_guider failed ({rc}): unsupported channel counts {self.cfg} "
-                                 "or out of device memory")
+        c = make_config(self.cfg.conditioning_channels, self.cfg.conditioning_embedding_channels, self.cfg.block_out_channels)
+        super().__init__(c, device, dtype, unsupported=f"unsupported channel counts {self.cfg}")
 
     @classmethod
     def from_pretrained(cls, pretrained_model_path, conditioning_embedding_channels: int, conditioning_channels: int = 3,
@@ -314,42 +201,18 @@ class PoseGuider:
         m.load_state_dict(state_dict, strict=False)
         return m
 
+    def _param_shapes(self):
+        return pose_guider_param_shapes(self.cfg)
+
     def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = True):
         todo, unexpected = check_pose_guider_state_dict(self.cfg, state_dict, strict)
-        load_weights_batched(self._h, todo, self.device)
-        l = _lib()
-        rc = l.mvb_finalize(self._h)
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_finalize: {l.mvb_handle_error(self._h).decode()}")
-        self._loaded = True
+        self._load(todo)
         return SimpleNamespace(missing_keys=[], unexpected_keys=unexpected)
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) and self._h.value:
-                _lib().mvb_destroy(self._h)
-                self._h = C.c_void_p()
-        except Exception:
-            pass
-
-    def eval(self):
-        return self
-
-    def to(self, *args, **kwargs):
-        for a in list(args) + list(kwargs.values()):
-            if isinstance(a, torch.dtype):
-                if a not in (torch.float16, torch.float32):
-                    raise ValueError("musev_b200 computes in fp16 with fp32 accumulation; I/O dtype is fp16 or fp32")
-                self.dtype = a
-            elif isinstance(a, (str, torch.device)) and torch.device(a).type != "cuda":
-                raise RuntimeError("musev_b200 has no CPU path")
-        return self
 
     @torch.no_grad()
     def embed_frames(self, images: torch.Tensor, out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
         """images [N, c, H, W] (fp16 / fp32, frames on the batch axis) -> [N, emb, H / 2^(nb-1), W / 2^(nb-1)]."""
-        if not self._loaded:
-            raise RuntimeError("weights not loaded: call load_state_dict first")
+        self._check_loaded()
         f = 2 ** (len(self.cfg.block_out_channels) - 1)
         if images.dim() != 4 or images.shape[1] != self.cfg.conditioning_channels:
             raise ValueError(f"conditioning must have {self.cfg.conditioning_channels} channels, got {tuple(images.shape)}")
@@ -362,29 +225,7 @@ class PoseGuider:
         x = x.contiguous()
         h, w = H // f, W // f
         out = torch.empty((N, self.cfg.conditioning_embedding_channels, h, w), dtype=out_dtype or self.dtype, device=self.device)
-        l = _lib()
-        step = max(1, self.frames_per_call)
-        for n0 in range(0, N, step):
-            n1 = min(N, n0 + step)
-            xc, oc = x[n0:n1], out[n0:n1]
-            a = MvbVaeDecodeArgs()
-            a.latents, a.latents_is_f32 = xc.data_ptr(), _is_f32(xc)
-            a.N, a.h, a.w = n1 - n0, h, w
-            a.latent_scale = 1.0
-            a.out, a.out_is_f32 = oc.data_ptr(), _is_f32(oc)
-            a.postprocess = 0
-            need = l.mvb_pose_guider_workspace_bytes(self._h, C.byref(a))
-            if need < 0:
-                raise _capi.MvbError(f"mvb_pose_guider_workspace_bytes: {l.mvb_handle_error(self._h).decode()}")
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = None
-                self._ws = torch.empty(int(need), dtype=torch.uint8, device=self.device)
-            rc = l.mvb_pose_guider_forward(self._h, C.byref(a), self._ws.data_ptr(), self._ws.numel(),
-                                           torch.cuda.current_stream(self.device).cuda_stream)
-            if rc != 0:
-                raise _capi.MvbError(f"mvb_pose_guider_forward ({rc}): {l.mvb_handle_error(self._h).decode()}")
-        self._keep = x
-        return out
+        return self._launch_frames(x, out, h, w, 1.0, 0)
 
     @torch.no_grad()
     def forward(self, conditioning: torch.Tensor) -> torch.Tensor:

@@ -12,141 +12,33 @@ struct mvb_handle {
   mvb::Engine* e;
 };
 
-extern "C" {
-
-int mvb_create(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out) return MVB_ERR_INVALID;
-  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->heads < 1 || cfg->norm_num_groups < 1) return MVB_ERR_INVALID;
+// Validators of each model kind's mvb_config: the shapes its kernels take (MVB_ERR_INVALID otherwise)
+static bool unet_config_ok(const mvb_config* cfg) {
+  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->heads < 1 || cfg->norm_num_groups < 1) return false;
   for (int i = 0; i < cfg->num_blocks; ++i) {
     const int c = cfg->block_out_channels[i];
-    if (c % 64 || c % cfg->heads || (c / cfg->heads) % 8 || c % cfg->norm_num_groups) return MVB_ERR_INVALID;
+    if (c % 64 || c % cfg->heads || (c / cfg->heads) % 8 || c % cfg->norm_num_groups) return false;
   }
-  if (cfg->cross_attention_dim % 64 || cfg->in_channels * 9 > 64 || cfg->out_channels > 16) return MVB_ERR_INVALID;
-  mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device);
-  if (!e) return MVB_ERR_STATE;
-  if (e->error()[0]) { delete e; return MVB_ERR_CUDA; }
-  mvb_handle* h = new (std::nothrow) mvb_handle{e};
-  if (!h) { delete e; return MVB_ERR_STATE; }
-  *out = h;
-  return MVB_OK;
+  return cfg->cross_attention_dim % 64 == 0 && cfg->in_channels * 9 <= 64;
 }
 
-static int check_config(const mvb_config* cfg) {
-  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->heads < 1 || cfg->norm_num_groups < 1) return MVB_ERR_INVALID;
-  for (int i = 0; i < cfg->num_blocks; ++i) {
-    const int c = cfg->block_out_channels[i];
-    if (c % 64 || c % cfg->heads || (c / cfg->heads) % 8 || c % cfg->norm_num_groups) return MVB_ERR_INVALID;
-  }
-  if (cfg->cross_attention_dim % 64 || cfg->in_channels * 9 > 64) return MVB_ERR_INVALID;
-  return MVB_OK;
-}
-
-int mvb_create_controlnet(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out) return MVB_ERR_INVALID;
-  if (check_config(cfg) != MVB_OK) return MVB_ERR_INVALID;
+// The ControlNet / ReferenceNet encoder: the UNet's down blocks + mid block, one output map per layer
+static bool encoder_config_ok(const mvb_config* cfg) {
+  if (!unet_config_ok(cfg)) return false;
   int n_out = 2;
   for (int i = 0; i < cfg->num_blocks; ++i) n_out += cfg->layers_per_block + (i == cfg->num_blocks - 1 ? 0 : 1);
-  if (n_out > MVB_CONTROLNET_MAX_OUT) return MVB_ERR_INVALID;
-  mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, 1);
-  if (!e) return MVB_ERR_STATE;
-  if (e->error()[0]) { delete e; return MVB_ERR_CUDA; }
-  mvb_handle* h = new (std::nothrow) mvb_handle{e};
-  if (!h) { delete e; return MVB_ERR_STATE; }
-  *out = h;
-  return MVB_OK;
+  return n_out <= MVB_CONTROLNET_MAX_OUT;
 }
 
-int mvb_create_referencenet(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out) return MVB_ERR_INVALID;
-  if (check_config(cfg) != MVB_OK) return MVB_ERR_INVALID;
-  int n_out = 2;
-  for (int i = 0; i < cfg->num_blocks; ++i) n_out += cfg->layers_per_block + (i == cfg->num_blocks - 1 ? 0 : 1);
-  if (n_out > MVB_CONTROLNET_MAX_OUT) return MVB_ERR_INVALID;
-  mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, 2);
-  if (!e) return MVB_ERR_STATE;
-  if (e->error()[0]) { delete e; return MVB_ERR_CUDA; }
-  mvb_handle* h = new (std::nothrow) mvb_handle{e};
-  if (!h) { delete e; return MVB_ERR_STATE; }
-  *out = h;
-  return MVB_OK;
-}
-
-long long mvb_referencenet_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args) {
-  if (!h || !args || h->e->kind() != 2) return -1;
-  return h->e->controlnet_workspace_bytes(*args);
-}
-
-int mvb_referencenet_forward(mvb_handle* h, const mvb_controlnet_args* args, void* workspace, long long workspace_bytes,
-                             void* stream) {
-  if (!h || !args) return MVB_ERR_INVALID;
-  if (h->e->kind() != 2) return MVB_ERR_STATE;
-  return h->e->controlnet_forward(*args, workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
-long long mvb_controlnet_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args) {
-  if (!h || !args) return -1;
-  return h->e->controlnet_workspace_bytes(*args);
-}
-
-int mvb_controlnet_forward(mvb_handle* h, const mvb_controlnet_args* args, void* workspace, long long workspace_bytes,
-                           void* stream) {
-  if (!h || !args) return MVB_ERR_INVALID;
-  return h->e->controlnet_forward(*args, workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
-int mvb_create_vae_decoder(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out) return MVB_ERR_INVALID;
-  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->norm_num_groups < 1 || cfg->layers_per_block < 1) return MVB_ERR_INVALID;
+// Either VAE half: conv_in is an im2col of 9 * in_channels <= 64 columns; conv_out writes 16 padded columns, which hold
+// out_channels image channels (decoder) or 2 * out_channels moments (encoder)
+static bool vae_config_ok(const mvb_config* cfg, int max_out_channels) {
+  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->norm_num_groups < 1 || cfg->layers_per_block < 1) return false;
   for (int i = 0; i < cfg->num_blocks; ++i) {
     const int c = cfg->block_out_channels[i];
-    if (c % 64 || c % cfg->norm_num_groups || (c / cfg->norm_num_groups) % 2) return MVB_ERR_INVALID;
+    if (c % 64 || c % cfg->norm_num_groups || (c / cfg->norm_num_groups) % 2) return false;
   }
-  if (cfg->in_channels < 1 || cfg->in_channels > 7 || cfg->out_channels < 1 || cfg->out_channels > 16) return MVB_ERR_INVALID;
-  mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, 3);
-  if (!e) return MVB_ERR_STATE;
-  if (e->error()[0]) { delete e; return MVB_ERR_CUDA; }
-  mvb_handle* h = new (std::nothrow) mvb_handle{e};
-  if (!h) { delete e; return MVB_ERR_STATE; }
-  *out = h;
-  return MVB_OK;
-}
-
-long long mvb_vae_decode_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args) {
-  if (!h || !args) return -1;
-  return h->e->vae_workspace_bytes(*args);
-}
-
-int mvb_vae_decode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes, void* stream) {
-  if (!h || !args) return MVB_ERR_INVALID;
-  return h->e->vae_decode(*args, workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
-int mvb_create_vae_encoder(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out) return MVB_ERR_INVALID;
-  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->norm_num_groups < 1 || cfg->layers_per_block < 1) return MVB_ERR_INVALID;
-  for (int i = 0; i < cfg->num_blocks; ++i) {
-    const int c = cfg->block_out_channels[i];
-    if (c % 64 || c % cfg->norm_num_groups || (c / cfg->norm_num_groups) % 2) return MVB_ERR_INVALID;
-  }
-  // conv_in is an im2col of 9 * in_channels <= 64 columns; conv_out's 2 * out_channels moments fit its 16 padded columns
-  if (cfg->in_channels < 1 || cfg->in_channels > 7 || cfg->out_channels < 1 || cfg->out_channels > 8) return MVB_ERR_INVALID;
-  mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, 4);
-  if (!e) return MVB_ERR_STATE;
-  if (e->error()[0]) { delete e; return MVB_ERR_CUDA; }
-  mvb_handle* h = new (std::nothrow) mvb_handle{e};
-  if (!h) { delete e; return MVB_ERR_STATE; }
-  *out = h;
-  return MVB_OK;
-}
-
-long long mvb_vae_encode_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args) {
-  if (!h || !args) return -1;
-  return h->e->vae_encode_workspace_bytes(*args);
-}
-
-int mvb_vae_encode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes, void* stream) {
-  if (!h || !args) return MVB_ERR_INVALID;
-  return h->e->vae_encode(*args, workspace, workspace_bytes, (cudaStream_t)stream);
+  return cfg->in_channels >= 1 && cfg->in_channels <= 7 && cfg->out_channels >= 1 && cfg->out_channels <= max_out_channels;
 }
 
 // The layer split of Engine::build_pose_guider: conv_in and every layer reading 16 / 32 channels run on the small-channel
@@ -167,16 +59,90 @@ static bool pose_guider_config_ok(const mvb_config* cfg) {
   return true;
 }
 
-int mvb_create_pose_guider(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out) return MVB_ERR_INVALID;
-  if (!pose_guider_config_ok(cfg)) return MVB_ERR_INVALID;
-  mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, 5);
+// A handle of a validated configuration: MVB_ERR_STATE when out of host memory, MVB_ERR_CUDA when the device refused
+static int create(const mvb_config* cfg, int device, mvb::Kind kind, mvb_handle** out) {
+  mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, kind);
   if (!e) return MVB_ERR_STATE;
   if (e->error()[0]) { delete e; return MVB_ERR_CUDA; }
   mvb_handle* h = new (std::nothrow) mvb_handle{e};
   if (!h) { delete e; return MVB_ERR_STATE; }
   *out = h;
   return MVB_OK;
+}
+
+extern "C" {
+
+int mvb_create(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out || !unet_config_ok(cfg) || cfg->out_channels > 16) return MVB_ERR_INVALID;
+  return create(cfg, device, mvb::Kind::UNet, out);
+}
+
+int mvb_create_controlnet(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out || !encoder_config_ok(cfg)) return MVB_ERR_INVALID;
+  return create(cfg, device, mvb::Kind::ControlNet, out);
+}
+
+int mvb_create_referencenet(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out || !encoder_config_ok(cfg)) return MVB_ERR_INVALID;
+  return create(cfg, device, mvb::Kind::ReferenceNet, out);
+}
+
+long long mvb_referencenet_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args) {
+  if (!h || !args || h->e->kind() != mvb::Kind::ReferenceNet) return -1;
+  return h->e->controlnet_workspace_bytes(*args);
+}
+
+int mvb_referencenet_forward(mvb_handle* h, const mvb_controlnet_args* args, void* workspace, long long workspace_bytes,
+                             void* stream) {
+  if (!h || !args) return MVB_ERR_INVALID;
+  if (h->e->kind() != mvb::Kind::ReferenceNet) return MVB_ERR_STATE;
+  return h->e->controlnet_forward(*args, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+long long mvb_controlnet_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args) {
+  if (!h || !args) return -1;
+  return h->e->controlnet_workspace_bytes(*args);
+}
+
+int mvb_controlnet_forward(mvb_handle* h, const mvb_controlnet_args* args, void* workspace, long long workspace_bytes,
+                           void* stream) {
+  if (!h || !args) return MVB_ERR_INVALID;
+  return h->e->controlnet_forward(*args, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mvb_create_vae_decoder(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out || !vae_config_ok(cfg, 16)) return MVB_ERR_INVALID;
+  return create(cfg, device, mvb::Kind::VaeDecoder, out);
+}
+
+long long mvb_vae_decode_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args) {
+  if (!h || !args) return -1;
+  return h->e->vae_workspace_bytes(*args);
+}
+
+int mvb_vae_decode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes, void* stream) {
+  if (!h || !args) return MVB_ERR_INVALID;
+  return h->e->vae_decode(*args, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mvb_create_vae_encoder(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out || !vae_config_ok(cfg, 8)) return MVB_ERR_INVALID;
+  return create(cfg, device, mvb::Kind::VaeEncoder, out);
+}
+
+long long mvb_vae_encode_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args) {
+  if (!h || !args) return -1;
+  return h->e->vae_encode_workspace_bytes(*args);
+}
+
+int mvb_vae_encode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes, void* stream) {
+  if (!h || !args) return MVB_ERR_INVALID;
+  return h->e->vae_encode(*args, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mvb_create_pose_guider(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out || !pose_guider_config_ok(cfg)) return MVB_ERR_INVALID;
+  return create(cfg, device, mvb::Kind::PoseGuider, out);
 }
 
 long long mvb_pose_guider_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args) {

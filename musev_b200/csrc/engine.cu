@@ -7,6 +7,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+
 #include "attention.cuh"
 #include "cond_embed.cuh"
 #include "conv_gemm.cuh"
@@ -17,40 +19,6 @@ namespace mvb {
 static inline int pad16(int d) { return (d + 15) / 16 * 16; }
 
 // ---------------------------------------------------------------------------------------------- packing kernels
-template <typename TSrc>
-__global__ void pack_matrix_kernel(__half* __restrict__ dst, long long ld, int rows_dst, int kdst, const TSrc* __restrict__ src,
-                                   int nsrc, int ksrc, int rowmode, int p0, int p1, int colmode, int cin, int taps,
-                                   int cin_dst) {
-  const long long total = (long long)rows_dst * kdst;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int r = (int)(i / kdst), kk = (int)(i % kdst);
-    int srow = r;
-    if (rowmode == 1) {            // pad heads: p0 = d, p1 = dp
-      const int h = r / p1, j = r % p1;
-      srow = j < p0 ? h * p0 + j : -1;
-    } else if (rowmode == 2) {     // GEGLU: chunks of [16 value | 16 gate]
-      const int chunk = r / 32, j = r % 32;
-      srow = j < 16 ? chunk * 16 + j : rows_dst / 2 + chunk * 16 + (j - 16);
-    }
-    int scol = kk;
-    if (colmode == 1) {
-      const int cd = cin_dst > cin ? cin_dst : cin;
-      if (kk < cd * taps) { const int tap = kk / cd, c = kk % cd; scol = c < cin ? c * taps + tap : -1; } else scol = -1;
-    } else if (kk >= ksrc) scol = -1;
-    float v = 0.f;
-    if (srow >= 0 && srow < nsrc && scol >= 0) v = (float)src[(long long)srow * ksrc + scol];
-    dst[(long long)r * ld + kk] = __float2half_rn(v);
-  }
-}
-template <typename TSrc>
-__global__ void pack_vec_kernel(float* __restrict__ dst, int n, const TSrc* __restrict__ src, int nsrc, int vmode) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    int si = i;
-    if (vmode == 2) { const int chunk = i / 32, j = i % 32; si = j < 16 ? chunk * 16 + j : n / 2 + chunk * 16 + (j - 16); }
-    dst[i] = (si < nsrc) ? (float)src[si] : 0.f;
-  }
-}
-
 struct OnesDesc { float* v_bias; int heads, d, dp; };
 // one launch for every V bias of the model: block b plants the ones column of entry b
 __global__ void set_ones_kernel(const OnesDesc* __restrict__ descs) {
@@ -58,64 +26,50 @@ __global__ void set_ones_kernel(const OnesDesc* __restrict__ descs) {
   for (int h = threadIdx.x; h < o.heads; h += blockDim.x) o.v_bias[h * o.dp + o.d] = 1.f;
 }
 
-// Batched packing (mvb_load_weights): one launch packs a whole batch of tensors; blockIdx.y selects the tensor and the
-// blocks of a row grid-stride over its elements. Same index arithmetic as the two single-tensor kernels above.
+// Weight packing (mvb_load_weights): one launch packs a whole batch of tensors; blockIdx.y selects the tensor and the
+// blocks of a row grid-stride over its elements.
 struct PackDesc {
-  void* dst; const void* src;
-  long long ld;
-  int rows_dst, kdst, nsrc, ksrc, rowmode, p0, p1, colmode, cin, taps;
-  int is_vec, vn, vmode, is_f32;
-  int cin_dst;
+  PackGeom g;          // matrix entry: the packed layout
+  const void* src;
+  int is_f32;
+  float* vdst;         // vector entry when non-null: vdst[0, vn) from src[0, vnsrc)
+  int vn, vnsrc, vmode;
 };
 __device__ __forceinline__ float pack_src(const void* src, long long i, int is_f32) {
   return is_f32 ? reinterpret_cast<const float*>(src)[i] : __half2float(reinterpret_cast<const __half*>(src)[i]);
 }
 __global__ void pack_batch_kernel(const PackDesc* __restrict__ descs) {
   const PackDesc d = descs[blockIdx.y];
-  if (d.is_vec) {
-    float* dst = reinterpret_cast<float*>(d.dst);
+  if (d.vdst) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < d.vn; i += gridDim.x * blockDim.x) {
-      int si = i;
-      if (d.vmode == 2) { const int chunk = i / 32, j = i % 32; si = j < 16 ? chunk * 16 + j : d.vn / 2 + chunk * 16 + (j - 16); }
-      dst[i] = (si < d.nsrc) ? pack_src(d.src, si, d.is_f32) : 0.f;
+      const int si = d.vmode == 2 ? geglu_src(i, d.vn) : i;
+      d.vdst[i] = (si < d.vnsrc) ? pack_src(d.src, si, d.is_f32) : 0.f;
     }
     return;
   }
-  __half* dst = reinterpret_cast<__half*>(d.dst);
-  const long long total = (long long)d.rows_dst * d.kdst;
+  const PackGeom& g = d.g;
+  const long long total = (long long)g.rows_dst * g.kdst;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int r = (int)(i / d.kdst), kk = (int)(i % d.kdst);
-    int srow = r;
-    if (d.rowmode == 1) {
-      const int h = r / d.p1, j = r % d.p1;
-      srow = j < d.p0 ? h * d.p0 + j : -1;
-    } else if (d.rowmode == 2) {
-      const int chunk = r / 32, j = r % 32;
-      srow = j < 16 ? chunk * 16 + j : d.rows_dst / 2 + chunk * 16 + (j - 16);
-    }
-    int scol = kk;
-    if (d.colmode == 1) {
-      const int cd = d.cin_dst > d.cin ? d.cin_dst : d.cin;
-      if (kk < cd * d.taps) { const int tap = kk / cd, c = kk % cd; scol = c < d.cin ? c * d.taps + tap : -1; } else scol = -1;
-    } else if (kk >= d.ksrc) scol = -1;
+    const int r = (int)(i / g.kdst), kk = (int)(i % g.kdst);
+    const int srow = src_row(g, r), scol = src_col(g, kk);
     float v = 0.f;
-    if (srow >= 0 && srow < d.nsrc && scol >= 0) v = pack_src(d.src, (long long)srow * d.ksrc + scol, d.is_f32);
-    dst[(long long)r * d.ld + kk] = __float2half_rn(v);
+    if (srow >= 0 && scol >= 0) v = pack_src(d.src, (long long)srow * g.ksrc + scol, d.is_f32);
+    g.dst[(long long)r * g.ld + kk] = __float2half_rn(v);
   }
 }
 
 // ---------------------------------------------------------------------------------------------- construction
-Engine::Engine(const mvb_config& cfg, int device, int kind) : cfg_(cfg), device_(device), kind_(kind) {
+Engine::Engine(const mvb_config& cfg, int device, Kind kind) : cfg_(cfg), device_(device), kind_(kind) {
   heads_ = cfg.heads;
-  if (kind_ == 1 || kind_ == 2) {
+  if (kind_ == Kind::ControlNet || kind_ == Kind::ReferenceNet) {
     // the encoder half of a plain SD-1.5 UNet: none of the musev switches apply
     cfg_.need_transformer_in = cfg_.use_anivv1_cfg = cfg_.resnet_2d_skip_time_act = cfg_.keep_vision_condtion = 0;
     cfg_.need_refer_emb = cfg_.ip_adapter_cross_attn = cfg_.need_t2i_ip_adapter = 0;
     // ControlNet uses the vanilla diffusers blocks (all three LayerNorm eps 1e-5); ReferenceNet2D is built from
     // musev/models/unet_2d_blocks.py -> musev BasicTransformerBlock and inherits the eps = 0 quirk (Q1)
-    ln_eps13_ = kind_ == 1 ? 1e-5f : 0.f;
+    ln_eps13_ = kind_ == Kind::ControlNet ? 1e-5f : 0.f;
   }
-  if (kind_ == 3 || kind_ == 4) {
+  if (kind_ == Kind::VaeDecoder || kind_ == Kind::VaeEncoder) {
     cfg_.need_transformer_in = cfg_.use_anivv1_cfg = cfg_.resnet_2d_skip_time_act = cfg_.keep_vision_condtion = 0;
     cfg_.need_refer_emb = cfg_.ip_adapter_cross_attn = cfg_.need_t2i_ip_adapter = 0;
     heads_ = 1;
@@ -196,14 +150,15 @@ void Engine::reg_mat(const std::string& name, Mat& m, int row0, int rows_dst, in
                      int ksrc, int colmode, int cin, int taps) {
   Loader l{};
   l.kind = LK_MAT;
-  l.dst = m.w ? m.w + (long long)row0 * m.K : nullptr;
-  l.ld = m.K; l.rows_dst = rows_dst; l.kdst = m.K; l.rowmode = rowmode; l.p0 = p0; l.p1 = p1;
-  l.colmode = colmode; l.cin = cin; l.taps = taps; l.nsrc = nsrc; l.ksrc = ksrc;
+  PackGeom& g = l.g;
+  g.dst = m.w ? m.w + (long long)row0 * m.K : nullptr;
+  g.ld = m.K; g.rows_dst = rows_dst; g.kdst = m.K; g.rowmode = rowmode; g.p0 = p0; g.p1 = p1;
+  g.colmode = colmode; g.cin = cin; g.taps = taps; g.nsrc = nsrc; g.ksrc = ksrc;
   loaders_[name] = l;
 }
 void Engine::reg_vec(const std::string& name, float* dst, int n, int nsrc, int vmode) {
   Loader l{};
-  l.kind = LK_VEC; l.vdst = dst; l.vn = n; l.nsrc = nsrc; l.vmode = vmode;
+  l.kind = LK_VEC; l.vdst = dst; l.vn = n; l.vnsrc = nsrc; l.vmode = vmode;
   loaders_[name] = l;
 }
 void Engine::reg_linear(const std::string& p, Mat& m, int N, int K, bool bias) {
@@ -317,11 +272,14 @@ void Engine::build_refer(const std::string& p, ReferAttn& r, int C) {
 }
 
 void Engine::build() {
-  if (kind_ == 1 || kind_ == 2) build_controlnet();
-  else if (kind_ == 3) build_vae();
-  else if (kind_ == 4) build_vae_encoder();
-  else if (kind_ == 5) build_pose_guider();
-  else build_unet();
+  switch (kind_) {
+    case Kind::UNet: build_unet(); break;
+    case Kind::ControlNet:
+    case Kind::ReferenceNet: build_controlnet(); break;
+    case Kind::VaeDecoder: build_vae(); break;
+    case Kind::VaeEncoder: build_vae_encoder(); break;
+    case Kind::PoseGuider: build_pose_guider(); break;
+  }
 }
 
 // UNetMidBlock2D of either VAE half (diffusers unet_2d_blocks.py; vae.py:113-122 / 236-245): resnet, one single-head
@@ -391,7 +349,7 @@ void Engine::build_pose_guider() {
     const int K = image ? 32 : 9 * L.cin_p;
     L.m = make_mat(L.cout_p, K, true);
     reg_mat(p + ".weight", L.m, 0, cout, 0, 0, 0, cout, cin * 9, 1, cin, 9);
-    if (!image) loaders_[p + ".weight"].cin_dst = L.cin_p;
+    if (!image) loaders_[p + ".weight"].g.cin_dst = L.cin_p;
     reg_vec(p + ".bias", L.m.bias, L.cout_p, cout);
     pg_.push_back(L);
   };
@@ -482,7 +440,7 @@ void Engine::build_controlnet() {
   build_spatial("mid_block.attentions.0", mid_st_, cm);
   build_resnet("mid_block.resnets.1", mid_res_[1], cm, cm);
   n_zero_convs_ = (int)tap_c.size() + 1;
-  if (kind_ == 2) return;   // ReferenceNet2D returns the taps themselves (referencenet.py:1063-1127): no zero convolutions
+  if (kind_ == Kind::ReferenceNet) return;   // ReferenceNet2D returns the taps themselves (referencenet.py:1063-1127): no zero convolutions
   for (int k = 0; k < (int)tap_c.size() && k < MVB_CONTROLNET_MAX_OUT - 1; ++k)
     reg_conv("controlnet_down_blocks." + std::to_string(k), zero_convs_[k], tap_c[k], tap_c[k], 1);
   reg_conv("controlnet_mid_block", zero_convs_[n_zero_convs_ - 1], cm, cm, 1);
@@ -591,43 +549,15 @@ void Engine::build_unet() {
   reg_vec("conv_out.bias", conv_out_.bias, 16, c.out_channels);
 }
 
+// One tensor through the batched path; only its element count is checked, so the shape is folded into one dimension.
 int Engine::load_weight(const char* name, const void* ptr, int is_f32, const long long* shape, int ndim) {
-  if (!slab_) { err_ = "engine not initialised"; return MVB_ERR_STATE; }
-  auto it = loaders_.find(name);
-  if (it == loaders_.end()) { err_ = std::string("unexpected weight name: ") + name; return MVB_ERR_INVALID; }
-  Loader& l = it->second;
-  long long numel = 1;
-  for (int i = 0; i < ndim; ++i) numel *= shape[i];
-  cudaSetDevice(device_);
-  if (l.kind == LK_ABS_SCALAR) {
-    if (numel != 1) { err_ = std::string("bad shape for ") + name; return MVB_ERR_INVALID; }
-    float v = 0.f;
-    if (is_f32) cudaMemcpy(&v, ptr, sizeof(float), cudaMemcpyDeviceToHost);
-    else { __half hv; cudaMemcpy(&hv, ptr, sizeof(__half), cudaMemcpyDeviceToHost); v = __half2float(hv); }
-    *l.host_scalar = fabsf(v);   // the reference applies torch.abs (musev/models/resnet.py:128, temporal_transformer.py:299)
-  } else if (l.kind == LK_VEC) {
-    if (numel != l.nsrc) { err_ = std::string("bad shape for ") + name; return MVB_ERR_INVALID; }
-    const int blocks = (l.vn + 255) / 256;
-    if (is_f32) pack_vec_kernel<float><<<blocks, 256>>>(l.vdst, l.vn, (const float*)ptr, l.nsrc, l.vmode);
-    else pack_vec_kernel<__half><<<blocks, 256>>>(l.vdst, l.vn, (const __half*)ptr, l.nsrc, l.vmode);
-  } else {
-    if (numel != (long long)l.nsrc * l.ksrc) { err_ = std::string("bad shape for ") + name; return MVB_ERR_INVALID; }
-    const long long total = (long long)l.rows_dst * l.kdst;
-    const int blocks = (int)((total + 255) / 256 < 132 * 32 ? (total + 255) / 256 : 132 * 32);
-    if (is_f32)
-      pack_matrix_kernel<float><<<blocks, 256>>>(l.dst, l.ld, l.rows_dst, l.kdst, (const float*)ptr, l.nsrc, l.ksrc,
-                                                 l.rowmode, l.p0, l.p1, l.colmode, l.cin, l.taps, l.cin_dst);
-    else
-      pack_matrix_kernel<__half><<<blocks, 256>>>(l.dst, l.ld, l.rows_dst, l.kdst, (const __half*)ptr, l.nsrc, l.ksrc,
-                                                  l.rowmode, l.p0, l.p1, l.colmode, l.cin, l.taps, l.cin_dst);
-  }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { err_ = std::string("pack kernel: ") + cudaGetErrorString(e); return MVB_ERR_CUDA; }
-  l.loaded = true;
-  return MVB_OK;
+  mvb_named_tensor t{};
+  t.name = name; t.device_ptr = ptr; t.is_f32 = is_f32; t.ndim = 1; t.shape[0] = 1;
+  for (int i = 0; i < ndim; ++i) t.shape[0] *= shape[i];
+  return load_weights(&t, 1);
 }
 
-// Batched form of load_weight: validates every entry first, then packs the whole batch with ONE kernel launch.
+// Validates every entry first, then packs the whole batch with ONE kernel launch and synchronises.
 int Engine::load_weights(const mvb_named_tensor* ts, int n) {
   if (!slab_) { err_ = "engine not initialised"; return MVB_ERR_STATE; }
   if (n <= 0) return MVB_OK;
@@ -655,13 +585,11 @@ int Engine::load_weights(const mvb_named_tensor* ts, int n) {
     PackDesc d{};
     d.src = t.device_ptr; d.is_f32 = t.is_f32;
     if (l.kind == LK_VEC) {
-      if (numel != l.nsrc) { err_ = std::string("bad shape for ") + t.name; return MVB_ERR_INVALID; }
-      d.is_vec = 1; d.dst = l.vdst; d.vn = l.vn; d.nsrc = l.nsrc; d.vmode = l.vmode;
+      if (numel != l.vnsrc) { err_ = std::string("bad shape for ") + t.name; return MVB_ERR_INVALID; }
+      d.vdst = l.vdst; d.vn = l.vn; d.vnsrc = l.vnsrc; d.vmode = l.vmode;
     } else {
-      if (numel != (long long)l.nsrc * l.ksrc) { err_ = std::string("bad shape for ") + t.name; return MVB_ERR_INVALID; }
-      d.dst = l.dst; d.ld = l.ld; d.rows_dst = l.rows_dst; d.kdst = l.kdst; d.nsrc = l.nsrc; d.ksrc = l.ksrc;
-      d.rowmode = l.rowmode; d.p0 = l.p0; d.p1 = l.p1; d.colmode = l.colmode; d.cin = l.cin; d.taps = l.taps;
-      d.cin_dst = l.cin_dst;
+      if (numel != (long long)l.g.nsrc * l.g.ksrc) { err_ = std::string("bad shape for ") + t.name; return MVB_ERR_INVALID; }
+      d.g = l.g;
     }
     descs.push_back(d);
     touched.push_back(&l);
@@ -702,13 +630,22 @@ struct Engine::Fwd {
   const mvb_unet_args* a;
   int B, T, H, W, NF;
   int heads;
-  float* gn_part;           // GroupNorm partial sums scratch
-  const float* temb_table;  // [NF, temb_total] fp32
-  const float* femb_table;  // [NF, femb_total] fp32
-  const __half* enc;        // [B*n_text, X] fp16
-  const __half* clip;       // [B*n_clip, X] fp16 or null
+  float* gn_part = nullptr;            // GroupNorm partial sums scratch
+  const float* temb_table = nullptr;   // [NF, temb_total] fp32
+  const float* femb_table = nullptr;   // [NF, femb_total] fp32
+  const __half* enc = nullptr;         // [B*n_text, X] fp16
+  const __half* clip = nullptr;        // [B*n_clip, X] fp16 or null
   bool skip_temporal;
   bool ok = true;
+
+  // `args` (B, T, H, W and what the layers read) must outlive the Fwd. Clears the taps of a real call and takes the
+  // GroupNorm scratch as the first allocation of the arena.
+  Fwd(Engine* e, Arena& arena, cudaStream_t st, const mvb_unet_args& args, bool skip_temporal_layers)
+      : E(e), ar(&arena), s(st), dry(arena.dry), a(&args), B(args.B), T(args.T), H(args.H), W(args.W), NF(args.B * args.T),
+        heads(e->heads_), skip_temporal(skip_temporal_layers) {
+    if (!dry) E->taps_.clear();
+    gn_part = alloc_f((long long)NF * (kGnMaxChunks + 1) * E->cfg_.norm_num_groups * 2);
+  }
 
   bool fail(const char* what, cudaError_t e) {
     if (ok) {
@@ -794,6 +731,61 @@ struct Engine::Fwd {
     const char* err = nullptr;
     cudaError_t e = launch_attention(s, aa, &err);
     if (e != cudaSuccess) fail(err, e);
+  }
+
+  // ---- stages shared by the model kinds
+  // conv_in at the full resolution: im2col of src (NCTHW [B, cin, T, H, W], 9 cin <= 64 columns) + one GEMM into x
+  // [NF*H*W, m.N]; res (NCHW [NF, m.N, H, W]) or null is added in the epilogue
+  void conv_in(__half* x, const void* src, int src_f32, int cin, const Mat& m, const void* res, int res_f32,
+               const char* what) {
+    const long long M = (long long)NF * H * W;
+    const size_t mk = mark();
+    __half* A = alloc_h(M, 64);
+    __half* r = res ? alloc_h(M, m.N) : nullptr;
+    if (!dry && ok) {
+      cudaError_t e = im2col_latent(s, src, src_f32, B, cin, T, H, W, A);
+      if (e == cudaSuccess && res) e = ncthw_to_tokens(s, res, res_f32, NF, m.N, 1, H * W, r, m.N, 1.f);
+      if (e != cudaSuccess) fail(what, e);
+    }
+    Epilogue ep; ep.out = x; ep.ldc = m.N;
+    if (res) { ep.res = r; ep.ld_res = m.N; }
+    gemm(A, M, 64, m, ep);
+    release(mk);
+  }
+  // Downsample2D: 3x3 stride-2 conv of x [NF, Hd, Wd, C] -> [NF, Hd/2, Wd/2, C]; pad 1: every side, 2: (0, 1, 0, 1)
+  __half* downsample(const __half* x, int C, int Hd, int Wd, const Mat& m, int pad) {
+    __half* y = alloc_h((long long)NF * (Hd / 2) * (Wd / 2), C);
+    if (!dry && ok) {
+      Epilogue ep; ep.out = y; ep.ldc = C; ep.bias = m.bias;
+      const char* err = nullptr;
+      cudaError_t e = launch_conv_s2(s, x, C, Wd, Hd, NF, m.w, C, ep, E->num_sms_, &err, pad);
+      if (e != cudaSuccess) fail(err, e);
+    }
+    return y;
+  }
+  // Upsample2D: nearest x2 then 3x3 conv (diffusers models/resnet.py:167-210), x [NF, Hd, Wd, C] -> [NF, 2Hd, 2Wd, C]
+  __half* upsample(const __half* x, int C, int Hd, int Wd, const Mat& m) {
+    __half* y = alloc_h((long long)NF * 4 * Hd * Wd, C);
+    const size_t mk = mark();
+    __half* up = alloc_h((long long)NF * 4 * Hd * Wd, C);
+    if (!dry && ok) {
+      cudaError_t e = upsample2x(s, x, NF, Hd, Wd, C, up);
+      if (e != cudaSuccess) fail("upsample2x", e);
+    }
+    Epilogue ep; ep.out = y; ep.ldc = C;
+    conv3x3(up, C, nullptr, 0, NF, 2 * Hd, 2 * Wd, m, ep);
+    release(mk);
+    return y;
+  }
+  // GroupNorm + SiLU + conv_out into 16 padded columns, fp16 or (out_f32) fp32: the last layers of the UNet and VAE halves
+  void* norm_out(const __half* x, int C, int Hd, int Wd, bool out_f32) {
+    const long long M = (long long)NF * Hd * Wd;
+    __half* hn = alloc_h(M, C);
+    gn(x, C, nullptr, 0, Hd * Wd, 1, E->cfg_.norm_eps, E->norm_out_, 1, hn);
+    void* o = out_f32 ? (void*)alloc_f(M * 16) : (void*)alloc_h(M, 16);
+    Epilogue ep; ep.out = (__half*)o; ep.ldc = 16; ep.out_f32 = out_f32 ? 1 : 0;
+    conv3x3(hn, C, nullptr, 0, NF, Hd, Wd, E->conv_out_, ep);
+    return o;
   }
 
   // ---- layers
@@ -1058,15 +1050,10 @@ struct Engine::Fwd {
   }
 };
 
-bool Engine::run(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
+bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
   const mvb_config& c = cfg_;
-  Fwd f;
-  f.E = this; f.ar = &ar; f.s = s; f.dry = ar.dry; f.a = &a;
-  f.B = a.B; f.T = a.T; f.H = a.H; f.W = a.W; f.NF = a.B * a.T;
-  f.heads = heads_;
-  f.skip_temporal = a.skip_temporal_layers != 0;
   const int nb = c.num_blocks, c0 = c.block_out_channels[0], temb = 4 * c0;
-  const int B = a.B, T = a.T, NF = f.NF;
+  const int B = a.B, T = a.T, NF = a.B * a.T;
   if (a.H % (1 << (nb - 1)) || a.W % (1 << (nb - 1))) { err_ = "H and W must be divisible by 2^(num_blocks-1)"; return false; }
   if (T > 32) { err_ = "at most 32 frames per window (temporal attention kernel)"; return false; }
   if (B < 1 || B > 64 || a.n_vis_cond > 64) { err_ = "batch (incl. CFG) must be in 1..64 and at most 64 vision-condition frames"; return false; }
@@ -1076,8 +1063,7 @@ bool Engine::run(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
     for (int i = 0; i < nb; ++i) expect += c.layers_per_block + (i == nb - 1 ? 0 : 1);
     if (a.n_refer != expect) { err_ = "down_block_refer_embs: wrong number of maps"; return false; }
   }
-  if (!ar.dry) taps_.clear();
-  f.gn_part = f.alloc_f((long long)NF * (kGnMaxChunks + 1) * c.norm_num_groups * 2);
+  Fwd f(this, ar, s, a, a.skip_temporal_layers != 0);
 
   // ---- embeddings (unet_3d_condition.py:887-937)
   __half* temb_rows = f.alloc_h(NF, temb);
@@ -1148,27 +1134,10 @@ bool Engine::run(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
 
   // ---- conv_in (unet_3d_condition.py:1008-1009)
   int Hc = a.H, Wc = a.W;
-  long long M = (long long)NF * Hc * Wc;
+  const long long M = (long long)NF * Hc * Wc;
   __half* x = f.alloc_h(M, c0);
-  {
-    const size_t mk = f.mark();
-    __half* A = f.alloc_h(M, 64);
-    if (!ar.dry && f.ok) {
-      cudaError_t e = im2col_latent(s, a.sample, a.sample_is_f32, B, c.in_channels, T, Hc, Wc, A);
-      if (e != cudaSuccess) f.fail("im2col_latent", e);
-    }
-    Epilogue ep; ep.out = x; ep.ldc = c0;
-    if (a.pose_guider_emb) {   // sample = conv_in(sample) + pose_guider_emb (:1011-1016), added in the GEMM epilogue
-      __half* pose = f.alloc_h(M, c0);
-      if (!ar.dry && f.ok) {
-        cudaError_t e = ncthw_to_tokens(s, a.pose_guider_emb, a.pose_is_f32, NF, c0, 1, Hc * Wc, pose, c0, 1.f);
-        if (e != cudaSuccess) f.fail("pose_guider_emb convert", e);
-      }
-      ep.res = pose; ep.ld_res = c0;
-    }
-    f.gemm(A, M, 64, conv_in_, ep);
-    f.release(mk);
-  }
+  // sample = conv_in(sample) + pose_guider_emb (:1011-1016), added in the GEMM epilogue
+  f.conv_in(x, a.sample, a.sample_is_f32, c.in_channels, conv_in_, a.pose_guider_emb, a.pose_is_f32, "conv_in inputs");
   f.tap("conv_in", x, M, c0);
   if (has_tin_) { x = f.temporal(tin_, x, Hc * Wc); f.tap("transformer_in", x, M, c0); }
   const bool use_ref = c.need_refer_emb && a.n_refer > 0;
@@ -1212,14 +1181,8 @@ bool Engine::run(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
       skips.push_back({x, ch, Hc, Wc});
     }
     if (!final) {
-      __half* y = f.alloc_h((long long)NF * (Hc / 2) * (Wc / 2), ch);
-      if (!ar.dry && f.ok) {
-        Epilogue ep; ep.out = y; ep.ldc = ch; ep.bias = blk.sampler.bias;
-        const char* err = nullptr;
-        cudaError_t e = launch_conv_s2(s, x, ch, Wc, Hc, NF, blk.sampler.w, ch, ep, num_sms_, &err, 1);
-        if (e != cudaSuccess) f.fail(err, e);
-      }
-      x = y; Hc /= 2; Wc /= 2;
+      x = f.downsample(x, ch, Hc, Wc, blk.sampler, 1);
+      Hc /= 2; Wc /= 2;
       if (use_ref) {
         const int ri = ref_start + c.layers_per_block;
         __half* tok = f.refer_tokens(a.refer_embs[ri], ch, a.refer_t[ri], a.refer_h[ri], a.refer_w[ri]);
@@ -1281,34 +1244,16 @@ bool Engine::run(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
       f.tap("up_blocks." + std::to_string(i) + "." + std::to_string(j), x, (long long)NF * Hc * Wc, ch);
     }
     if (!final) {
-      // Upsample2D: nearest x2 then 3x3 conv (diffusers models/resnet.py:167-210)
-      __half* y = f.alloc_h((long long)NF * 4 * Hc * Wc, ch);
-      const size_t mk = f.mark();
-      __half* up = f.alloc_h((long long)NF * 4 * Hc * Wc, ch);
-      if (!ar.dry && f.ok) {
-        cudaError_t e = upsample2x(s, x, NF, Hc, Wc, ch, up);
-        if (e != cudaSuccess) f.fail("upsample2x", e);
-      }
+      x = f.upsample(x, ch, Hc, Wc, blk.sampler);
       Hc *= 2; Wc *= 2;
-      Epilogue ep; ep.out = y; ep.ldc = ch;
-      f.conv3x3(up, ch, nullptr, 0, NF, Hc, Wc, blk.sampler, ep);
-      f.release(mk);
-      x = y;
       f.tap("up_blocks." + std::to_string(i) + ".up", x, (long long)NF * Hc * Wc, ch);
     }
   }
   // ---- out (unet_3d_condition.py:1258-1263)
-  M = (long long)NF * Hc * Wc;
-  {
-    __half* hn = f.alloc_h(M, c0);
-    f.gn(x, c0, nullptr, 0, Hc * Wc, 1, c.norm_eps, norm_out_, 1, hn);
-    __half* o16 = f.alloc_h(M, 16);
-    Epilogue ep; ep.out = o16; ep.ldc = 16;
-    f.conv3x3(hn, c0, nullptr, 0, NF, Hc, Wc, conv_out_, ep);
-    if (!ar.dry && f.ok) {
-      cudaError_t e = tokens_to_ncthw(s, o16, 16, B, c.out_channels, T, Hc * Wc, a.out, a.out_is_f32);
-      if (e != cudaSuccess) f.fail("tokens_to_ncthw", e);
-    }
+  const __half* o16 = (const __half*)f.norm_out(x, c0, Hc, Wc, false);
+  if (!ar.dry && f.ok) {
+    cudaError_t e = tokens_to_ncthw(s, o16, 16, B, c.out_channels, T, Hc * Wc, a.out, a.out_is_f32);
+    if (e != cudaSuccess) f.fail("tokens_to_ncthw", e);
   }
   return f.ok;
 }
@@ -1321,21 +1266,13 @@ bool Engine::run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_
   if (NF < 1 || a.H < 1 || a.W < 1) { err_ = "controlnet: bad shape"; return false; }
   if (a.H % (1 << (nb - 1)) || a.W % (1 << (nb - 1))) { err_ = "H and W must be divisible by 2^(num_blocks-1)"; return false; }
   if (a.n_out != n_zero_convs_) { err_ = "controlnet: n_out must be the number of residual maps (12 + 1 for SD-1.5)"; return false; }
-  const bool refnet = kind_ == 2;
+  const bool refnet = kind_ == Kind::ReferenceNet;
   // output layout [out_b, C, out_t, h, w] with NF = out_b * out_t; ControlNet: (b t) c h w, i.e. out_t = 1
   const int out_t = (refnet && a.out_frames > 0) ? a.out_frames : 1;
   if (NF % out_t) { err_ = "referencenet: num_frames must divide the batch"; return false; }
   mvb_unet_args ua{};                     // what the shared layer functions read
   ua.B = NF; ua.T = 1; ua.H = a.H; ua.W = a.W; ua.n_text = a.n_text; ua.n_vis_cond = 0; ua.ip_adapter_scale = 0.f;
-  Fwd f;
-  f.E = this; f.ar = &ar; f.s = s; f.dry = ar.dry; f.a = &ua;
-  f.B = NF; f.T = 1; f.H = a.H; f.W = a.W; f.NF = NF;     // every frame is its own batch element (own text rows)
-  f.heads = heads_;
-  f.skip_temporal = true;
-  f.femb_table = nullptr;
-  f.clip = nullptr;
-  if (!ar.dry) taps_.clear();
-  f.gn_part = f.alloc_f((long long)NF * (kGnMaxChunks + 1) * c.norm_num_groups * 2);
+  Fwd f(this, ar, s, ua, true);           // every frame is its own batch element (own text rows)
   // ---- time embedding (:733-741): one timestep for all frames; ResnetBlock2D applies SiLU before time_emb_proj
   float* temb_table = f.alloc_f((long long)NF * temb_total_);
   f.temb_table = temb_table;
@@ -1369,22 +1306,9 @@ bool Engine::run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_
   f.enc = enc;
   // ---- conv_in + condition embedding (:780-785)
   int Hc = a.H, Wc = a.W;
-  long long M = (long long)NF * Hc * Wc;
-  __half* x = f.alloc_h(M, c0);
-  {
-    const size_t mk = f.mark();
-    __half* A = f.alloc_h(M, 64);
-    __half* cond = refnet ? nullptr : f.alloc_h(M, c0);
-    if (!ar.dry && f.ok) {
-      cudaError_t e = im2col_latent(s, a.sample, a.sample_is_f32, NF, c.in_channels, 1, Hc, Wc, A);
-      if (e == cudaSuccess && !refnet) e = ncthw_to_tokens(s, a.cond_latents, a.cond_is_f32, NF, c0, 1, Hc * Wc, cond, c0, 1.f);
-      if (e != cudaSuccess) f.fail("controlnet inputs", e);
-    }
-    Epilogue ep; ep.out = x; ep.ldc = c0;
-    if (!refnet) { ep.res = cond; ep.ld_res = c0; }
-    f.gemm(A, M, 64, conv_in_, ep);
-    f.release(mk);
-  }
+  __half* x = f.alloc_h((long long)NF * Hc * Wc, c0);
+  f.conv_in(x, a.sample, a.sample_is_f32, c.in_channels, conv_in_, refnet ? nullptr : a.cond_latents, a.cond_is_f32,
+            "controlnet inputs");
   struct TapT { __half* p; int C, H, W; };
   std::vector<TapT> tp;
   tp.push_back({x, c0, Hc, Wc});
@@ -1401,14 +1325,8 @@ bool Engine::run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_
       tp.push_back({x, ch, Hc, Wc});
     }
     if (!final) {
-      __half* y = f.alloc_h((long long)NF * (Hc / 2) * (Wc / 2), ch);
-      if (!ar.dry && f.ok) {
-        Epilogue ep; ep.out = y; ep.ldc = ch; ep.bias = blk.sampler.bias;
-        const char* err = nullptr;
-        cudaError_t e = launch_conv_s2(s, x, ch, Wc, Hc, NF, blk.sampler.w, ch, ep, num_sms_, &err, 1);
-        if (e != cudaSuccess) f.fail(err, e);
-      }
-      x = y; Hc /= 2; Wc /= 2;
+      x = f.downsample(x, ch, Hc, Wc, blk.sampler, 1);
+      Hc /= 2; Wc /= 2;
       tp.push_back({x, ch, Hc, Wc});
     }
   }
@@ -1452,14 +1370,7 @@ bool Engine::run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s) {
   }
   mvb_unet_args ua{};
   ua.B = NF; ua.T = 1; ua.H = a.h; ua.W = a.w;
-  Fwd f;
-  f.E = this; f.ar = &ar; f.s = s; f.dry = ar.dry; f.a = &ua;
-  f.B = NF; f.T = 1; f.H = a.h; f.W = a.w; f.NF = NF;
-  f.heads = 1;
-  f.skip_temporal = true;
-  f.temb_table = nullptr; f.femb_table = nullptr; f.enc = nullptr; f.clip = nullptr;
-  if (!ar.dry) taps_.clear();
-  f.gn_part = f.alloc_f((long long)NF * (kGnMaxChunks + 1) * c.norm_num_groups * 2);
+  Fwd f(this, ar, s, ua, true);
   int Hc = a.h, Wc = a.w;
   const long long M0 = (long long)NF * Hc * Wc;
   // ---- post_quant_conv + conv_in (autoencoder_kl.py:283, vae.py:268)
@@ -1467,14 +1378,11 @@ bool Engine::run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s) {
   {
     const size_t mk = f.mark();
     float* z = f.alloc_f((long long)NF * zc * Hc * Wc);
-    __half* A = f.alloc_h(M0, 64);
     if (!ar.dry && f.ok) {
       cudaError_t e = latent_pointwise(s, a.latents, a.latents_is_f32, NF, zc, Hc * Wc, vae_pq_w_, vae_pq_b_, a.latent_scale, z);
-      if (e == cudaSuccess) e = im2col_latent(s, z, 1, NF, zc, 1, Hc, Wc, A);
       if (e != cudaSuccess) f.fail("vae inputs", e);
     }
-    Epilogue ep; ep.out = x; ep.ldc = cm;
-    f.gemm(A, M0, 64, conv_in_, ep);
+    f.conv_in(x, z, 1, zc, conv_in_, nullptr, 0, "vae inputs");
     f.release(mk);
   }
   f.tap("conv_in", x, M0, cm);
@@ -1489,26 +1397,12 @@ bool Engine::run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s) {
     }
     f.tap("up_blocks." + std::to_string(i), x, (long long)NF * Hc * Wc, ch);
     if (blk.has_sampler) {
-      __half* y = f.alloc_h((long long)NF * 4 * Hc * Wc, ch);
-      const size_t mk = f.mark();
-      __half* up = f.alloc_h((long long)NF * 4 * Hc * Wc, ch);
-      if (!ar.dry && f.ok) {
-        cudaError_t e = upsample2x(s, x, NF, Hc, Wc, ch, up);
-        if (e != cudaSuccess) f.fail("upsample2x", e);
-      }
+      x = f.upsample(x, ch, Hc, Wc, blk.sampler);
       Hc *= 2; Wc *= 2;
-      Epilogue ep; ep.out = y; ep.ldc = ch;
-      f.conv3x3(up, ch, nullptr, 0, NF, Hc, Wc, blk.sampler, ep);
-      f.release(mk);
-      x = y;
     }
   }
   // ---- out (vae.py:307-314)
-  const long long M = (long long)NF * Hc * Wc;
-  __half* hn = f.alloc_h(M, ch);
-  f.gn(x, ch, nullptr, 0, Hc * Wc, 1, c.norm_eps, norm_out_, 1, hn);
-  __half* o16 = f.alloc_h(M, 16);
-  { Epilogue ep; ep.out = o16; ep.ldc = 16; f.conv3x3(hn, ch, nullptr, 0, NF, Hc, Wc, conv_out_, ep); }
+  const __half* o16 = (const __half*)f.norm_out(x, ch, Hc, Wc, false);
   if (!ar.dry && f.ok) {
     cudaError_t e = a.postprocess
         ? tokens_to_ncthw_affine(s, o16, 16, NF, c.out_channels, 1, Hc * Wc, a.out, a.out_is_f32, 0.5f, 0.5f, 0.f, 1.f)
@@ -1535,29 +1429,11 @@ bool Engine::run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_
   if (const char* bad = vae_encode_shape_error(a)) { err_ = bad; return false; }
   mvb_unet_args ua{};
   ua.B = NF; ua.T = 1; ua.H = a.h * f; ua.W = a.w * f;
-  Fwd fw;
-  fw.E = this; fw.ar = &ar; fw.s = s; fw.dry = ar.dry; fw.a = &ua;
-  fw.B = NF; fw.T = 1; fw.H = ua.H; fw.W = ua.W; fw.NF = NF;
-  fw.heads = 1;
-  fw.skip_temporal = true;
-  fw.temb_table = nullptr; fw.femb_table = nullptr; fw.enc = nullptr; fw.clip = nullptr;
-  if (!ar.dry) taps_.clear();
-  fw.gn_part = fw.alloc_f((long long)NF * (kGnMaxChunks + 1) * c.norm_num_groups * 2);
+  Fwd fw(this, ar, s, ua, true);
   int Hc = ua.H, Wc = ua.W;
   // ---- conv_in (vae.py:136): im2col of the C-channel image (9 C of 64 columns) + one GEMM
   __half* x = fw.alloc_h((long long)NF * Hc * Wc, c0);
-  {
-    const long long M = (long long)NF * Hc * Wc;
-    const size_t mk = fw.mark();
-    __half* A = fw.alloc_h(M, 64);
-    if (!ar.dry && fw.ok) {
-      cudaError_t e = im2col_latent(s, a.latents, a.latents_is_f32, NF, c.in_channels, 1, Hc, Wc, A);
-      if (e != cudaSuccess) fw.fail("vae encode input", e);
-    }
-    Epilogue ep; ep.out = x; ep.ldc = c0;
-    fw.gemm(A, M, 64, conv_in_, ep);
-    fw.release(mk);
-  }
+  fw.conv_in(x, a.latents, a.latents_is_f32, c.in_channels, conv_in_, nullptr, 0, "vae encode input");
   fw.tap("conv_in", x, (long long)NF * Hc * Wc, c0);
   // ---- down blocks (unet_2d_blocks.py DownEncoderBlock2D; Downsample2D(padding=0) pads (0, 1, 0, 1), resnet.py:213-278)
   int ch = c0;
@@ -1568,25 +1444,15 @@ bool Engine::run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_
       ch = blk.layers[j].res.C;
     }
     if (blk.has_sampler) {
-      __half* y = fw.alloc_h((long long)NF * (Hc / 2) * (Wc / 2), ch);
-      if (!ar.dry && fw.ok) {
-        Epilogue ep; ep.out = y; ep.ldc = ch; ep.bias = blk.sampler.bias;
-        const char* err = nullptr;
-        cudaError_t e = launch_conv_s2(s, x, ch, Wc, Hc, NF, blk.sampler.w, ch, ep, num_sms_, &err, 2);
-        if (e != cudaSuccess) fw.fail(err, e);
-      }
-      x = y; Hc /= 2; Wc /= 2;
+      x = fw.downsample(x, ch, Hc, Wc, blk.sampler, 2);
+      Hc /= 2; Wc /= 2;
     }
     fw.tap("down_blocks." + std::to_string(i), x, (long long)NF * Hc * Wc, ch);
   }
   x = fw.vae_mid(x, cm, Hc, Wc);
   // ---- out (vae.py:170-173) + quant_conv (autoencoder_kl.py:284): conv_out stores fp32 so the moments are not rounded
   // to fp16 before quant_conv
-  const long long M = (long long)NF * Hc * Wc;
-  __half* hn = fw.alloc_h(M, cm);
-  fw.gn(x, cm, nullptr, 0, Hc * Wc, 1, c.norm_eps, norm_out_, 1, hn);
-  float* o32 = fw.alloc_f(M * 16);
-  { Epilogue ep; ep.out = (__half*)o32; ep.ldc = 16; ep.out_f32 = 1; fw.conv3x3(hn, cm, nullptr, 0, NF, Hc, Wc, conv_out_, ep); }
+  const float* o32 = (const float*)fw.norm_out(x, cm, Hc, Wc, true);
   if (!ar.dry && fw.ok) {
     cudaError_t e = vae_moments(s, o32, 16, NF, zc2, Hc * Wc, vae_pq_w_, vae_pq_b_, a.postprocess, a.latent_scale, a.out,
                                 a.out_is_f32);
@@ -1595,27 +1461,7 @@ bool Engine::run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_
   return fw.ok;
 }
 
-long long Engine::vae_encode_workspace_bytes(const mvb_vae_decode_args& a) {
-  if (kind_ != 4) { err_ = "not a VAE encoder handle"; return -1; }
-  Arena ar;
-  ar.dry = true;
-  if (!run_vae_encode(a, ar, nullptr)) return -1;
-  return (long long)ar.peak + 4096;
-}
 
-int Engine::vae_encode(const mvb_vae_decode_args& a, void* workspace, long long wbytes, cudaStream_t stream) {
-  if (kind_ != 4) { err_ = "not a VAE encoder handle"; return MVB_ERR_STATE; }
-  if (!finalized_) { err_ = "mvb_finalize has not been called (or weights are missing)"; return MVB_ERR_STATE; }
-  if (!a.latents || !a.out || !workspace) { err_ = "null pointer argument"; return MVB_ERR_INVALID; }
-  if (const char* bad = vae_encode_shape_error(a)) { err_ = bad; return MVB_ERR_INVALID; }
-  cudaSetDevice(device_);
-  Arena ar;
-  ar.dry = false;
-  ar.base = (char*)workspace;
-  ar.cap = (size_t)wbytes;
-  if (!run_vae_encode(a, ar, stream)) return MVB_ERR_CUDA;
-  return MVB_OK;
-}
 
 static const char* pose_guider_shape_error(const mvb_vae_decode_args& a, int nb) {
   if (a.N < 1 || a.h < 1 || a.w < 1) return "pose guider: bad shape (N, h, w must be positive)";
@@ -1686,89 +1532,73 @@ bool Engine::run_pose_guider(const mvb_vae_decode_args& a, Arena& ar, cudaStream
   return true;
 }
 
-long long Engine::pose_guider_workspace_bytes(const mvb_vae_decode_args& a) {
-  if (kind_ != 5) { err_ = "not a PoseGuider handle"; return -1; }
+// ---------------------------------------------------------------------------------------------- entry points
+template <typename Args>
+long long Engine::dry_run(RunFn<Args> run, std::initializer_list<Kind> kinds, const char* wrong_kind, const Args& a) {
+  if (std::find(kinds.begin(), kinds.end(), kind_) == kinds.end()) { err_ = wrong_kind; return -1; }
   Arena ar;
   ar.dry = true;
-  if (!run_pose_guider(a, ar, nullptr)) return -1;
+  if (!(this->*run)(a, ar, nullptr)) return -1;
   return (long long)ar.peak + 4096;
 }
 
-int Engine::pose_guider_forward(const mvb_vae_decode_args& a, void* workspace, long long wbytes, cudaStream_t stream) {
-  if (kind_ != 5) { err_ = "not a PoseGuider handle"; return MVB_ERR_STATE; }
+template <typename Args>
+int Engine::launch(RunFn<Args> run, std::initializer_list<Kind> kinds, const char* wrong_kind, const char* bad_args,
+                   const Args& a, void* workspace, long long wbytes, cudaStream_t stream) {
+  if (std::find(kinds.begin(), kinds.end(), kind_) == kinds.end()) { err_ = wrong_kind; return MVB_ERR_STATE; }
   if (!finalized_) { err_ = "mvb_finalize has not been called (or weights are missing)"; return MVB_ERR_STATE; }
-  if (!a.latents || !a.out || !workspace) { err_ = "null pointer argument"; return MVB_ERR_INVALID; }
-  if (const char* bad = pose_guider_shape_error(a, cfg_.num_blocks)) { err_ = bad; return MVB_ERR_INVALID; }
+  if (bad_args) { err_ = bad_args; return MVB_ERR_INVALID; }
   cudaSetDevice(device_);
   Arena ar;
   ar.dry = false;
   ar.base = (char*)workspace;
   ar.cap = (size_t)wbytes;
-  if (!run_pose_guider(a, ar, stream)) return MVB_ERR_CUDA;
+  if (!(this->*run)(a, ar, stream)) return MVB_ERR_CUDA;
   return MVB_OK;
 }
 
-long long Engine::vae_workspace_bytes(const mvb_vae_decode_args& a) {
-  if (kind_ != 3) { err_ = "not a VAE decoder handle"; return -1; }
-  Arena ar;
-  ar.dry = true;
-  if (!run_vae(a, ar, nullptr)) return -1;
-  return (long long)ar.peak + 4096;
-}
+static const char* kNullArg = "null pointer argument";
 
-int Engine::vae_decode(const mvb_vae_decode_args& a, void* workspace, long long wbytes, cudaStream_t stream) {
-  if (kind_ != 3) { err_ = "not a VAE decoder handle"; return MVB_ERR_STATE; }
-  if (!finalized_) { err_ = "mvb_finalize has not been called (or weights are missing)"; return MVB_ERR_STATE; }
-  if (!a.latents || !a.out || !workspace) { err_ = "null pointer argument"; return MVB_ERR_INVALID; }
-  cudaSetDevice(device_);
-  Arena ar;
-  ar.dry = false;
-  ar.base = (char*)workspace;
-  ar.cap = (size_t)wbytes;
-  if (!run_vae(a, ar, stream)) return MVB_ERR_CUDA;
-  return MVB_OK;
+long long Engine::workspace_bytes(const mvb_unet_args& a) {
+  return dry_run(&Engine::run_unet, {Kind::UNet}, "not a UNet handle", a);
+}
+int Engine::forward(const mvb_unet_args& a, void* ws, long long wbytes, cudaStream_t stream) {
+  const char* bad = (!a.sample || !a.out || !a.encoder_hidden_states || !ws) ? kNullArg : nullptr;
+  return launch(&Engine::run_unet, {Kind::UNet}, "not a UNet handle", bad, a, ws, wbytes, stream);
 }
 
 long long Engine::controlnet_workspace_bytes(const mvb_controlnet_args& a) {
-  if (kind_ != 1 && kind_ != 2) { err_ = "not a ControlNet / ReferenceNet handle"; return -1; }
-  Arena ar;
-  ar.dry = true;
-  if (!run_controlnet(a, ar, nullptr)) return -1;
-  return (long long)ar.peak + 4096;
+  return dry_run(&Engine::run_controlnet, {Kind::ControlNet, Kind::ReferenceNet}, "not a ControlNet / ReferenceNet handle", a);
+}
+int Engine::controlnet_forward(const mvb_controlnet_args& a, void* ws, long long wbytes, cudaStream_t stream) {
+  const bool cond_missing = kind_ == Kind::ControlNet && !a.cond_latents;
+  const char* bad = (!a.sample || cond_missing || !a.encoder_hidden_states || !ws) ? kNullArg : nullptr;
+  return launch(&Engine::run_controlnet, {Kind::ControlNet, Kind::ReferenceNet}, "not a ControlNet / ReferenceNet handle", bad,
+                a, ws, wbytes, stream);
 }
 
-int Engine::controlnet_forward(const mvb_controlnet_args& a, void* workspace, long long wbytes, cudaStream_t stream) {
-  if (kind_ != 1 && kind_ != 2) { err_ = "not a ControlNet / ReferenceNet handle"; return MVB_ERR_STATE; }
-  if (!finalized_) { err_ = "mvb_finalize has not been called (or weights are missing)"; return MVB_ERR_STATE; }
-  if (!a.sample || (kind_ == 1 && !a.cond_latents) || !a.encoder_hidden_states || !workspace) { err_ = "null pointer argument"; return MVB_ERR_INVALID; }
-  cudaSetDevice(device_);
-  Arena ar;
-  ar.dry = false;
-  ar.base = (char*)workspace;
-  ar.cap = (size_t)wbytes;
-  if (!run_controlnet(a, ar, stream)) return MVB_ERR_CUDA;
-  return MVB_OK;
+long long Engine::vae_workspace_bytes(const mvb_vae_decode_args& a) {
+  return dry_run(&Engine::run_vae, {Kind::VaeDecoder}, "not a VAE decoder handle", a);
+}
+int Engine::vae_decode(const mvb_vae_decode_args& a, void* ws, long long wbytes, cudaStream_t stream) {
+  const char* bad = (!a.latents || !a.out || !ws) ? kNullArg : nullptr;
+  return launch(&Engine::run_vae, {Kind::VaeDecoder}, "not a VAE decoder handle", bad, a, ws, wbytes, stream);
 }
 
-long long Engine::workspace_bytes(const mvb_unet_args& a) {
-  if (kind_ != 0) { err_ = "not a UNet handle"; return -1; }
-  Arena ar;
-  ar.dry = true;
-  if (!run(a, ar, nullptr)) return -1;
-  return (long long)ar.peak + 4096;
+long long Engine::vae_encode_workspace_bytes(const mvb_vae_decode_args& a) {
+  return dry_run(&Engine::run_vae_encode, {Kind::VaeEncoder}, "not a VAE encoder handle", a);
+}
+int Engine::vae_encode(const mvb_vae_decode_args& a, void* ws, long long wbytes, cudaStream_t stream) {
+  const char* bad = (!a.latents || !a.out || !ws) ? kNullArg : vae_encode_shape_error(a);
+  return launch(&Engine::run_vae_encode, {Kind::VaeEncoder}, "not a VAE encoder handle", bad, a, ws, wbytes, stream);
 }
 
-int Engine::forward(const mvb_unet_args& a, void* workspace, long long wbytes, cudaStream_t stream) {
-  if (kind_ != 0) { err_ = "not a UNet handle"; return MVB_ERR_STATE; }
-  if (!finalized_) { err_ = "mvb_finalize has not been called (or weights are missing)"; return MVB_ERR_STATE; }
-  if (!a.sample || !a.out || !a.encoder_hidden_states || !workspace) { err_ = "null pointer argument"; return MVB_ERR_INVALID; }
-  cudaSetDevice(device_);
-  Arena ar;
-  ar.dry = false;
-  ar.base = (char*)workspace;
-  ar.cap = (size_t)wbytes;
-  if (!run(a, ar, stream)) return MVB_ERR_CUDA;
-  return MVB_OK;
+long long Engine::pose_guider_workspace_bytes(const mvb_vae_decode_args& a) {
+  return dry_run(&Engine::run_pose_guider, {Kind::PoseGuider}, "not a PoseGuider handle", a);
+}
+int Engine::pose_guider_forward(const mvb_vae_decode_args& a, void* ws, long long wbytes, cudaStream_t stream) {
+  const char* bad = (!a.latents || !a.out || !ws) ? kNullArg : pose_guider_shape_error(a, cfg_.num_blocks);
+  return launch(&Engine::run_pose_guider, {Kind::PoseGuider}, "not a PoseGuider handle", bad, a, ws, wbytes, stream);
 }
 
 }  // namespace mvb

@@ -4,6 +4,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <initializer_list>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -77,22 +78,56 @@ struct Block {
   ReferAttn ref_down; // ReferEmbFuseAttention applied after the downsampler
 };
 
-enum LoadKind { LK_MAT, LK_VEC, LK_ABS_SCALAR };
-struct Loader {
-  LoadKind kind;
-  // LK_MAT: dst [.., ld] rows [row0, row0+rows_dst): source [Nsrc, Ksrc]
+// Packed layout of one matrix / convolution weight: rows [0, rows_dst) x columns [0, kdst) of dst (leading dimension ld)
+// hold the reference tensor [nsrc, ksrc] (row-major; a convolution's [N, cin, taps] flattened). The packer, the LoRA
+// merge and the read-back all map packed elements to source elements through src_row / src_col below.
+struct PackGeom {
   __half* dst = nullptr;
   long long ld = 0;
   int rows_dst = 0, kdst = 0;
+  int nsrc = 0, ksrc = 0;
   int rowmode = 0;  // 0 copy, 1 pad heads (p0 = d, p1 = dp), 2 geglu interleave
   int p0 = 0, p1 = 0;
-  int colmode = 0;  // 0 identity (zero fill beyond Ksrc), 1 conv [N, Cin, taps] -> (tap, c)
+  int colmode = 0;  // 0 identity (zero fill beyond ksrc), 1 conv [N, cin, taps] -> (tap, c)
   int cin = 0, taps = 1;
   int cin_dst = 0;  // colmode 1: destination channel stride per tap when > cin (the padding columns stay zero)
-  int nsrc = 0, ksrc = 0;
-  // LK_VEC
+};
+
+// GEGLU interleave of a packed vector / row index i of n: chunks of [16 value | 16 gate] -> value i or gate n/2 + i
+__host__ __device__ __forceinline__ int geglu_src(int i, int n) {
+  const int chunk = i / 32, j = i % 32;
+  return j < 16 ? chunk * 16 + j : n / 2 + chunk * 16 + (j - 16);
+}
+// packed row -> source row, -1 for padding that has no source element
+__host__ __device__ __forceinline__ int src_row(const PackGeom& g, int r) {
+  int s = r;
+  if (g.rowmode == 1) {
+    const int h = r / g.p1, j = r % g.p1;
+    s = j < g.p0 ? h * g.p0 + j : -1;
+  } else if (g.rowmode == 2) {
+    s = geglu_src(r, g.rows_dst);
+  }
+  return (r < g.rows_dst && s >= 0 && s < g.nsrc) ? s : -1;
+}
+// packed column -> source column, -1 for padding that has no source element
+__host__ __device__ __forceinline__ int src_col(const PackGeom& g, int kk) {
+  if (kk >= g.kdst) return -1;
+  if (g.colmode == 1) {
+    const int cd = g.cin_dst > g.cin ? g.cin_dst : g.cin;
+    if (kk >= cd * g.taps) return -1;
+    const int tap = kk / cd, c = kk % cd;
+    return c < g.cin ? c * g.taps + tap : -1;
+  }
+  return kk < g.ksrc ? kk : -1;
+}
+
+enum LoadKind { LK_MAT, LK_VEC, LK_ABS_SCALAR };
+struct Loader {
+  LoadKind kind;
+  PackGeom g;       // LK_MAT
+  // LK_VEC: vdst[0, vn) from a source of vnsrc elements
   float* vdst = nullptr;
-  int vn = 0;       // destination length
+  int vn = 0, vnsrc = 0;
   int vmode = 0;    // 0 copy (zero fill beyond source), 2 geglu interleave
   // LK_ABS_SCALAR
   float* host_scalar = nullptr;
@@ -121,13 +156,15 @@ struct Arena {
   }
 };
 
+// UNet: UNet3DConditionModel; ControlNet: ControlNet encoder (diffusers models/controlnet.py);
+// ReferenceNet: ReferenceNet2D encoder + mid block (musev/models/referencenet.py);
+// VaeDecoder / VaeEncoder: the AutoencoderKL halves (diffusers models/autoencoder_kl.py, vae.py);
+// PoseGuider: musev/models/controlnet.py:326-371
+enum class Kind { UNet, ControlNet, ReferenceNet, VaeDecoder, VaeEncoder, PoseGuider };
+
 class Engine {
  public:
-  // kind 0: UNet3DConditionModel; kind 1: ControlNet encoder (diffusers models/controlnet.py);
-  // kind 2: ReferenceNet2D encoder + mid block (musev/models/referencenet.py);
-  // kind 3: AutoencoderKL decoder (diffusers models/autoencoder_kl.py, vae.py); kind 4: AutoencoderKL encoder (same files);
-  // kind 5: PoseGuider (musev/models/controlnet.py:326-371)
-  explicit Engine(const mvb_config& cfg, int device, int kind = 0);
+  Engine(const mvb_config& cfg, int device, Kind kind);
   ~Engine();
   int load_weight(const char* name, const void* dev_ptr, int is_f32, const long long* shape, int ndim);
   int load_weights(const mvb_named_tensor* tensors, int n);
@@ -147,7 +184,7 @@ class Engine {
   int pose_guider_forward(const mvb_vae_decode_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long controlnet_workspace_bytes(const mvb_controlnet_args& a);
   int controlnet_forward(const mvb_controlnet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
-  int kind() const { return kind_; }
+  Kind kind() const { return kind_; }
   const char* error() const { return err_.c_str(); }
   struct Tap { std::string name; const __half* p; long long rows; int C; };
   const std::vector<Tap>& taps() const { return taps_; }
@@ -179,7 +216,15 @@ class Engine {
 
   // forward helpers (all return false on error, message in err_)
   struct Fwd;
-  bool run(const mvb_unet_args& a, Arena& ar, cudaStream_t s);
+  template <typename Args> using RunFn = bool (Engine::*)(const Args&, Arena&, cudaStream_t);
+  // Every kind's workspace query: `run` on a dry arena, its peak + 4096 bytes; -1 on a handle of another kind
+  template <typename Args>
+  long long dry_run(RunFn<Args> run, std::initializer_list<Kind> kinds, const char* wrong_kind, const Args& a);
+  // Every kind's forward: handle checks, then `bad_args` (message of a rejected argument, or null), then `run`
+  template <typename Args>
+  int launch(RunFn<Args> run, std::initializer_list<Kind> kinds, const char* wrong_kind, const char* bad_args, const Args& a,
+             void* workspace, long long workspace_bytes, cudaStream_t stream);
+  bool run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s);
   bool run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_t s);
   bool run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
   bool run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
@@ -187,7 +232,7 @@ class Engine {
 
   mvb_config cfg_;
   int device_ = 0, num_sms_ = 132;
-  int kind_ = 0;
+  Kind kind_ = Kind::UNet;
   float ln_eps13_ = 0.f;       // LayerNorm eps of norm1 / norm3: 0 in the musev blocks (Q1), 1e-5 in the vanilla diffusers blocks
   int heads_ = 8;
   bool finalized_ = false;

@@ -1,4 +1,5 @@
-// LoRA merge into the packed UNet weights, and read-back of a packed weight in the reference layout.
+// LoRA merge into the packed UNet weights, and read-back of a packed weight in the reference layout. Both map packed
+// elements to source elements with the packer's src_row / src_col (engine.cuh).
 // Reference arithmetic: musev/utils/model_util.py:153-262 (update_pipeline_lora_model) and :468-475 (unload_lora):
 //   delta32 = fl32(scale) * (up @ down)  (fp32),  delta16 = fp16(delta32),  W16 = fp16(float(W16) +- float(delta16)).
 // `scale` already folds in the 0 / 1 block weight of LORA_BLOCK_WEIGHT_MAP (for finite products this gives the same
@@ -21,10 +22,8 @@ static constexpr int kRankChunk = 32; // rank slice staged in shared memory at a
 static constexpr int kMaxRank = 256;
 
 struct LoraDesc {
-  __half* dst;
-  long long ld;
+  PackGeom g;                    // the target's packed layout
   long long tile0;               // first CTA of this target in the flat grid
-  int rows_dst, kdst, nsrc, ksrc, rowmode, p0, p1, colmode, cin, taps;
   int tiles_x;                   // column tiles
   const void* up;                // [nsrc, r]
   const void* down;              // [r, ksrc] (conv: [r, cin, taps] flattened, the source column order)
@@ -32,28 +31,6 @@ struct LoraDesc {
   float scale;
 };
 
-// The packer's index maps (pack_batch_kernel in engine.cu): packed row -> source row, packed column -> source column,
-// -1 for padding that has no source element.
-__device__ __forceinline__ int src_row(const LoraDesc& d, int r) {
-  int s = r;
-  if (d.rowmode == 1) {
-    const int h = r / d.p1, j = r % d.p1;
-    s = j < d.p0 ? h * d.p0 + j : -1;
-  } else if (d.rowmode == 2) {
-    const int chunk = r / 32, j = r % 32;
-    s = j < 16 ? chunk * 16 + j : d.rows_dst / 2 + chunk * 16 + (j - 16);
-  }
-  return (r < d.rows_dst && s >= 0 && s < d.nsrc) ? s : -1;
-}
-__device__ __forceinline__ int src_col(const LoraDesc& d, int kk) {
-  if (kk >= d.kdst) return -1;
-  if (d.colmode == 1) {
-    if (kk >= d.cin * d.taps) return -1;
-    const int tap = kk / d.cin, c = kk % d.cin;
-    return c * d.taps + tap;
-  }
-  return kk < d.ksrc ? kk : -1;
-}
 __device__ __forceinline__ float ld_any(const void* p, long long i, int is_f32) {
   return is_f32 ? reinterpret_cast<const float*>(p)[i] : __half2float(reinterpret_cast<const __half*>(p)[i]);
 }
@@ -74,8 +51,8 @@ __global__ void __launch_bounds__(256) lora_merge_kernel(const LoraDesc* __restr
   const long long t = bid - d.tile0;
   const int row0 = (int)(t / d.tiles_x) * kTile, col0 = (int)(t % d.tiles_x) * kTile;
   const int tid = threadIdx.x, ty = tid / 16, tx = tid % 16;
-  if (tid < kTile) sr[tid] = src_row(d, row0 + tid);
-  else if (tid < 2 * kTile) sc[tid - kTile] = src_col(d, col0 + tid - kTile);
+  if (tid < kTile) sr[tid] = src_row(d.g, row0 + tid);
+  else if (tid < 2 * kTile) sc[tid - kTile] = src_col(d.g, col0 + tid - kTile);
   float acc[4][4];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -93,7 +70,7 @@ __global__ void __launch_bounds__(256) lora_merge_kernel(const LoraDesc* __restr
     for (int idx = tid; idx < kRankChunk * kTile; idx += 256) {
       const int col = idx % kTile, jj = idx / kTile;
       const int s = sc[col];
-      ds[jj][col] = (jj < nj && s >= 0) ? ld_any(d.down, (long long)(j0 + jj) * d.ksrc + s, d.down_f32) : 0.f;
+      ds[jj][col] = (jj < nj && s >= 0) ? ld_any(d.down, (long long)(j0 + jj) * d.g.ksrc + s, d.down_f32) : 0.f;
     }
     __syncthreads();
     for (int jj = 0; jj < nj; ++jj) {
@@ -110,7 +87,7 @@ __global__ void __launch_bounds__(256) lora_merge_kernel(const LoraDesc* __restr
   for (int i = 0; i < 4; ++i) {
     const int row = ty * 4 + i;
     if (sr[row] < 0) continue;                 // head padding rows (and rows past the tile) are never written
-    __half* p = d.dst + (long long)(row0 + row) * d.ld + col0 + tx * 4;
+    __half* p = d.g.dst + (long long)(row0 + row) * d.g.ld + col0 + tx * 4;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       if (sc[tx * 4 + j] < 0) continue;        // zero column padding stays zero
@@ -122,20 +99,13 @@ __global__ void __launch_bounds__(256) lora_merge_kernel(const LoraDesc* __restr
 }
 
 // Inverse of the packer: packed weight -> fp16 [nsrc, ksrc] in the reference layout.
-__global__ void read_weight_kernel(const __half* __restrict__ src, long long ld, LoraDesc d, __half* __restrict__ out) {
-  const long long total = (long long)d.rows_dst * d.kdst;
+__global__ void read_weight_kernel(const PackGeom g, __half* __restrict__ out) {
+  const long long total = (long long)g.rows_dst * g.kdst;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int r = (int)(i / d.kdst), kk = (int)(i % d.kdst);
-    const int s = src_row(d, r), c = src_col(d, kk);
-    if (s >= 0 && c >= 0) out[(long long)s * d.ksrc + c] = src[(long long)r * ld + kk];
+    const int r = (int)(i / g.kdst), kk = (int)(i % g.kdst);
+    const int s = src_row(g, r), c = src_col(g, kk);
+    if (s >= 0 && c >= 0) out[(long long)s * g.ksrc + c] = g.dst[(long long)r * g.ld + kk];
   }
-}
-
-static LoraDesc geometry(const Loader& l) {
-  LoraDesc d{};
-  d.dst = l.dst; d.ld = l.ld; d.rows_dst = l.rows_dst; d.kdst = l.kdst; d.nsrc = l.nsrc; d.ksrc = l.ksrc;
-  d.rowmode = l.rowmode; d.p0 = l.p0; d.p1 = l.p1; d.colmode = l.colmode; d.cin = l.cin; d.taps = l.taps;
-  return d;
 }
 
 static std::string shape_str(const mvb_named_tensor& t) {
@@ -145,7 +115,7 @@ static std::string shape_str(const mvb_named_tensor& t) {
 }
 
 int Engine::merge_lora(const mvb_named_tensor* up, const mvb_named_tensor* down, const float* scale, int n, int subtract) {
-  if (kind_ != 0) { err_ = "mvb_unet_merge_lora: LoRA weights merge into a UNet3DConditionModel handle only"; return MVB_ERR_STATE; }
+  if (kind_ != Kind::UNet) { err_ = "mvb_unet_merge_lora: LoRA weights merge into a UNet3DConditionModel handle only"; return MVB_ERR_STATE; }
   if (!finalized_) { err_ = "mvb_unet_merge_lora: call mvb_finalize first"; return MVB_ERR_STATE; }
   if (n < 0 || (n > 0 && (!up || !down || !scale))) { err_ = "mvb_unet_merge_lora: bad arguments"; return MVB_ERR_INVALID; }
   if (n == 0) return MVB_OK;
@@ -163,29 +133,30 @@ int Engine::merge_lora(const mvb_named_tensor* up, const mvb_named_tensor* down,
       return MVB_ERR_INVALID;
     }
     if (!seen.insert(name).second) { err_ = "mvb_unet_merge_lora: target " + name + " appears twice in one call"; return MVB_ERR_INVALID; }
-    const Loader& l = it->second;
+    const PackGeom& g = it->second.g;
     if (!u.device_ptr || !dn.device_ptr) { err_ = "mvb_unet_merge_lora: null factor for " + name; return MVB_ERR_INVALID; }
     const bool ok_dims = (u.ndim == 2 || u.ndim == 4) && u.ndim == dn.ndim;
     const long long r = ok_dims ? u.shape[1] : 0;
-    bool ok = ok_dims && u.shape[0] == l.nsrc && r >= 1 && dn.shape[0] == r;
+    bool ok = ok_dims && u.shape[0] == g.nsrc && r >= 1 && dn.shape[0] == r;
     if (ok && u.ndim == 4) ok = u.shape[2] == 1 && u.shape[3] == 1;
     if (ok) {
-      if (dn.ndim == 2) ok = dn.shape[1] == l.ksrc && l.colmode == 0;
-      else if (l.colmode == 1) ok = dn.shape[1] == l.cin && dn.shape[2] * dn.shape[3] == l.taps;
-      else ok = dn.shape[1] == l.ksrc && dn.shape[2] == 1 && dn.shape[3] == 1;
+      if (dn.ndim == 2) ok = dn.shape[1] == g.ksrc && g.colmode == 0;
+      else if (g.colmode == 1) ok = dn.shape[1] == g.cin && dn.shape[2] * dn.shape[3] == g.taps;
+      else ok = dn.shape[1] == g.ksrc && dn.shape[2] == 1 && dn.shape[3] == 1;
     }
     if (!ok) {
       err_ = "mvb_unet_merge_lora: factor shapes up " + shape_str(u) + " / down " + shape_str(dn) + " do not fit " + name +
-             " (" + std::to_string(l.nsrc) + " x " + std::to_string(l.ksrc) + ")";
+             " (" + std::to_string(g.nsrc) + " x " + std::to_string(g.ksrc) + ")";
       return MVB_ERR_INVALID;
     }
     if (r > kMaxRank) { err_ = "mvb_unet_merge_lora: rank " + std::to_string(r) + " of " + name + " exceeds 256"; return MVB_ERR_INVALID; }
-    LoraDesc d = geometry(l);
+    LoraDesc d{};
+    d.g = g;
     d.up = u.device_ptr; d.down = dn.device_ptr; d.up_f32 = u.is_f32 ? 1 : 0; d.down_f32 = dn.is_f32 ? 1 : 0;
     d.rank = (int)r; d.scale = scale[i];
-    d.tiles_x = (d.kdst + kTile - 1) / kTile;
+    d.tiles_x = (g.kdst + kTile - 1) / kTile;
     d.tile0 = tiles;
-    tiles += (long long)((d.rows_dst + kTile - 1) / kTile) * d.tiles_x;
+    tiles += (long long)((g.rows_dst + kTile - 1) / kTile) * d.tiles_x;
     descs.push_back(d);
   }
   cudaSetDevice(device_);
@@ -209,13 +180,12 @@ int Engine::read_weight(const char* name, void* dst_f16) {
     err_ = std::string("mvb_debug_read_weight: ") + name + " is not a matrix or convolution weight of this model";
     return MVB_ERR_INVALID;
   }
-  const Loader& l = it->second;
-  if (!l.dst) { err_ = "engine not initialised"; return MVB_ERR_STATE; }
+  const PackGeom& g = it->second.g;
+  if (!g.dst) { err_ = "engine not initialised"; return MVB_ERR_STATE; }
   cudaSetDevice(device_);
-  const LoraDesc d = geometry(l);
-  const long long total = (long long)d.rows_dst * d.kdst;
+  const long long total = (long long)g.rows_dst * g.kdst;
   const int blocks = (int)((total + 255) / 256 < 132 * 32 ? (total + 255) / 256 : 132 * 32);
-  read_weight_kernel<<<blocks, 256>>>(l.dst, l.ld, d, reinterpret_cast<__half*>(dst_f16));
+  read_weight_kernel<<<blocks, 256>>>(g, reinterpret_cast<__half*>(dst_f16));
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) { err_ = std::string("read_weight_kernel: ") + cudaGetErrorString(e); return MVB_ERR_CUDA; }

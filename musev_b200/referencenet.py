@@ -12,60 +12,33 @@ There is no CPU / PyTorch fallback.
 """
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import asdict
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Tuple, Union
+from typing import Dict, List, Tuple, Union
 
 import torch
 
-from . import _capi, ops
-from .controlnet import MvbControlnetArgs, _lib as _cn_lib
+from . import ops
+from ._capi import EngineModel, MvbControlnetArgs, _is_f32, make_config
+# Names callers imported from this module before the binding moved to _capi; they are the binding's own objects.
+from ._capi import lib as _lib  # noqa: F401
 from .schema import ImageProjConfig, ReferenceNetConfig, image_proj_param_shapes, referencenet_param_shapes
-from .unet import MvbConfig, _is_f32, load_weights_batched
-
-_declared = False
 
 
-def _lib():
-    global _declared
-    l = _cn_lib()
-    if not _declared:
-        l.mvb_create_referencenet.argtypes = [C.POINTER(MvbConfig), C.c_int, C.POINTER(C.c_void_p)]
-        l.mvb_create_referencenet.restype = C.c_int
-        l.mvb_referencenet_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(MvbControlnetArgs)]
-        l.mvb_referencenet_workspace_bytes.restype = C.c_longlong
-        l.mvb_referencenet_forward.argtypes = [C.c_void_p, C.POINTER(MvbControlnetArgs), C.c_void_p, C.c_longlong, C.c_void_p]
-        l.mvb_referencenet_forward.restype = C.c_int
-        _declared = True
-    return l
-
-
-class ReferenceNet2D:
+class ReferenceNet2D(EngineModel):
     """CUDA engine behind the call surface of `musev.models.referencenet.ReferenceNet2D` (need_block_embs=True,
     need_self_attn_block_embs=False -- the only configuration the released presets use, referencenet_loader.py:109-118)."""
 
+    _create = "mvb_create_referencenet"
+    _workspace, _forward = "mvb_referencenet_workspace_bytes", "mvb_referencenet_forward"
+
     def __init__(self, config: ReferenceNetConfig, device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16):
-        if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.cfg = config
-        self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
-        self.dtype = dtype
         self.config = SimpleNamespace(**asdict(config))
         self.need_block_embs, self.need_self_attn_block_embs = True, False
-        self._ws: Optional[torch.Tensor] = None
-        self._h = C.c_void_p()
-        self._loaded = False
-        c = MvbConfig()
-        c.in_channels, c.out_channels = config.in_channels, config.in_channels
-        c.num_blocks = len(config.block_out_channels)
-        for i, v in enumerate(config.block_out_channels):
-            c.block_out_channels[i] = v
-        c.layers_per_block, c.heads = config.layers_per_block, config.attention_head_dim
-        c.cross_attention_dim, c.norm_num_groups, c.norm_eps = config.cross_attention_dim, config.norm_num_groups, config.norm_eps
-        rc = _lib().mvb_create_referencenet(C.byref(c), self.device.index or 0, C.byref(self._h))
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_create_referencenet failed ({rc}): unsupported configuration or out of device memory")
+        c = make_config(config.in_channels, config.in_channels, config.block_out_channels, config.layers_per_block,
+                        config.attention_head_dim, config.cross_attention_dim, config.norm_num_groups, config.norm_eps)
+        super().__init__(c, device, dtype)
         self._maps: List[Tuple[int, int]] = [(config.block_out_channels[0], 1)]     # (channels, downscale) of the 12 + 1 maps
         ds, nb = 1, len(config.block_out_channels)
         for i, ch in enumerate(config.block_out_channels):
@@ -82,48 +55,8 @@ class ReferenceNet2D:
         m.load_state_dict(state_dict)
         return m
 
-    def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = True):
-        expected = referencenet_param_shapes(self.cfg)
-        missing = [k for k in expected if k not in state_dict]
-        unexpected = [k for k in state_dict if k not in expected]
-        if strict and (missing or unexpected):
-            raise RuntimeError(f"Error(s) in loading state_dict: missing {missing[:5]} unexpected {unexpected[:5]}")
-        todo = []
-        for name, shape in expected.items():
-            if name not in state_dict:
-                continue
-            t = state_dict[name]
-            if tuple(t.shape) != tuple(shape):
-                raise RuntimeError(f"size mismatch for {name}: {tuple(t.shape)} vs {tuple(shape)}")
-            todo.append((name, t))
-        load_weights_batched(self._h, todo, self.device)
-        l = _lib()
-        rc = l.mvb_finalize(self._h)
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_finalize: {l.mvb_handle_error(self._h).decode()}")
-        self._loaded = True
-        return SimpleNamespace(missing_keys=missing, unexpected_keys=unexpected)
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) and self._h.value:
-                _lib().mvb_destroy(self._h)
-                self._h = C.c_void_p()
-        except Exception:
-            pass
-
-    def eval(self):
-        return self
-
-    def to(self, *args, **kwargs):
-        for a in list(args) + list(kwargs.values()):
-            if isinstance(a, torch.dtype):
-                if a not in (torch.float16, torch.float32):
-                    raise ValueError("musev_b200 computes in fp16 with fp32 accumulation; I/O dtype is fp16 or fp32")
-                self.dtype = a
-            elif isinstance(a, (str, torch.device)) and torch.device(a).type != "cuda":
-                raise RuntimeError("musev_b200 has no CPU path")
-        return self
+    def _param_shapes(self):
+        return referencenet_param_shapes(self.cfg)
 
     @torch.no_grad()
     def forward(self, sample: torch.Tensor, timestep, encoder_hidden_states: torch.Tensor, class_labels=None,
@@ -133,8 +66,7 @@ class ReferenceNet2D:
                 num_frames: int = None, return_ndim: int = 5):
         """Reference: ReferenceNet2D.forward, musev/models/referencenet.py:640-1127. Returns
         (down_block_refer_embs [12 x (b, C, t, h, w)], mid_block_refer_emb, None)."""
-        if not self._loaded:
-            raise RuntimeError("weights not loaded: call load_state_dict first")
+        self._check_loaded()
         for name, v in (("class_labels", class_labels), ("timestep_cond", timestep_cond), ("attention_mask", attention_mask),
                         ("added_cond_kwargs", added_cond_kwargs), ("down_block_additional_residuals", down_block_additional_residuals),
                         ("mid_block_additional_residual", mid_block_additional_residual),
@@ -172,17 +104,7 @@ class ReferenceNet2D:
             a.outs[k] = outs[k].data_ptr()
         a.out_is_f32 = _is_f32(outs[0])
         a.out_frames = frames
-        l = _lib()
-        need = l.mvb_referencenet_workspace_bytes(self._h, C.byref(a))
-        if need < 0:
-            raise _capi.MvbError(f"mvb_referencenet_workspace_bytes: {l.mvb_handle_error(self._h).decode()}")
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = None
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        rc = l.mvb_referencenet_forward(self._h, C.byref(a), self._ws.data_ptr(), self._ws.numel(),
-                                        torch.cuda.current_stream(dev).cuda_stream)
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_referencenet_forward: {l.mvb_handle_error(self._h).decode()}")
+        self._launch(a)
         self._keep = (sample, ehs)
         return outs[:-1], outs[-1], None          # referencenet.py:1116-1127 (self_attn_block_embs is None)
 

@@ -13,124 +13,10 @@ from typing import Any, Dict, Optional, Sequence, Tuple, Union
 
 import torch
 
-from . import _capi
+from ._capi import MAX_REFER, EngineModel, MvbError, MvbNamedTensor, MvbUnetArgs, _is_f32, _named, lib, make_config
+# Names callers imported from this module before the binding moved to _capi; they are the binding's own objects.
+from ._capi import MvbConfig, lib as _lib  # noqa: F401
 from .schema import UNetConfig, preset_config, unet_param_shapes
-
-
-class MvbConfig(C.Structure):
-    _fields_ = [
-        ("in_channels", C.c_int), ("out_channels", C.c_int), ("num_blocks", C.c_int),
-        ("block_out_channels", C.c_int * 4), ("layers_per_block", C.c_int), ("heads", C.c_int),
-        ("cross_attention_dim", C.c_int), ("norm_num_groups", C.c_int), ("norm_eps", C.c_float),
-        ("need_transformer_in", C.c_int), ("use_anivv1_cfg", C.c_int), ("resnet_2d_skip_time_act", C.c_int),
-        ("keep_vision_condtion", C.c_int), ("need_refer_emb", C.c_int), ("ip_adapter_cross_attn", C.c_int),
-        ("need_t2i_ip_adapter", C.c_int),
-    ]
-
-
-MAX_REFER = 16
-
-
-class MvbUnetArgs(C.Structure):
-    _fields_ = [
-        ("sample", C.c_void_p), ("sample_is_f32", C.c_int),
-        ("B", C.c_int), ("T", C.c_int), ("H", C.c_int), ("W", C.c_int),
-        ("timestep", C.c_float),
-        ("encoder_hidden_states", C.c_void_p), ("ehs_is_f32", C.c_int), ("n_text", C.c_int),
-        ("has_sample_index", C.c_int),
-        ("n_vis_cond", C.c_int), ("vis_cond_first", C.c_int),
-        ("sample_frame_rate", C.c_float),
-        ("vision_clip_emb", C.c_void_p), ("clip_is_f32", C.c_int), ("n_clip", C.c_int), ("ip_adapter_scale", C.c_float),
-        ("n_refer", C.c_int),
-        ("refer_embs", C.c_void_p * MAX_REFER), ("refer_t", C.c_int * MAX_REFER), ("refer_h", C.c_int * MAX_REFER),
-        ("refer_w", C.c_int * MAX_REFER),
-        ("mid_refer_emb", C.c_void_p), ("mid_refer_t", C.c_int), ("mid_refer_h", C.c_int), ("mid_refer_w", C.c_int),
-        ("refer_is_f32", C.c_int),
-        ("n_down_residuals", C.c_int), ("down_residuals", C.c_void_p * MAX_REFER),
-        ("mid_residual", C.c_void_p), ("residual_is_f32", C.c_int),
-        ("skip_temporal_layers", C.c_int),
-        ("out", C.c_void_p), ("out_is_f32", C.c_int),
-        ("pose_guider_emb", C.c_void_p), ("pose_is_f32", C.c_int),
-    ]
-
-
-class MvbNamedTensor(C.Structure):
-    _fields_ = [("name", C.c_char_p), ("device_ptr", C.c_void_p), ("is_f32", C.c_int), ("ndim", C.c_int),
-                ("shape", C.c_longlong * 5)]
-
-
-_declared = False
-PACK_BATCH_BYTES = 512 << 20     # source bytes staged on the device per mvb_load_weights call
-
-
-def load_weights_batched(handle, named_tensors, device) -> None:
-    """Feeds (name, tensor) pairs to `mvb_load_weights` in batches of ~PACK_BATCH_BYTES: one host->device staging copy
-    per tensor, ONE packing kernel per batch (the per-tensor entry point costs a launch + a sync per tensor)."""
-    l = _lib()
-    batch, keep, nbytes = [], [], 0
-
-    def flush():
-        nonlocal batch, keep, nbytes
-        if not batch:
-            return
-        arr = (MvbNamedTensor * len(batch))(*batch)
-        rc = l.mvb_load_weights(handle, arr, len(batch))
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_load_weights: {l.mvb_handle_error(handle).decode()}")
-        batch, keep, nbytes = [], [], 0
-
-    for name, t in named_tensors:
-        if t.dtype not in (torch.float16, torch.float32):
-            t = t.float()
-        t = t.to(device).contiguous()
-        e = MvbNamedTensor()
-        e.name, e.device_ptr, e.is_f32, e.ndim = name.encode(), t.data_ptr(), _is_f32(t), t.dim()
-        for i, v in enumerate(t.shape):
-            e.shape[i] = v
-        batch.append(e)
-        keep.append(t)
-        nbytes += t.numel() * t.element_size()
-        if nbytes >= PACK_BATCH_BYTES:
-            torch.cuda.current_stream(device).synchronize()
-            flush()
-    torch.cuda.current_stream(device).synchronize()
-    flush()
-
-
-def _lib():
-    global _declared
-    l = _capi.lib()
-    if not _declared:
-        l.mvb_create.argtypes = [C.POINTER(MvbConfig), C.c_int, C.POINTER(C.c_void_p)]
-        l.mvb_create.restype = C.c_int
-        l.mvb_destroy.argtypes = [C.c_void_p]
-        l.mvb_destroy.restype = None
-        l.mvb_load_weight.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.POINTER(C.c_longlong), C.c_int]
-        l.mvb_load_weight.restype = C.c_int
-        l.mvb_load_weights.argtypes = [C.c_void_p, C.POINTER(MvbNamedTensor), C.c_int]
-        l.mvb_load_weights.restype = C.c_int
-        l.mvb_finalize.argtypes = [C.c_void_p]
-        l.mvb_finalize.restype = C.c_int
-        l.mvb_num_params.argtypes = [C.c_void_p]
-        l.mvb_num_params.restype = C.c_int
-        l.mvb_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(MvbUnetArgs)]
-        l.mvb_workspace_bytes.restype = C.c_longlong
-        l.mvb_unet_forward.argtypes = [C.c_void_p, C.POINTER(MvbUnetArgs), C.c_void_p, C.c_longlong, C.c_void_p]
-        l.mvb_unet_forward.restype = C.c_int
-        l.mvb_handle_error.argtypes = [C.c_void_p]
-        l.mvb_handle_error.restype = C.c_char_p
-        l.mvb_debug_num_taps.argtypes = [C.c_void_p]
-        l.mvb_debug_num_taps.restype = C.c_int
-        l.mvb_debug_tap.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.POINTER(C.c_void_p),
-                                    C.POINTER(C.c_longlong), C.POINTER(C.c_int)]
-        l.mvb_debug_tap.restype = C.c_int
-        l.mvb_unet_merge_lora.argtypes = [C.c_void_p, C.POINTER(MvbNamedTensor), C.POINTER(MvbNamedTensor),
-                                          C.POINTER(C.c_float), C.c_int, C.c_int]
-        l.mvb_unet_merge_lora.restype = C.c_int
-        l.mvb_debug_read_weight.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
-        l.mvb_debug_read_weight.restype = C.c_int
-        _declared = True
-    return l
 
 
 @dataclass
@@ -140,22 +26,6 @@ class UNet3DConditionOutput:
 
     def __getitem__(self, i):
         return (self.sample,)[i]
-
-
-def _named(name: str, t: torch.Tensor) -> MvbNamedTensor:
-    e = MvbNamedTensor()
-    e.name, e.device_ptr, e.is_f32, e.ndim = name.encode(), t.data_ptr(), _is_f32(t), t.dim()
-    for i, v in enumerate(t.shape):
-        e.shape[i] = v
-    return e
-
-
-def _is_f32(t: torch.Tensor) -> int:
-    if t.dtype == torch.float32:
-        return 1
-    if t.dtype == torch.float16:
-        return 0
-    raise ValueError(f"musev_b200 takes float16 or float32 tensors, got {t.dtype}")
 
 
 def check_pose_guider_emb(emb: torch.Tensor, B: int, T: int, c0: int, H: int, W: int) -> None:
@@ -180,44 +50,30 @@ def _contiguous_index_range(idx, name) -> Tuple[int, int]:
     return v[0], len(v)
 
 
-class UNet3DConditionModel:
+class UNet3DConditionModel(EngineModel):
     """CUDA engine behind the call surface of the reference model (musev/models/unet_3d_condition.py:179).
 
     Kept: `forward` signature and return type (:773-803, :1277-1280), `.config`, `.dtype`, `.device`,
-    `.ip_adapter_cross_attn`, `.set_skip_temporal_layers` (:1639), `.to()`, `.eval()`, reference state-dict names.
+    `.ip_adapter_cross_attn`, `.set_skip_temporal_layers` (:1639), `.to()`, `.eval()`, reference state-dict names
+    (load_state_dict: from_pretrained_2d / load_state_dict, unet_3d_condition.py:1284-1637).
     """
 
+    _create, _workspace, _forward = "mvb_create", "mvb_workspace_bytes", "mvb_unet_forward"
+
     def __init__(self, config: UNetConfig, device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16):
-        if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.cfg = config
-        self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
-        self.dtype = dtype
         self.config = SimpleNamespace(**config.to_dict())
         self.ip_adapter_cross_attn = config.ip_adapter_cross_attn
         self.need_refer_emb = config.need_refer_emb
         self.skip_temporal_layers = False
         self.skip_refer_downblock_emb = False
-        self._ws: Optional[torch.Tensor] = None
-        self._h = C.c_void_p()
-        self._loaded = False
-        c = MvbConfig()
-        c.in_channels, c.out_channels = config.in_channels, config.out_channels
-        c.num_blocks = len(config.block_out_channels)
-        for i, v in enumerate(config.block_out_channels):
-            c.block_out_channels[i] = v
-        c.layers_per_block, c.heads = config.layers_per_block, config.attention_head_dim
-        c.cross_attention_dim, c.norm_num_groups, c.norm_eps = config.cross_attention_dim, config.norm_num_groups, config.norm_eps
-        c.need_transformer_in = int(config.need_transformer_in)
-        c.use_anivv1_cfg = int(config.use_anivv1_cfg)
-        c.resnet_2d_skip_time_act = int(config.resnet_2d_skip_time_act)
-        c.keep_vision_condtion = int(config.keep_vision_condtion)
-        c.need_refer_emb = int(config.need_refer_emb)
-        c.ip_adapter_cross_attn = int(config.ip_adapter_cross_attn)
-        c.need_t2i_ip_adapter = int(config.need_t2i_ip_adapter)
-        rc = _lib().mvb_create(C.byref(c), self.device.index or 0, C.byref(self._h))
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_create failed ({rc}): unsupported configuration or out of device memory")
+        c = make_config(config.in_channels, config.out_channels, config.block_out_channels, config.layers_per_block,
+                        config.attention_head_dim, config.cross_attention_dim, config.norm_num_groups, config.norm_eps,
+                        need_transformer_in=config.need_transformer_in, use_anivv1_cfg=config.use_anivv1_cfg,
+                        resnet_2d_skip_time_act=config.resnet_2d_skip_time_act,
+                        keep_vision_condtion=config.keep_vision_condtion, need_refer_emb=config.need_refer_emb,
+                        ip_adapter_cross_attn=config.ip_adapter_cross_attn, need_t2i_ip_adapter=config.need_t2i_ip_adapter)
+        super().__init__(c, device, dtype)
 
     # ------------------------------------------------------------------ construction helpers
     @classmethod
@@ -227,51 +83,8 @@ class UNet3DConditionModel:
         m.load_state_dict(state_dict)
         return m
 
-    def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = True):
-        """Reference: from_pretrained_2d / load_state_dict (unet_3d_condition.py:1284-1637). Tensors are packed into
-        the kernel layouts on the device in batches (peak extra memory = one ~512 MB staging batch)."""
-        expected = unet_param_shapes(self.cfg)
-        missing = [k for k in expected if k not in state_dict]
-        unexpected = [k for k in state_dict if k not in expected]
-        if strict and (missing or unexpected):
-            raise RuntimeError(f"Error(s) in loading state_dict: missing {missing[:5]} unexpected {unexpected[:5]}")
-        l = _lib()
-        todo = []
-        for name, shape in expected.items():
-            if name not in state_dict:
-                continue
-            t = state_dict[name]
-            if tuple(t.shape) != tuple(shape):
-                raise RuntimeError(f"size mismatch for {name}: {tuple(t.shape)} vs {tuple(shape)}")
-            todo.append((name, t))
-        load_weights_batched(self._h, todo, self.device)
-        rc = l.mvb_finalize(self._h)
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_finalize: {l.mvb_handle_error(self._h).decode()}")
-        self._loaded = True
-        return SimpleNamespace(missing_keys=missing, unexpected_keys=unexpected)
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) and self._h.value:
-                _lib().mvb_destroy(self._h)
-                self._h = C.c_void_p()
-        except Exception:
-            pass
-
-    # ------------------------------------------------------------------ nn.Module-like surface
-    def eval(self):
-        return self
-
-    def to(self, *args, **kwargs):
-        for a in list(args) + list(kwargs.values()):
-            if isinstance(a, torch.dtype):
-                if a not in (torch.float16, torch.float32):
-                    raise ValueError("musev_b200 computes in fp16 with fp32 accumulation; I/O dtype is fp16 or fp32")
-                self.dtype = a
-            elif isinstance(a, (str, torch.device)) and torch.device(a).type != "cuda":
-                raise RuntimeError("musev_b200 has no CPU path")
-        return self
+    def _param_shapes(self):
+        return unet_param_shapes(self.cfg)
 
     def set_skip_temporal_layers(self, valid: bool, ignore_names=()):
         """musev/models/unet_3d_condition.py:1639-1661 (temporal layers + ReferenceNet down-block fusion)."""
@@ -312,8 +125,7 @@ class UNet3DConditionModel:
         pose_guider_emb: torch.Tensor = None,
     ):
         """Reference: UNet3DConditionModel.forward, musev/models/unet_3d_condition.py:773-1280."""
-        if not self._loaded:
-            raise RuntimeError("weights not loaded: call load_state_dict first")
+        self._check_loaded()
         for name, v in (("class_labels", class_labels), ("timestep_cond", timestep_cond), ("attention_mask", attention_mask),
                         ("frame_index", frame_index), ("refer_self_attn_emb", refer_self_attn_emb),
                         ("face_emb", face_emb), ("ip_adapter_face_emb", ip_adapter_face_emb)):
@@ -394,17 +206,7 @@ class UNet3DConditionModel:
         a.skip_temporal_layers = int(self.skip_temporal_layers)
         out = torch.empty((B, self.cfg.out_channels, T, H, W), dtype=sample.dtype, device=dev)
         a.out, a.out_is_f32 = out.data_ptr(), _is_f32(out)
-        l = _lib()
-        need = l.mvb_workspace_bytes(self._h, C.byref(a))
-        if need < 0:
-            raise _capi.MvbError(f"mvb_workspace_bytes: {l.mvb_handle_error(self._h).decode()}")
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = None
-            self._ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
-        rc = l.mvb_unet_forward(self._h, C.byref(a), self._ws.data_ptr(), self._ws.numel(),
-                                torch.cuda.current_stream(dev).cuda_stream)
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_unet_forward ({rc}): {l.mvb_handle_error(self._h).decode()}")
+        self._launch(a)
         self._keep = keep  # inputs must outlive the asynchronous launch sequence
         if skip_temporal_layers is not None:
             self.set_skip_temporal_layers(not skip_temporal_layers)   # unet_3d_condition.py:1275-1276
@@ -429,27 +231,14 @@ class UNet3DConditionModel:
         down_arr = (MvbNamedTensor * max(n, 1))(*[_named(nm, d) for nm, d in zip(targets, downs)])
         sc = (C.c_float * max(n, 1))(*[float(s) for s in scales])
         torch.cuda.current_stream(self.device).synchronize()      # the factors may still be in flight
-        l = _lib()
-        rc = l.mvb_unet_merge_lora(self._h, up_arr, down_arr, sc, n, int(bool(subtract)))
+        rc = lib().mvb_unet_merge_lora(self._h, up_arr, down_arr, sc, n, int(bool(subtract)))
         if rc != 0:
-            raise _capi.MvbError(f"mvb_unet_merge_lora ({rc}): {l.mvb_handle_error(self._h).decode()}")
-
-    def debug_weight(self, name: str) -> torch.Tensor:
-        """The packed matrix / convolution weight `name` read back into its reference shape, fp16 on the device."""
-        shape = unet_param_shapes(self.cfg).get(name)
-        if shape is None or len(shape) < 2:
-            raise ValueError(f"{name} is not a matrix or convolution weight of this UNet")
-        out = torch.empty(shape, dtype=torch.float16, device=self.device)
-        l = _lib()
-        rc = l.mvb_debug_read_weight(self._h, name.encode(), out.data_ptr())
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_debug_read_weight ({rc}): {l.mvb_handle_error(self._h).decode()}")
-        return out
+            raise MvbError(f"mvb_unet_merge_lora ({rc}): {self._error()}")
 
     # ------------------------------------------------------------------ debug
     def debug_taps(self) -> Dict[str, torch.Tensor]:
         """Layer outputs of the last forward as [(b t), C, h*w]-ordered channels-last copies (fp32, [rows, C])."""
-        l = _lib()
+        l = lib()
         out = {}
         torch.cuda.synchronize()
         base = self._ws.data_ptr()

@@ -15,44 +15,16 @@ for a whole video in the library. `AutoencoderKL` holds both halves and stands i
 """
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import asdict, dataclass
 from types import SimpleNamespace
 from typing import Dict, Optional, Union
 
 import torch
 
-from . import _capi
+from ._capi import EngineModel, make_config
+# Names callers imported from this module before the binding moved to _capi; they are the binding's own objects.
+from ._capi import MvbVaeDecodeArgs, lib as _lib  # noqa: F401
 from .schema import VAEConfig, vae_decoder_param_shapes, vae_encoder_param_shapes
-from .unet import MvbConfig, _is_f32, _lib as _unet_lib, load_weights_batched
-
-
-class MvbVaeDecodeArgs(C.Structure):
-    _fields_ = [("latents", C.c_void_p), ("latents_is_f32", C.c_int), ("N", C.c_int), ("h", C.c_int), ("w", C.c_int),
-                ("latent_scale", C.c_float), ("out", C.c_void_p), ("out_is_f32", C.c_int), ("postprocess", C.c_int)]
-
-
-_declared = False
-
-
-def _lib():
-    global _declared
-    l = _unet_lib()
-    if not _declared:
-        l.mvb_create_vae_decoder.argtypes = [C.POINTER(MvbConfig), C.c_int, C.POINTER(C.c_void_p)]
-        l.mvb_create_vae_decoder.restype = C.c_int
-        l.mvb_vae_decode_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(MvbVaeDecodeArgs)]
-        l.mvb_vae_decode_workspace_bytes.restype = C.c_longlong
-        l.mvb_vae_decode.argtypes = [C.c_void_p, C.POINTER(MvbVaeDecodeArgs), C.c_void_p, C.c_longlong, C.c_void_p]
-        l.mvb_vae_decode.restype = C.c_int
-        l.mvb_create_vae_encoder.argtypes = [C.POINTER(MvbConfig), C.c_int, C.POINTER(C.c_void_p)]
-        l.mvb_create_vae_encoder.restype = C.c_int
-        l.mvb_vae_encode_workspace_bytes.argtypes = [C.c_void_p, C.POINTER(MvbVaeDecodeArgs)]
-        l.mvb_vae_encode_workspace_bytes.restype = C.c_longlong
-        l.mvb_vae_encode.argtypes = [C.c_void_p, C.POINTER(MvbVaeDecodeArgs), C.c_void_p, C.c_longlong, C.c_void_p]
-        l.mvb_vae_encode.restype = C.c_int
-        _declared = True
-    return l
 
 
 @dataclass
@@ -97,108 +69,26 @@ class AutoencoderKLOutput:
         return (self.latent_dist,)[i]
 
 
-class _EngineHalf:
-    """One engine handle of a VAE half: creation from a `VAEConfig`, weight loading by reference names, chunked calls."""
-
-    _kind = ""                      # "decoder" / "encoder": selects the C entry points
-    _own: tuple = ()                # state-dict prefixes of this half
-    _other: tuple = ()              # prefixes of the other half (ignored by load_state_dict)
+class _VaeHalf(EngineModel):
+    """One engine handle of a VAE half, created from a `VAEConfig`; entries of the other half in a full VAE state dict are
+    ignored by load_state_dict."""
 
     def __init__(self, config: VAEConfig, device, dtype, frames_per_call, in_channels, out_channels):
-        if not torch.cuda.is_available():
-            raise RuntimeError("musev_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.cfg = config
-        self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
-        self.dtype = dtype
         self.config = SimpleNamespace(**asdict(config))
         self.frames_per_call = int(frames_per_call)
-        self._ws: Optional[torch.Tensor] = None
-        self._h = C.c_void_p()
-        self._loaded = False
-        c = MvbConfig()
-        c.in_channels, c.out_channels = in_channels, out_channels
-        c.num_blocks = len(config.block_out_channels)
-        for i, v in enumerate(config.block_out_channels):
-            c.block_out_channels[i] = v
-        c.layers_per_block, c.heads = config.layers_per_block, 1
-        c.cross_attention_dim, c.norm_num_groups, c.norm_eps = 64, config.norm_num_groups, 1e-6
-        create = getattr(_lib(), f"mvb_create_vae_{self._kind}")
-        rc = create(C.byref(c), self.device.index or 0, C.byref(self._h))
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_create_vae_{self._kind} failed ({rc}): unsupported configuration or out of device memory")
-
-    def _param_shapes(self):
-        raise NotImplementedError
-
-    def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = True):
-        expected = self._param_shapes()
-        missing = [k for k in expected if k not in state_dict]
-        unexpected = [k for k in state_dict if k not in expected and not k.startswith(self._other)]
-        if strict and (missing or unexpected):
-            raise RuntimeError(f"Error(s) in loading state_dict: missing {missing[:5]} unexpected {unexpected[:5]}")
-        todo = []
-        for name, shape in expected.items():
-            if name not in state_dict:
-                continue
-            t = state_dict[name]
-            if tuple(t.shape) != tuple(shape):
-                raise RuntimeError(f"size mismatch for {name}: {tuple(t.shape)} vs {tuple(shape)}")
-            todo.append((name, t))
-        load_weights_batched(self._h, todo, self.device)
-        l = _lib()
-        rc = l.mvb_finalize(self._h)
-        if rc != 0:
-            raise _capi.MvbError(f"mvb_finalize: {l.mvb_handle_error(self._h).decode()}")
-        self._loaded = True
-        return SimpleNamespace(missing_keys=missing, unexpected_keys=unexpected)
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) and self._h.value:
-                _lib().mvb_destroy(self._h)
-                self._h = C.c_void_p()
-        except Exception:
-            pass
-
-    def eval(self):
-        return self
-
-    def _call(self, x: torch.Tensor, out: torch.Tensor, h: int, w: int, latent_scale: float, postprocess: int) -> torch.Tensor:
-        """Runs the half on x [N, ...] -> out [N, ...] in chunks of `frames_per_call` frames; h, w = latent size."""
-        l = _lib()
-        ws_fn = getattr(l, "mvb_vae_decode_workspace_bytes" if self._kind == "decoder" else "mvb_vae_encode_workspace_bytes")
-        run_fn = getattr(l, "mvb_vae_decode" if self._kind == "decoder" else "mvb_vae_encode")
-        N = x.shape[0]
-        step = max(1, self.frames_per_call)
-        for n0 in range(0, N, step):
-            n1 = min(N, n0 + step)
-            a = MvbVaeDecodeArgs()
-            xc, oc = x[n0:n1], out[n0:n1]
-            a.latents, a.latents_is_f32 = xc.data_ptr(), _is_f32(xc)
-            a.N, a.h, a.w = n1 - n0, h, w
-            a.latent_scale = float(latent_scale)
-            a.out, a.out_is_f32 = oc.data_ptr(), _is_f32(oc)
-            a.postprocess = int(postprocess)
-            need = ws_fn(self._h, C.byref(a))
-            if need < 0:
-                raise _capi.MvbError(f"{ws_fn.__name__}: {l.mvb_handle_error(self._h).decode()}")
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = None
-                self._ws = torch.empty(int(need), dtype=torch.uint8, device=self.device)
-            rc = run_fn(self._h, C.byref(a), self._ws.data_ptr(), self._ws.numel(), torch.cuda.current_stream(self.device).cuda_stream)
-            if rc != 0:
-                raise _capi.MvbError(f"{run_fn.__name__}: {l.mvb_handle_error(self._h).decode()}")
-        self._keep = x
-        return out
+        c = make_config(in_channels, out_channels, config.block_out_channels, config.layers_per_block, 1, 64,
+                        config.norm_num_groups, 1e-6)
+        super().__init__(c, device, dtype)
 
 
-class AutoencoderKLDecoder(_EngineHalf):
+class AutoencoderKLDecoder(_VaeHalf):
     """Decode half of `AutoencoderKL` on the CUDA engine: `.decode(z)` (autoencoder_kl.py:275-302) and the pipeline-level
     `.decode_latents(latents)`; `.config.scaling_factor`, `.dtype`, `.device`, reference state-dict names (`decoder.*`,
     `post_quant_conv.*`; encoder / quant_conv entries of a full VAE state dict are ignored)."""
 
-    _kind = "decoder"
-    _other = ("encoder.", "quant_conv.")
+    _create, _workspace, _forward = "mvb_create_vae_decoder", "mvb_vae_decode_workspace_bytes", "mvb_vae_decode"
+    _ignored = ("encoder.", "quant_conv.")
 
     def __init__(self, config: VAEConfig = VAEConfig(), device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16,
                  frames_per_call: int = 4):
@@ -208,8 +98,7 @@ class AutoencoderKLDecoder(_EngineHalf):
         return vae_decoder_param_shapes(self.cfg)
 
     def _run(self, z: torch.Tensor, latent_scale: float, postprocess: bool, out_dtype: torch.dtype) -> torch.Tensor:
-        if not self._loaded:
-            raise RuntimeError("weights not loaded: call load_state_dict first")
+        self._check_loaded()
         if z.dim() != 4 or z.shape[1] != self.cfg.latent_channels:
             raise ValueError(f"latents must be [N, {self.cfg.latent_channels}, h, w], got {tuple(z.shape)}")
         z = z.to(self.device)
@@ -219,7 +108,7 @@ class AutoencoderKLDecoder(_EngineHalf):
         N, _, h, w = z.shape
         up = 2 ** (len(self.cfg.block_out_channels) - 1)
         out = torch.empty((N, self.cfg.out_channels, h * up, w * up), dtype=out_dtype, device=self.device)
-        return self._call(z, out, h, w, latent_scale, postprocess)
+        return self._launch_frames(z, out, h, w, latent_scale, postprocess)
 
     @torch.no_grad()
     def decode(self, z: torch.Tensor, return_dict: bool = True):
@@ -240,14 +129,14 @@ class AutoencoderKLDecoder(_EngineHalf):
         return img.view(b, f, *img.shape[1:]).permute(0, 2, 1, 3, 4).contiguous()
 
 
-class AutoencoderKLEncoder(_EngineHalf):
+class AutoencoderKLEncoder(_VaeHalf):
     """Encode half of `AutoencoderKL` on the CUDA engine: `.encode(x)` (autoencoder_kl.py:256-297) and `.encode_video(video)`;
     reference state-dict names (`encoder.*`, `quant_conv.*`; decoder / post_quant_conv entries of a full VAE state dict are
     ignored). The engine computes in fp16 with fp32 accumulation and statistics; conv_out and quant_conv stay in fp32.
     The moments come back in the input's dtype, as the reference returns them (autoencoder_kl.py:286-290)."""
 
-    _kind = "encoder"
-    _other = ("decoder.", "post_quant_conv.")
+    _create, _workspace, _forward = "mvb_create_vae_encoder", "mvb_vae_encode_workspace_bytes", "mvb_vae_encode"
+    _ignored = ("decoder.", "post_quant_conv.")
 
     def __init__(self, config: VAEConfig = VAEConfig(), device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16,
                  frames_per_call: int = 4):
@@ -257,8 +146,7 @@ class AutoencoderKLEncoder(_EngineHalf):
         return vae_encoder_param_shapes(self.cfg)
 
     def _run(self, x: torch.Tensor, postprocess: int, out_dtype: torch.dtype) -> torch.Tensor:
-        if not self._loaded:
-            raise RuntimeError("weights not loaded: call load_state_dict first")
+        self._check_loaded()
         f = 2 ** (len(self.cfg.block_out_channels) - 1)
         if x.dim() != 4 or x.shape[1] != self.cfg.in_channels:
             raise ValueError(f"images must have {self.cfg.in_channels} channels ([N, {self.cfg.in_channels}, H, W]), got {tuple(x.shape)}")
@@ -274,7 +162,7 @@ class AutoencoderKLEncoder(_EngineHalf):
         x = x.contiguous()
         zc = self.cfg.latent_channels
         out = torch.empty((N, zc if postprocess else 2 * zc, h, w), dtype=out_dtype, device=self.device)
-        return self._call(x, out, h, w, self.cfg.scaling_factor, postprocess)
+        return self._launch_frames(x, out, h, w, self.cfg.scaling_factor, postprocess)
 
     @torch.no_grad()
     def encode(self, x: torch.Tensor, return_dict: bool = True):

@@ -213,7 +213,8 @@ def test_rejected_calls_change_no_weight(built_lib):
     from musev_b200._capi import MvbError
     from musev_b200.controlnet import ControlNetModel
     from musev_b200.schema import ControlNetConfig
-    from musev_b200.unet import MvbNamedTensor, UNet3DConditionModel, _lib, _named
+    from musev_b200._capi import MvbNamedTensor, _named, lib
+    from musev_b200.unet import UNet3DConditionModel
     cfg = preset_config("musev", block_out_channels=NARROW)
     sd16 = {k: v.half() for k, v in make_state_dict(cfg, seed=0).items()}
     model = _model(cfg, sd16)
@@ -236,7 +237,7 @@ def test_rejected_calls_change_no_weight(built_lib):
     cn = ControlNetModel(ControlNetConfig(block_out_channels=NARROW), device=dev)
     arr_u, arr_d = (MvbNamedTensor * 1)(_named(a, up_a)), (MvbNamedTensor * 1)(_named(a, down_a))
     import ctypes as C
-    assert _lib().mvb_unet_merge_lora(cn._h, arr_u, arr_d, (C.c_float * 1)(1.0), 1, 0) == -3
+    assert lib().mvb_unet_merge_lora(cn._h, arr_u, arr_d, (C.c_float * 1)(1.0), 1, 0) == -3
     for n in mats:
         assert torch.equal(model.debug_weight(n), before[n]), n
 

@@ -116,6 +116,27 @@ def test_pose_guider_full_512_vs_oracle(built_lib):
     assert torch.equal(again[0], out[0, :, 1])
 
 
+@pytest.mark.parametrize("cfg", CONFIGS, ids=["narrow", "script"])
+def test_packed_weights_read_back_bit_exact(built_lib, cfg):
+    """Every weight reads back from its packed layout bit for bit. The layers alternate between the per-tensor and the
+    batched load; the script config's blocks.4 / blocks.5 read 96 channels stored as 128 (zero padding columns)."""
+    from musev_b200 import _capi
+    from musev_b200.controlnet import PoseGuider
+    sd = {k: v.half().to(dev).contiguous() for k, v in make_pose_guider_state_dict(cfg, seed=5).items()}
+    pg = PoseGuider(cfg.conditioning_embedding_channels, cfg.conditioning_channels, cfg.block_out_channels, device=dev)
+    layers = list(dict.fromkeys(n.rsplit(".", 1)[0] for n in sd))
+    per_tensor = [n for n in sd if layers.index(n.rsplit(".", 1)[0]) % 2 == 0]
+    l = _capi.lib()
+    for name in per_tensor:
+        t = sd[name]
+        shape = (C.c_longlong * t.dim())(*t.shape)
+        assert l.mvb_load_weight(pg._h, name.encode(), t.data_ptr(), 0, shape, t.dim()) == 0, pg._error()
+    _capi.load_weights_batched(pg._h, [(n, t) for n, t in sd.items() if n not in per_tensor], pg.device)
+    assert l.mvb_finalize(pg._h) == 0, pg._error()
+    bad = [n for n, t in sd.items() if t.dim() > 1 and not torch.equal(pg.debug_weight(n).view(torch.int16), t.view(torch.int16))]
+    assert not bad, bad
+
+
 def _unet(preset):
     from musev_b200.unet import UNet3DConditionModel
     from oracle.pose_guider_oracle import UNet3DPoseOracle
@@ -204,8 +225,8 @@ def test_parallel_denoise_loop_with_pose_emb_vs_oracle_loop(built_lib):
 
 def test_rejects_bad_shapes_before_any_launch(built_lib):
     from musev_b200 import _capi
-    from musev_b200.controlnet import PoseGuider, _lib
-    from musev_b200.vae import MvbVaeDecodeArgs
+    from musev_b200._capi import MvbVaeDecodeArgs
+    from musev_b200.controlnet import PoseGuider
     with pytest.raises(_capi.MvbError, match="mvb_create_pose_guider"):
         PoseGuider(320, 3, (16, 256), device=dev)                     # a 16-channel layer cannot produce 256 channels
     pg, _ = _pose_guider(CONFIGS[0], 21)
@@ -213,7 +234,7 @@ def test_rejects_bad_shapes_before_any_launch(built_lib):
     for bad in (torch.zeros(1, 3, 2, 60, 64), torch.zeros(1, 4, 2, 64, 64), torch.zeros(3, 64, 64), torch.zeros(1, 3, 2, 4, 8)):
         with pytest.raises(ValueError):
             pg(bad.to(dev))
-    l = _lib()
+    l = _capi.lib()
     x = torch.zeros(1, 3, 64, 64, device=dev)
     out = torch.zeros(1, 64, 8, 8, device=dev)
     ws = torch.empty(1 << 20, dtype=torch.uint8, device=dev)

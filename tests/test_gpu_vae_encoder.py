@@ -143,7 +143,8 @@ def test_autoencoderkl_drop_in(built_lib):
 def test_vae_encode_rejects_bad_shapes_before_launch(built_lib):
     from musev_b200 import _capi
     from musev_b200.schema import VAEConfig
-    from musev_b200.vae import AutoencoderKLEncoder, MvbVaeDecodeArgs, _lib
+    from musev_b200._capi import MvbVaeDecodeArgs
+    from musev_b200.vae import AutoencoderKLEncoder
     cfg = VAEConfig(block_out_channels=(64, 64, 128, 128))
     enc = AutoencoderKLEncoder(cfg, device=dev, dtype=torch.float16)
     enc.load_state_dict(_sd16(cfg))
@@ -154,7 +155,7 @@ def test_vae_encode_rejects_bad_shapes_before_launch(built_lib):
             enc.encode(torch.zeros(shape, device=dev, dtype=torch.float16))
     assert _capi.launch_count(-1) == n0
     # the library checks the latent size itself, before any launch
-    l = _lib()
+    l = _capi.lib()
     x = torch.zeros(1, 3, 1024, 768, device=dev, dtype=torch.float16)
     out = torch.empty(1, 8, 128, 96, device=dev, dtype=torch.float16)
     a = MvbVaeDecodeArgs()

@@ -192,13 +192,13 @@ def test_parallel_denoiser_pose_emb_under_cfg_split_two_ranks(tmp_path):
 
 def test_ctypes_argtypes_of_pose_guider_entry_points(built_lib):
     from test_capi_symbols import _prototypes
-    from musev_b200 import controlnet, unet
+    from musev_b200 import _capi
     protos = _prototypes()
-    lib = controlnet._lib()
+    lib = _capi.lib()
     for name in ("mvb_create_pose_guider", "mvb_pose_guider_workspace_bytes", "mvb_pose_guider_forward"):
         assert name in protos
         assert len(getattr(lib, name).argtypes) == protos[name], name
     # mvb_unet_args grew at the end only: every earlier field keeps its offset
-    names = [f[0] for f in unet.MvbUnetArgs._fields_]
+    names = [f[0] for f in _capi.MvbUnetArgs._fields_]
     assert names[-2:] == ["pose_guider_emb", "pose_is_f32"] and names[-4:-2] == ["out", "out_is_f32"]
-    assert unet._lib().mvb_version() >= 2
+    assert lib.mvb_version() >= 2

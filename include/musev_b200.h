@@ -54,7 +54,7 @@ typedef struct mvb_conv_gemm_desc {
   const void* residual; long long ld_res;
   float alpha, beta;
   int geglu;
-  int act; /* 0 none, 1 SiLU */
+  int act; /* 0 none, 1 SiLU, 2 GELU (erf), 3 quick-GELU x * sigmoid(1.702 x); 2 / 3 ignore geglu = 1 */
   int out_f32; /* store fp32 (no residual / geglu) */
   int stride2; /* 3x3 stride-2 conv of a contiguous [NF,H,W,c0] input with even H, W (taps ignored); 0: off,
                   1: pad 1 on every side (UNet Downsample2D), 2: pad (0, 1, 0, 1) = right / bottom only
@@ -373,6 +373,40 @@ int mvb_vae_encode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspa
 int mvb_create_pose_guider(const mvb_config* cfg, int device, mvb_handle** out);
 long long mvb_pose_guider_workspace_bytes(mvb_handle* h, const mvb_vae_decode_args* args);
 int mvb_pose_guider_forward(mvb_handle* h, const mvb_vae_decode_args* args, void* workspace, long long workspace_bytes,
+                            void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * CLIP vision tower, the IP-Adapter image encoder, once per pipeline call before the denoise loop (since mvb_version 3).
+ * Reference: transformers `CLIPVisionModelWithProjection.forward(pixel_values)` (models/clip/modeling_clip.py) as
+ * `get_ip_adapter_image_emb` runs it (musev/pipelines/pipeline_controlnet.py:686-780, through MMCM's
+ * ImageClipVisionFeatureExtractor): patch conv (no bias), class + position embeddings, pre_layrnorm, pre-norm encoder
+ * layers (LayerNorm, q/k/v with bias, softmax(q k^T d^-0.5) v, out_proj + residual; LayerNorm, fc1, activation, fc2 +
+ * residual), then post_layernorm on token 0 and visual_projection (no bias). Image preprocessing (resize, crop, normalise)
+ * stays with the caller. The handle is created from an `mvb_config` whose fields mean, for the CLIP vision tower:
+ *   in_channels           image channels (`num_channels`, 1..4);
+ *   out_channels          `projection_dim` (a multiple of 8);
+ *   block_out_channels    {hidden_size (multiple of 64, <= 2048), intermediate_size (multiple of 64), patch_size, image_size};
+ *   num_blocks            must be 4 (the four entries above);
+ *   layers_per_block      `num_hidden_layers`;
+ *   heads                 `num_attention_heads`; hidden_size / heads a multiple of 8 and at most 192;
+ *   norm_eps              `layer_norm_eps` of every LayerNorm;
+ *   norm_num_groups       the MLP activation `hidden_act`: 2 gelu (erf), 3 quick_gelu (the act codes of mvb_conv_gemm_desc);
+ *   other fields are ignored.
+ * Weights by the `CLIPVisionModelWithProjection.state_dict()` names (`vision_model.*`, `visual_projection.weight`).
+ * It takes `mvb_controlnet_args`, whose fields mean, for the CLIP vision tower:
+ *   sample / sample_is_f32   pixel_values [NF, in_channels, S, S], NCHW fp16 / fp32;
+ *   NF                       images, 1..1024;
+ *   H, W                     S; both must equal image_size (no position-embedding interpolation);
+ *   n_out                    must be 2;
+ *   outs[0]                  image_embeds [NF, projection_dim], or NULL;
+ *   outs[1]                  last_hidden_state [NF, (S / patch)^2 + 1, hidden_size] (the encoder output, not
+ *                            post-normalised), or NULL; at least one of the two must be given;
+ *   out_is_f32               both outputs fp32 (1) or fp16 (0);
+ *   other fields are ignored.
+ * Bad arguments are rejected before any launch (negative return, mvb_handle_error). */
+int mvb_create_clip_vision(const mvb_config* cfg, int device, mvb_handle** out);
+long long mvb_clip_vision_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args);
+int mvb_clip_vision_forward(mvb_handle* h, const mvb_controlnet_args* args, void* workspace, long long workspace_bytes,
                             void* stream);
 
 #ifdef __cplusplus

@@ -6,7 +6,7 @@ importing this package does not load it, using any op does -- and fails loudly i
 from .schema import UNetConfig, preset_config, unet_param_shapes  # noqa: F401
 
 __all__ = ["UNetConfig", "preset_config", "unet_param_shapes", "UNet3DConditionModel", "DDIMScheduler",
-           "ParallelDenoiser"]
+           "ParallelDenoiser", "CLIPVisionModelWithProjection"]
 
 
 def __getattr__(name):
@@ -19,4 +19,7 @@ def __getattr__(name):
     if name == "ParallelDenoiser":
         from .pipeline import ParallelDenoiser
         return ParallelDenoiser
+    if name == "CLIPVisionModelWithProjection":
+        from .clip_vision import CLIPVisionModelWithProjection
+        return CLIPVisionModelWithProjection
     raise AttributeError(name)

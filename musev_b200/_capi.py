@@ -180,7 +180,7 @@ def _declare(l: C.CDLL) -> None:
     # whole-model handles
     H, I, LL, P = C.c_void_p, C.c_int, C.c_longlong, C.POINTER
     for create in ("mvb_create", "mvb_create_controlnet", "mvb_create_referencenet", "mvb_create_vae_decoder",
-                   "mvb_create_vae_encoder", "mvb_create_pose_guider"):
+                   "mvb_create_vae_encoder", "mvb_create_pose_guider", "mvb_create_clip_vision"):
         fn(create, I, P(MvbConfig), I, P(C.c_void_p))
     fn("mvb_destroy", None, H)
     fn("mvb_load_weight", I, H, C.c_char_p, C.c_void_p, I, P(LL), I)
@@ -197,7 +197,8 @@ def _declare(l: C.CDLL) -> None:
                           ("mvb_referencenet_workspace_bytes", "mvb_referencenet_forward", MvbControlnetArgs),
                           ("mvb_vae_decode_workspace_bytes", "mvb_vae_decode", MvbVaeDecodeArgs),
                           ("mvb_vae_encode_workspace_bytes", "mvb_vae_encode", MvbVaeDecodeArgs),
-                          ("mvb_pose_guider_workspace_bytes", "mvb_pose_guider_forward", MvbVaeDecodeArgs)):
+                          ("mvb_pose_guider_workspace_bytes", "mvb_pose_guider_forward", MvbVaeDecodeArgs),
+                          ("mvb_clip_vision_workspace_bytes", "mvb_clip_vision_forward", MvbControlnetArgs)):
         fn(ws, LL, H, P(args))
         fn(run, I, H, P(args), C.c_void_p, LL, C.c_void_p)
 

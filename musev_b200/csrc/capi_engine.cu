@@ -59,6 +59,19 @@ static bool pose_guider_config_ok(const mvb_config* cfg) {
   return true;
 }
 
+// The CLIP vision tower (Engine::build_clip_vision): hidden size a multiple of 64 (conv_gemm K), head dim a multiple of 8 and
+// at most 192 (attention kernel), the MLP width a multiple of 64, the image a whole number of patches, act 2 / 3.
+static bool clip_vision_config_ok(const mvb_config* cfg) {
+  const int C = cfg->block_out_channels[0], I = cfg->block_out_channels[1], p = cfg->block_out_channels[2],
+            S = cfg->block_out_channels[3];
+  if (cfg->num_blocks != 4 || cfg->in_channels < 1 || cfg->in_channels > 4 || cfg->layers_per_block < 1) return false;
+  if (C < 64 || C > 2048 || C % 64 || cfg->heads < 1 || C % cfg->heads) return false;
+  const int d = C / cfg->heads;
+  if (d % 8 || d > 192 || I < 64 || I % 64 || p < 1 || S < p || S % p || (S / p) * (S / p) > 4096) return false;
+  if (cfg->out_channels < 8 || cfg->out_channels % 8 || !(cfg->norm_eps >= 0.f)) return false;
+  return cfg->norm_num_groups == 2 || cfg->norm_num_groups == 3;
+}
+
 // A handle of a validated configuration: MVB_ERR_STATE when out of host memory, MVB_ERR_CUDA when the device refused
 static int create(const mvb_config* cfg, int device, mvb::Kind kind, mvb_handle** out) {
   mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, kind);
@@ -154,6 +167,22 @@ int mvb_pose_guider_forward(mvb_handle* h, const mvb_vae_decode_args* args, void
                             void* stream) {
   if (!h || !args) return MVB_ERR_INVALID;
   return h->e->pose_guider_forward(*args, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mvb_create_clip_vision(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out || !clip_vision_config_ok(cfg)) return MVB_ERR_INVALID;
+  return create(cfg, device, mvb::Kind::ClipVision, out);
+}
+
+long long mvb_clip_vision_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args) {
+  if (!h || !args) return -1;
+  return h->e->clip_vision_workspace_bytes(*args);
+}
+
+int mvb_clip_vision_forward(mvb_handle* h, const mvb_controlnet_args* args, void* workspace, long long workspace_bytes,
+                            void* stream) {
+  if (!h || !args) return MVB_ERR_INVALID;
+  return h->e->clip_vision_forward(*args, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 void mvb_destroy(mvb_handle* h) {

@@ -33,7 +33,7 @@ extern "C" {
 
 const char* mvb_last_error(void) { return g_err; }
 
-int mvb_version(void) { return 2; }   // 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle
+int mvb_version(void) { return 3; }   // 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   if (!d || !d->a0 || !d->weight || !d->out) return fail("mvb_op_conv_gemm: null pointer", cudaSuccess);

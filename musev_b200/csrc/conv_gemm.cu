@@ -8,7 +8,7 @@
 //   warpgroups 1, 2     : MMA + epilogue -- warpgroup g owns accumulator rows [64 g, 64 g + 64) of the tile: 4 x
 //                         wgmma m64nBNk16 per K block, one K block kept in flight; then the accumulator goes through a
 //                         padded fp32 smem slice (128 columns at a time) so that each thread finishes whole 32-column
-//                         runs of one output row: bias / time-embedding / residual / GEGLU (four template variants) ->
+//                         runs of one output row: bias / time-embedding / residual / GEGLU / GELU (five template variants) ->
 //                         fp16 -> 16-byte global stores.
 // Pipeline: smem operand ring (full/empty mbarriers, 3..8 stages depending on BN).
 #include "conv_gemm.cuh"
@@ -89,8 +89,13 @@ enum : int {
   kEpiGeneric = 0,
   kEpiPlain = 1,      // fp16 out, bias / row-add optional, alpha == 1, no residual, no activation, N % 32 == 0
   kEpiResidual = 2,   // fp16 out, alpha * (acc + bias) + residual (beta == 1), N % 32 == 0
-  kEpiGeglu = 3       // fp16 out, value * gelu(gate) on the packed [16 value | 16 gate] column layout
+  kEpiGeglu = 3,      // fp16 out, value * gelu(gate) on the packed [16 value | 16 gate] column layout
+  kEpiAct = 4         // the generic epilogue followed by GELU (act 2) or quick-GELU (act 3): ViT MLPs (clip_vision.cu)
 };
+// act 2: exact-erf GELU (transformers ACT2FN["gelu"]); act 3: x * sigmoid(1.702 x) (ACT2FN["quick_gelu"], ViT-L CLIP)
+__device__ __forceinline__ float gelu_act(float x, int act) {
+  return act == 2 ? gelu_erf(x) : act == 3 ? __fdividef(x, 1.f + __expf(-1.702f * x)) : x;
+}
 
 struct AMaps {
   CUtensorMap m[4];   // activation views: [0] source 0, [1] skip-concat source / stride-2 phases 1..3
@@ -248,7 +253,7 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
       }
     };
     named_bar_sync(1 + wg, 128);                      // the previous tile's reads of the bias / accumulator slices are done
-    if constexpr (kEpi != kEpiGeneric) {
+    if constexpr (kEpi != kEpiGeneric && kEpi != kEpiAct) {
       for (int c = t; c < BN; c += 128) wbias[c] = (p.bias && ncol0 + c < p.N) ? __ldg(p.bias + ncol0 + c) : 0.f;
     }
 #pragma unroll
@@ -275,7 +280,7 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
           }
         };
         load_res(c0, rcur);
-        if constexpr (kEpi != kEpiGeneric) {
+        if constexpr (kEpi != kEpiGeneric && kEpi != kEpiAct) {
           const int nbase = ncol0 + c0;
           uint32_t v[32], vg[32];
           ld32(srow, v);
@@ -400,6 +405,10 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
                   o4.x = f[g * 4 + 0] * p.alpha; o4.y = f[g * 4 + 1] * p.alpha;
                   o4.z = f[g * 4 + 2] * p.alpha; o4.w = f[g * 4 + 3] * p.alpha;
                   if (p.act == 1) { o4.x = silu(o4.x); o4.y = silu(o4.y); o4.z = silu(o4.z); o4.w = silu(o4.w); }
+                  if constexpr (kEpi == kEpiAct) {
+                    o4.x = gelu_act(o4.x, p.act); o4.y = gelu_act(o4.y, p.act);
+                    o4.z = gelu_act(o4.z, p.act); o4.w = gelu_act(o4.w, p.act);
+                  }
                   *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + m * p.ldc + nn) = o4;
                 }
               }
@@ -419,6 +428,7 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
                     x *= p.alpha;
                     if (use_res) x = fmaf(p.beta, __half2float(rh8[j]), x);
                     if (p.act == 1) x = silu(x);
+                    if constexpr (kEpi == kEpiAct) x = gelu_act(x, p.act);
                   }
                   o[j] = __float2half_rn(x);
                 }
@@ -590,13 +600,15 @@ static void pick_box(int W, int H, int NF, int* bw, int* bh, int* bn) {
 // channels exactly; the GEGLU epilogue needs whole 64-column [value | gate] chunks.
 static const int kBlockNs[4] = {64, 128, 160, 256};
 
-static int pick_block_n(int N, int geglu, long long tiles_m, int num_sms) {
+// The GELU epilogue (kEpiAct) is not instantiated at 256 columns, where the generic epilogue it extends spills 8 bytes.
+static int pick_block_n(int N, int geglu, int gelu, long long tiles_m, int num_sms) {
   // prefer few padded columns, then fewer waves
   int best = 0;
   double best_cost = 1e30;
   for (int i = 3; i >= 0; --i) {
     const int bn = kBlockNs[i];
     if (geglu && (bn % 64)) continue;
+    if (gelu && bn == 256) continue;
     const int tn = ceil_div(N, bn);
     const long long tiles = tiles_m * tn;
     const long long waves = (tiles + num_sms - 1) / num_sms;
@@ -613,8 +625,10 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   typedef void (*KernelFn)(const AMaps, const CUtensorMap, const ConvGemmParams);
 #define MVB_GEMM_ROW(BN) \
   {conv_gemm_kernel<kEpiGeneric, BN>, conv_gemm_kernel<kEpiPlain, BN>, conv_gemm_kernel<kEpiResidual, BN>, \
-   conv_gemm_kernel<kEpiGeglu, BN>}
-  static const KernelFn kernels[4][4] = {MVB_GEMM_ROW(64), MVB_GEMM_ROW(128), MVB_GEMM_ROW(160), MVB_GEMM_ROW(256)};
+   conv_gemm_kernel<kEpiGeglu, BN>, conv_gemm_kernel<kEpiAct, BN>}
+  static const KernelFn kernels[4][5] = {MVB_GEMM_ROW(64), MVB_GEMM_ROW(128), MVB_GEMM_ROW(160),
+                                         {conv_gemm_kernel<kEpiGeneric, 256>, conv_gemm_kernel<kEpiPlain, 256>,
+                                          conv_gemm_kernel<kEpiResidual, 256>, conv_gemm_kernel<kEpiGeglu, 256>, nullptr}};
 #undef MVB_GEMM_ROW
   // the opt-in is per device: key the "already set" state by the current device ordinal
   static bool attr_set_dev[64] = {};
@@ -623,7 +637,8 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   bool& attr_set = attr_set_dev[cur_dev & 63];
   if (!attr_set) {
     for (int a = 0; a < 4; ++a)
-      for (int b = 0; b < 4; ++b) {
+      for (int b = 0; b < 5; ++b) {
+        if (!kernels[a][b]) continue;
         cudaError_t e = cudaFuncSetAttribute(reinterpret_cast<const void*>(kernels[a][b]),
                                              cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
         if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(conv_gemm_kernel)"; return e; }
@@ -631,7 +646,8 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
     attr_set = true;
   }
   const long long tiles_m = (long long)p.tiles_w * p.tiles_h * p.tiles_n;
-  p.block_n = pick_block_n(p.N, ep.geglu, tiles_m, num_sms);
+  const int gelu = ep.act == 2 || ep.act == 3;
+  p.block_n = pick_block_n(p.N, ep.geglu, gelu, tiles_m, num_sms);
   int bn_idx = 0;
   while (kBlockNs[bn_idx] != p.block_n) ++bn_idx;
   p.tiles_nn = ceil_div(p.N, p.block_n);
@@ -663,6 +679,7 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
       else if (!ep.res && ep.alpha == 1.f) epi = kEpiPlain;
     }
   }
+  if (gelu) epi = kEpiAct;
   static const bool trace = getenv("MVB_TRACE") != nullptr;
   if (trace)
     fprintf(stderr, "MVB_TRACE gemm M=%lld N=%d K=%lld taps=%d block_n=%d tiles=%lld geglu=%d res=%d f32=%d epi=%d\n",

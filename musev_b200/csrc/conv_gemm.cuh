@@ -39,7 +39,7 @@ struct ConvGemmParams {
   long long ld_res;
   float alpha, beta;
   int geglu;  // packed columns are [16 value | 16 gate] chunks: out = value * gelu_erf(gate)
-  int act;    // 0 none, 1 SiLU
+  int act;    // 0 none, 1 SiLU, 2 GELU (erf), 3 quick-GELU x sigmoid(1.702 x)
   int out_f32;  // store fp32 instead of fp16 (embedding tables)
 };
 

@@ -10,6 +10,7 @@
 #include <algorithm>
 
 #include "attention.cuh"
+#include "clip_vision.cuh"
 #include "cond_embed.cuh"
 #include "conv_gemm.cuh"
 #include "ops.cuh"
@@ -29,7 +30,7 @@ __global__ void set_ones_kernel(const OnesDesc* __restrict__ descs) {
 // Weight packing (mvb_load_weights): one launch packs a whole batch of tensors; blockIdx.y selects the tensor and the
 // blocks of a row grid-stride over its elements.
 struct PackDesc {
-  PackGeom g;          // matrix entry: the packed layout
+  PackGeom g;          // matrix entry: the packed layout; vector entry with vmode 1: p0 = d, p1 = dp
   const void* src;
   int is_f32;
   float* vdst;         // vector entry when non-null: vdst[0, vn) from src[0, vnsrc)
@@ -42,8 +43,10 @@ __global__ void pack_batch_kernel(const PackDesc* __restrict__ descs) {
   const PackDesc d = descs[blockIdx.y];
   if (d.vdst) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < d.vn; i += gridDim.x * blockDim.x) {
-      const int si = d.vmode == 2 ? geglu_src(i, d.vn) : i;
-      d.vdst[i] = (si < d.vnsrc) ? pack_src(d.src, si, d.is_f32) : 0.f;
+      int si = i;
+      if (d.vmode == 2) si = geglu_src(i, d.vn);
+      else if (d.vmode == 1) si = (i % d.g.p1) < d.g.p0 ? (i / d.g.p1) * d.g.p0 + i % d.g.p1 : -1;   // as src_row rowmode 1
+      d.vdst[i] = (si >= 0 && si < d.vnsrc) ? pack_src(d.src, si, d.is_f32) : 0.f;
     }
     return;
   }
@@ -156,9 +159,10 @@ void Engine::reg_mat(const std::string& name, Mat& m, int row0, int rows_dst, in
   g.colmode = colmode; g.cin = cin; g.taps = taps; g.nsrc = nsrc; g.ksrc = ksrc;
   loaders_[name] = l;
 }
-void Engine::reg_vec(const std::string& name, float* dst, int n, int nsrc, int vmode) {
+void Engine::reg_vec(const std::string& name, float* dst, int n, int nsrc, int vmode, int p0, int p1) {
   Loader l{};
   l.kind = LK_VEC; l.vdst = dst; l.vn = n; l.vnsrc = nsrc; l.vmode = vmode;
+  l.g.p0 = p0; l.g.p1 = p1;
   loaders_[name] = l;
 }
 void Engine::reg_linear(const std::string& p, Mat& m, int N, int K, bool bias) {
@@ -279,6 +283,7 @@ void Engine::build() {
     case Kind::VaeDecoder: build_vae(); break;
     case Kind::VaeEncoder: build_vae_encoder(); break;
     case Kind::PoseGuider: build_pose_guider(); break;
+    case Kind::ClipVision: build_clip_vision(); break;
   }
 }
 
@@ -359,6 +364,43 @@ void Engine::build_pose_guider() {
     add("blocks." + std::to_string(2 * i + 1), c.block_out_channels[i], c.block_out_channels[i + 1], 2, false, true);
   }
   add("conv_out", c.block_out_channels[nb - 1], c.out_channels, 1, false, false);
+}
+
+// CLIPVisionModelWithProjection.__init__ (transformers models/clip/modeling_clip.py: CLIPVisionEmbeddings :138-200,
+// CLIPEncoderLayer :354-386, CLIPVisionTransformer :647-697, visual_projection :1015-1030). mvb_config: in_channels =
+// image channels, out_channels = projection dim, block_out_channels = {hidden, intermediate, patch, image size},
+// layers_per_block = layers, heads, norm_eps, norm_num_groups = the MLP activation (conv_gemm act code 2 / 3).
+void Engine::build_clip_vision() {
+  const mvb_config& c = cfg_;
+  const int C = c.block_out_channels[0], I = c.block_out_channels[1], p = c.block_out_channels[2], S = c.block_out_channels[3];
+  const int P = (S / p) * (S / p), Kp = (c.in_channels * p * p + 63) / 64 * 64;
+  const int H = heads_, d = C / H, dp = pad16(d), hd = H * dp;
+  const std::string e = "vision_model.embeddings.", v = "vision_model.";
+  clip_patch_ = make_mat(C, Kp, false);
+  reg_mat(e + "patch_embedding.weight", clip_patch_, 0, C, 0, 0, 0, C, c.in_channels * p * p);   // columns (c, ky, kx)
+  clip_cls_ = slab<float>(C);
+  reg_vec(e + "class_embedding", clip_cls_, C, C);
+  clip_pos_ = slab<float>((size_t)(P + 1) * C);
+  reg_vec(e + "position_embedding.weight", clip_pos_, (P + 1) * C, (P + 1) * C);
+  clip_pre_ = make_norm(v + "pre_layrnorm", C);
+  clip_.assign(c.layers_per_block, ClipLayer{});
+  for (int i = 0; i < c.layers_per_block; ++i) {
+    ClipLayer& L = clip_[i];
+    const std::string q = v + "encoder.layers." + std::to_string(i) + ".";
+    L.ln1 = make_norm(q + "layer_norm1", C);
+    L.qkv = make_mat(3 * hd, C, true);
+    const char* proj[3] = {"q_proj", "k_proj", "v_proj"};
+    for (int j = 0; j < 3; ++j) {
+      reg_mat(q + "self_attn." + proj[j] + ".weight", L.qkv, j * hd, hd, 1, d, dp, C, C);
+      reg_vec(q + "self_attn." + proj[j] + ".bias", L.qkv.bias ? L.qkv.bias + j * hd : nullptr, hd, C, 1, d, dp);
+    }
+    reg_linear(q + "self_attn.out_proj", L.out, C, C, true);
+    L.ln2 = make_norm(q + "layer_norm2", C);
+    reg_linear(q + "mlp.fc1", L.fc1, I, C, true);
+    reg_linear(q + "mlp.fc2", L.fc2, C, I, true);
+  }
+  clip_post_ = make_norm(v + "post_layernorm", C);
+  reg_linear("visual_projection", clip_proj_, c.out_channels, C, false);
 }
 
 // AutoencoderKL decoder half: post_quant_conv + Decoder.__init__ (diffusers models/autoencoder_kl.py:102-104, vae.py:201-263):
@@ -587,6 +629,7 @@ int Engine::load_weights(const mvb_named_tensor* ts, int n) {
     if (l.kind == LK_VEC) {
       if (numel != l.vnsrc) { err_ = std::string("bad shape for ") + t.name; return MVB_ERR_INVALID; }
       d.vdst = l.vdst; d.vn = l.vn; d.vnsrc = l.vnsrc; d.vmode = l.vmode;
+      d.g.p0 = l.g.p0; d.g.p1 = l.g.p1;
     } else {
       if (numel != (long long)l.g.nsrc * l.g.ksrc) { err_ = std::string("bad shape for ") + t.name; return MVB_ERR_INVALID; }
       d.g = l.g;
@@ -1532,6 +1575,94 @@ bool Engine::run_pose_guider(const mvb_vae_decode_args& a, Arena& ar, cudaStream
   return true;
 }
 
+static const char* clip_vision_shape_error(const mvb_controlnet_args& a, const mvb_config& c) {
+  if (a.NF < 1 || a.NF > 1024) return "clip vision: NF (images per call) must be in 1..1024";
+  if (a.H != c.block_out_channels[3] || a.W != c.block_out_channels[3])
+    return "clip vision: pixel_values must be image_size x image_size (no position-embedding interpolation)";
+  if (a.n_out != 2) return "clip vision: n_out must be 2 (outs[0] = image_embeds, outs[1] = last_hidden_state)";
+  if (!a.outs[0] && !a.outs[1]) return "clip vision: no output requested (outs[0] and outs[1] are both NULL)";
+  return nullptr;
+}
+
+// CLIPVisionModelWithProjection.forward (transformers models/clip/modeling_clip.py:1036-1075 -> CLIPVisionTransformer.forward
+// :667-690): a.sample = pixel_values [NF, in_channels, S, S]. The residual stream is fp16 [NF (P + 1), C] channels-last;
+// every linear layer is a conv_gemm with its bias / residual / activation in the epilogue.
+bool Engine::run_clip_vision(const mvb_controlnet_args& a, Arena& ar, cudaStream_t s) {
+  const mvb_config& c = cfg_;
+  if (const char* bad = clip_vision_shape_error(a, c)) { err_ = bad; return false; }
+  const int C = c.block_out_channels[0], I = c.block_out_channels[1], p = c.block_out_channels[2], S = c.block_out_channels[3];
+  const int P = (S / p) * (S / p), T = P + 1, Kp = clip_patch_.K, NF = a.NF;
+  const int Hh = heads_, d = C / Hh, dp = pad16(d), hd = Hh * dp;
+  const float eps = c.norm_eps;
+  const long long M = (long long)NF * T;
+  mvb_unet_args ua{};
+  ua.B = NF; ua.T = 1; ua.H = 1; ua.W = 1;
+  Fwd f(this, ar, s, ua, true);
+  // ---- embeddings (:202-218) + pre_layrnorm (:677): patch unfold, the patch conv as one GEMM into fp32, then one kernel
+  __half* x = f.alloc_h(M, C);
+  {
+    const size_t mk = f.mark();
+    __half* A = f.alloc_h((long long)NF * P, Kp);
+    float* pe = f.alloc_f((long long)NF * P * C);
+    if (!ar.dry && f.ok) {
+      cudaError_t e = clip_patchify(s, a.sample, a.sample_is_f32, NF, c.in_channels, S, p, Kp, A);
+      if (e != cudaSuccess) f.fail("clip_patchify", e);
+    }
+    Epilogue ep; ep.out = (__half*)pe; ep.ldc = C; ep.out_f32 = 1;
+    f.gemm(A, (long long)NF * P, Kp, clip_patch_, ep, false);
+    if (!ar.dry && f.ok) {
+      cudaError_t e = clip_embed_layernorm(s, pe, clip_cls_, clip_pos_, NF, P, C, eps, clip_pre_.g, clip_pre_.b, x);
+      if (e != cudaSuccess) f.fail("clip_embed_layernorm", e);
+    }
+    f.release(mk);
+  }
+  f.tap("embeddings", x, M, C);
+  // ---- encoder layers (CLIPEncoderLayer.forward :363-386)
+  for (size_t i = 0; i < clip_.size(); ++i) {
+    const ClipLayer& L = clip_[i];
+    const size_t mk = f.mark();
+    __half* nbuf = f.alloc_h(M, C);
+    f.ln(x, M, C, eps, L.ln1, nbuf);
+    __half* qkv = f.alloc_h(M, 3 * hd);
+    { Epilogue ep; ep.out = qkv; ep.ldc = 3 * hd; f.gemm(nbuf, M, C, L.qkv, ep); }
+    __half* ao = f.alloc_h(M, C);
+    AttnArgs aa{};   // eager_attention_forward (:261-280): softmax(q k^T d^-0.5) v per head over the T tokens of one image
+    aa.q = qkv; aa.ldq = 3 * hd; aa.NF = NF; aa.Nq = T; aa.heads = Hh; aa.d = d; aa.dp = dp;
+    aa.scale = 1.f / sqrtf((float)d);
+    aa.nseg = 1;
+    aa.seg[0] = AttnSegment{qkv + hd, qkv + 2 * hd, 3 * hd, M, T, 1, T, 0};
+    aa.out = ao; aa.ldo = C; aa.out_scale = 1.f;
+    f.attn(aa);
+    { Epilogue ep; ep.out = x; ep.ldc = C; ep.res = x; ep.ld_res = C; f.gemm(ao, M, C, L.out, ep); }
+    f.ln(x, M, C, eps, L.ln2, nbuf);
+    __half* h = f.alloc_h(M, I);
+    { Epilogue ep; ep.out = h; ep.ldc = I; ep.act = c.norm_num_groups; f.gemm(nbuf, M, C, L.fc1, ep); }   // CLIPMLP :347-351
+    { Epilogue ep; ep.out = x; ep.ldc = C; ep.res = x; ep.ld_res = C; f.gemm(h, M, I, L.fc2, ep); }
+    f.release(mk);
+    f.tap("encoder.layers." + std::to_string(i), x, M, C);
+  }
+  // ---- outputs: last_hidden_state is the encoder output (not post-normalised, :684); image_embeds = visual_projection(
+  // post_layernorm(last_hidden_state[:, 0])) (:685-686, :1068-1069)
+  if (a.outs[1] && !ar.dry && f.ok) {
+    cudaError_t e = a.out_is_f32 ? half_to_float(s, x, M * C, (float*)a.outs[1])
+                                 : cudaMemcpyAsync(a.outs[1], x, (size_t)M * C * sizeof(__half), cudaMemcpyDeviceToDevice, s);
+    if (e != cudaSuccess) f.fail("clip vision last_hidden_state", e);
+  }
+  if (a.outs[0]) {
+    __half* pooled = f.alloc_h(NF, C);
+    __half* pn = f.alloc_h(NF, C);
+    if (!ar.dry && f.ok) {
+      cudaError_t e = cudaMemcpy2DAsync(pooled, (size_t)C * sizeof(__half), x, (size_t)T * C * sizeof(__half),
+                                        (size_t)C * sizeof(__half), NF, cudaMemcpyDeviceToDevice, s);
+      if (e != cudaSuccess) f.fail("clip vision pooled rows", e);
+    }
+    f.ln(pooled, NF, C, eps, clip_post_, pn);
+    Epilogue ep; ep.out = (__half*)a.outs[0]; ep.ldc = c.out_channels; ep.out_f32 = a.out_is_f32 ? 1 : 0;
+    f.gemm(pn, NF, C, clip_proj_, ep, false);
+  }
+  return f.ok;
+}
+
 // ---------------------------------------------------------------------------------------------- entry points
 template <typename Args>
 long long Engine::dry_run(RunFn<Args> run, std::initializer_list<Kind> kinds, const char* wrong_kind, const Args& a) {
@@ -1599,6 +1730,15 @@ long long Engine::pose_guider_workspace_bytes(const mvb_vae_decode_args& a) {
 int Engine::pose_guider_forward(const mvb_vae_decode_args& a, void* ws, long long wbytes, cudaStream_t stream) {
   const char* bad = (!a.latents || !a.out || !ws) ? kNullArg : pose_guider_shape_error(a, cfg_.num_blocks);
   return launch(&Engine::run_pose_guider, {Kind::PoseGuider}, "not a PoseGuider handle", bad, a, ws, wbytes, stream);
+}
+
+
+long long Engine::clip_vision_workspace_bytes(const mvb_controlnet_args& a) {
+  return dry_run(&Engine::run_clip_vision, {Kind::ClipVision}, "not a CLIP vision handle", a);
+}
+int Engine::clip_vision_forward(const mvb_controlnet_args& a, void* ws, long long wbytes, cudaStream_t stream) {
+  const char* bad = (!a.sample || !ws) ? kNullArg : clip_vision_shape_error(a, cfg_);
+  return launch(&Engine::run_clip_vision, {Kind::ClipVision}, "not a CLIP vision handle", bad, a, ws, wbytes, stream);
 }
 
 }  // namespace mvb

@@ -128,7 +128,7 @@ struct Loader {
   // LK_VEC: vdst[0, vn) from a source of vnsrc elements
   float* vdst = nullptr;
   int vn = 0, vnsrc = 0;
-  int vmode = 0;    // 0 copy (zero fill beyond source), 2 geglu interleave
+  int vmode = 0;    // 0 copy (zero fill beyond source), 1 pad heads (g.p0 = d, g.p1 = dp), 2 geglu interleave
   // LK_ABS_SCALAR
   float* host_scalar = nullptr;
   bool loaded = false;
@@ -141,6 +141,13 @@ struct CondConv {
   int cin = 0, cin_p = 0, cout = 0, cout_p = 0, stride = 1;
   bool small = false;    // cond_embed.cu small-channel kernel (cin 16 / 32 or the image conv_in); else conv_gemm / conv_s2
   bool act = true;       // SiLU after every conv except conv_out
+};
+
+// One pre-norm ViT encoder layer (transformers CLIPEncoderLayer, models/clip/modeling_clip.py:354-386)
+struct ClipLayer {
+  Norm ln1, ln2;
+  Mat qkv;            // q | k | v projections, heads padded to dp columns (rowmode 1), biases padded alike
+  Mat out, fc1, fc2;
 };
 
 struct Arena {
@@ -159,8 +166,9 @@ struct Arena {
 // UNet: UNet3DConditionModel; ControlNet: ControlNet encoder (diffusers models/controlnet.py);
 // ReferenceNet: ReferenceNet2D encoder + mid block (musev/models/referencenet.py);
 // VaeDecoder / VaeEncoder: the AutoencoderKL halves (diffusers models/autoencoder_kl.py, vae.py);
-// PoseGuider: musev/models/controlnet.py:326-371
-enum class Kind { UNet, ControlNet, ReferenceNet, VaeDecoder, VaeEncoder, PoseGuider };
+// PoseGuider: musev/models/controlnet.py:326-371;
+// ClipVision: transformers CLIPVisionModelWithProjection (models/clip/modeling_clip.py), the IP-Adapter image encoder
+enum class Kind { UNet, ControlNet, ReferenceNet, VaeDecoder, VaeEncoder, PoseGuider, ClipVision };
 
 class Engine {
  public:
@@ -182,6 +190,8 @@ class Engine {
   int vae_encode(const mvb_vae_decode_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long pose_guider_workspace_bytes(const mvb_vae_decode_args& a);
   int pose_guider_forward(const mvb_vae_decode_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
+  long long clip_vision_workspace_bytes(const mvb_controlnet_args& a);
+  int clip_vision_forward(const mvb_controlnet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long controlnet_workspace_bytes(const mvb_controlnet_args& a);
   int controlnet_forward(const mvb_controlnet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   Kind kind() const { return kind_; }
@@ -199,12 +209,13 @@ class Engine {
   void build_vae_encoder();
   void build_vae_mid(const std::string& p, int C);
   void build_pose_guider();
+  void build_clip_vision();
   template <typename T> T* slab(size_t n);
   Mat make_mat(int N, int K, bool bias);
   Norm make_norm(const std::string& p, int C);
   void reg_mat(const std::string& name, Mat& m, int row0, int rows_dst, int rowmode, int p0, int p1, int nsrc, int ksrc,
                int colmode = 0, int cin = 0, int taps = 1);
-  void reg_vec(const std::string& name, float* dst, int n, int nsrc_expected, int vmode = 0);
+  void reg_vec(const std::string& name, float* dst, int n, int nsrc_expected, int vmode = 0, int p0 = 0, int p1 = 0);
   void reg_linear(const std::string& p, Mat& m, int N, int K, bool bias);
   void reg_conv(const std::string& p, Mat& m, int N, int Cin, int taps);
   void build_tblock(const std::string& p, TBlock& b, int C, bool cross);
@@ -229,6 +240,7 @@ class Engine {
   bool run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
   bool run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
   bool run_pose_guider(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
+  bool run_clip_vision(const mvb_controlnet_args& a, Arena& ar, cudaStream_t s);
 
   mvb_config cfg_;
   int device_ = 0, num_sms_ = 132;
@@ -274,6 +286,13 @@ class Engine {
   Norm vae_attn_norm_;
   Mat vae_q_, vae_k_, vae_v_, vae_o_;
   std::vector<CondConv> pg_;   // PoseGuider: conv_in, blocks.0 .. blocks.{2 (num_blocks - 1) - 1}, conv_out
+  // ClipVision (mvb_create_clip_vision): patch embedding [C, Kp] (no bias), class / position embeddings (fp32), the layers,
+  // pre_layrnorm / post_layernorm and visual_projection [proj, C] (no bias)
+  Mat clip_patch_, clip_proj_;
+  float* clip_cls_ = nullptr;
+  float* clip_pos_ = nullptr;
+  Norm clip_pre_, clip_post_;
+  std::vector<ClipLayer> clip_;
 };
 
 // Channel count a PoseGuider activation is stored with: 16 / 32 as is (small-channel kernel), others padded to 64k.

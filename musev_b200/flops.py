@@ -233,3 +233,20 @@ def pose_guider_flops(cfg, N: int, H: int, W: int) -> Dict[str, float]:
         H, W = (H - 1) // stride + 1, (W - 1) // stride + 1
         conv(N * H * W, cin, cout, 9)
     return _vae_total(f)
+
+
+def clip_vision_flops(cfg, N: int) -> Dict[str, float]:
+    """`CLIPVisionModelWithProjection.forward` on N images (ClipVisionConfig `cfg`; transformers models/clip/modeling_clip.py),
+    2 M N K per matrix product: the patch conv, q / k / v / out_proj / fc1 / fc2 per layer, q k^T and P v per head, and
+    visual_projection on the class token. ViT-H/14 at 224 x 224: 0.3346 TFLOP per image."""
+    f, conv, lin, attn = _vae_counters()
+    C, I, T = cfg.hidden_size, cfg.intermediate_size, cfg.num_patches + 1
+    conv(N * cfg.num_patches, cfg.num_channels, C, cfg.patch_size ** 2)
+    for _ in range(cfg.num_hidden_layers):
+        for _ in range(4):                      # q, k, v, out_proj
+            lin(N * T, C, C)
+        attn(N * cfg.num_attention_heads, T, T, C // cfg.num_attention_heads)
+        lin(N * T, C, I)
+        lin(N * T, I, C)
+    lin(N, C, cfg.projection_dim)
+    return _vae_total(f)

@@ -8,7 +8,7 @@ reference's own `state_dict()` key by key.
 from __future__ import annotations
 
 from collections import OrderedDict
-from dataclasses import asdict, dataclass, field
+from dataclasses import asdict, dataclass, field, fields
 from typing import Dict, Tuple
 
 
@@ -469,4 +469,79 @@ def pose_guider_param_shapes(cfg: PoseGuiderConfig) -> "OrderedDict[str, Tuple[i
     for name, cin, cout, _ in pose_guider_layers(cfg):
         out[f"{name}.weight"] = (cout, cin, 3, 3)
         out[f"{name}.bias"] = (cout,)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ CLIP vision tower
+CLIP_ACT_CODES = {"gelu": 2, "quick_gelu": 3}   # transformers ACT2FN name -> conv_gemm epilogue act code
+
+
+@dataclass
+class ClipVisionConfig:
+    """The `transformers.CLIPVisionConfig` fields `CLIPVisionModelWithProjection` computes with. The defaults are the
+    IP-Adapter SD-1.5 image encoder (OpenCLIP ViT-H/14): 632 M parameters, 257 tokens per 224 x 224 image."""
+    hidden_size: int = 1280
+    intermediate_size: int = 5120
+    num_hidden_layers: int = 32
+    num_attention_heads: int = 16
+    num_channels: int = 3
+    image_size: int = 224
+    patch_size: int = 14
+    projection_dim: int = 1024
+    hidden_act: str = "gelu"
+    layer_norm_eps: float = 1e-5
+
+    @property
+    def num_patches(self) -> int:
+        return (self.image_size // self.patch_size) ** 2
+
+
+def clip_vision_config(config) -> ClipVisionConfig:
+    """A `ClipVisionConfig` from a `ClipVisionConfig`, a `transformers.CLIPVisionConfig` or a dict (other keys are ignored).
+    Raises ValueError for an activation other than gelu / quick_gelu and for geometry the engine's kernels do not take."""
+    if isinstance(config, ClipVisionConfig):
+        cfg = ClipVisionConfig(**asdict(config))
+    else:
+        get = config.get if isinstance(config, dict) else (lambda k, d=None: getattr(config, k, d))
+        cfg = ClipVisionConfig(**{f.name: get(f.name, f.default) for f in fields(ClipVisionConfig)})
+    if cfg.hidden_act not in CLIP_ACT_CODES:
+        raise ValueError(f"hidden_act {cfg.hidden_act!r} is not supported (the engine has {sorted(CLIP_ACT_CODES)})")
+    C, H = cfg.hidden_size, cfg.num_attention_heads
+    if C % 64 or not 64 <= C <= 2048 or H < 1 or C % H or (C // H) % 8 or C // H > 192:
+        raise ValueError(f"hidden_size {C} / {H} heads: the hidden size must be a multiple of 64 (at most 2048) and the "
+                         "head dim a multiple of 8, at most 192")
+    if cfg.intermediate_size % 64 or cfg.projection_dim % 8 or cfg.image_size % cfg.patch_size or cfg.num_hidden_layers < 1:
+        raise ValueError("intermediate_size must be a multiple of 64, projection_dim of 8, image_size of patch_size")
+    if not 1 <= cfg.num_channels <= 4:
+        raise ValueError(f"num_channels must be 1..4, got {cfg.num_channels}")
+    return cfg
+
+
+def clip_vision_param_shapes(cfg: ClipVisionConfig) -> "OrderedDict[str, Tuple[int, ...]]":
+    """name -> shape of `transformers.CLIPVisionModelWithProjection.state_dict()` (models/clip/modeling_clip.py; the
+    non-persistent `position_ids` buffer is not part of it)."""
+    out: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    C, I, p = cfg.hidden_size, cfg.intermediate_size, cfg.patch_size
+    e = "vision_model.embeddings."
+    out[e + "class_embedding"] = (C,)
+    out[e + "patch_embedding.weight"] = (C, cfg.num_channels, p, p)
+    out[e + "position_embedding.weight"] = (cfg.num_patches + 1, C)
+    out["vision_model.pre_layrnorm.weight"] = (C,)
+    out["vision_model.pre_layrnorm.bias"] = (C,)
+    for i in range(cfg.num_hidden_layers):
+        q = f"vision_model.encoder.layers.{i}."
+        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
+            out[f"{q}self_attn.{n}.weight"] = (C, C)
+            out[f"{q}self_attn.{n}.bias"] = (C,)
+        out[q + "layer_norm1.weight"] = (C,)
+        out[q + "layer_norm1.bias"] = (C,)
+        out[q + "mlp.fc1.weight"] = (I, C)
+        out[q + "mlp.fc1.bias"] = (I,)
+        out[q + "mlp.fc2.weight"] = (C, I)
+        out[q + "mlp.fc2.bias"] = (C,)
+        out[q + "layer_norm2.weight"] = (C,)
+        out[q + "layer_norm2.bias"] = (C,)
+    out["vision_model.post_layernorm.weight"] = (C,)
+    out["vision_model.post_layernorm.bias"] = (C,)
+    out["visual_projection.weight"] = (cfg.projection_dim, C)
     return out

@@ -14,8 +14,8 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from .schema import (ControlNetConfig, ImageProjConfig, PoseGuiderConfig, ReferenceNetConfig, UNetConfig, VAEConfig,
-                     controlnet_param_shapes, image_proj_param_shapes, pose_guider_param_shapes, refer_emb_shapes,
+from .schema import (ClipVisionConfig, ControlNetConfig, ImageProjConfig, PoseGuiderConfig, ReferenceNetConfig, UNetConfig,
+                     VAEConfig, clip_vision_param_shapes, controlnet_param_shapes, image_proj_param_shapes, pose_guider_param_shapes, refer_emb_shapes,
                      referencenet_param_shapes, unet_param_shapes, vae_decoder_param_shapes, vae_encoder_param_shapes)
 
 _BRANCH_OUT = ("conv2.weight", "proj_out.weight", "to_out.0.weight", "ff.net.2.weight", "conv4.3.weight")
@@ -214,3 +214,56 @@ def make_pose_images(frames: int, H: int, W: int, seed: int = 1717, channels: in
 def make_pose_guider_emb(frames: int, channels: int, h: int, w: int, seed: int = 5151, scale: float = 0.5) -> torch.Tensor:
     """A seeded stand-in for the UNet's `pose_guider_emb`: [(b t), channels, h, w] fp32."""
     return torch.randn(frames, channels, h, w, generator=torch.Generator().manual_seed(seed)) * scale
+
+
+def make_clip_vision_state_dict(cfg: ClipVisionConfig, seed: int = 0, dtype: torch.dtype = torch.float32,
+                                outlier_channels: int = 0, outlier_offset: float = 40.0) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded weights for `CLIPVisionModelWithProjection` (`clip_vision_param_shapes`), one generator per name as in
+    `make_state_dict`. Matrices have std 1 / sqrt(fan_in); the two residual-branch outputs (`out_proj`, `fc2`) are scaled by
+    1 / sqrt(2 num_hidden_layers), so a 32-layer residual stream stays O(1) and fits fp16 with room to spare. LayerNorm
+    weights are 1 + 0.1 N(0, 1), biases 0.02 N(0, 1), the class embedding N(0, 1) and the position embedding 0.5 N(0, 1).
+
+    `outlier_channels` > 0 picks that many channels (seeded) and adds `outlier_offset` to them in the position embedding
+    (the input of pre_layrnorm) and in layer 0's fc2 bias, so every later LayerNorm sees a few residual channels with a large
+    constant offset, as trained ViTs carry."""
+    sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+    branch_gain = (2.0 * cfg.num_hidden_layers) ** -0.5
+    for name, shape in clip_vision_param_shapes(cfg).items():
+        g = _gen(seed, "clip_vision." + name)
+        if name.endswith("class_embedding"):
+            t = torch.randn(shape, generator=g)
+        elif name.endswith("position_embedding.weight"):
+            t = torch.randn(shape, generator=g) * 0.5
+        elif len(shape) == 1:
+            t = torch.randn(shape, generator=g) * (0.1 if name.endswith(".weight") else 0.02)
+            if name.endswith(".weight"):
+                t = t + 1.0
+        else:
+            fan_in = 1
+            for d in shape[1:]:
+                fan_in *= d
+            gain = branch_gain if name.endswith(("out_proj.weight", "fc2.weight")) else 1.0
+            t = torch.randn(shape, generator=g) * (gain / fan_in ** 0.5)
+        sd[name] = t
+    if outlier_channels > 0:
+        ch = torch.randperm(cfg.hidden_size, generator=_gen(seed, "clip_vision.outliers"))[:outlier_channels]
+        sd["vision_model.embeddings.position_embedding.weight"][:, ch] += outlier_offset
+        sd["vision_model.encoder.layers.0.mlp.fc2.bias"][ch] += outlier_offset
+    return OrderedDict((k, v.to(dtype)) for k, v in sd.items())
+
+
+OPENAI_CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)   # CLIPImageProcessor image_mean / image_std
+OPENAI_CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
+
+
+def make_clip_pixel_values(n: int, image_size: int = 224, seed: int = 3131, channels: int = 3) -> torch.Tensor:
+    """Seeded `pixel_values` as `CLIPImageProcessor` returns them: smooth images in [0, 1] normalised with the OpenAI CLIP
+    mean / std, [n, channels, image_size, image_size] fp32."""
+    g = torch.Generator().manual_seed(seed)
+    lo = torch.rand(n, channels, max(1, image_size // 16), max(1, image_size // 16), generator=g)
+    hi = torch.rand(n, channels, image_size, image_size, generator=g)
+    img = (0.8 * torch.nn.functional.interpolate(lo, size=(image_size, image_size), mode="bilinear", align_corners=False)
+           + 0.2 * hi).clamp(0, 1)
+    mean = torch.tensor((OPENAI_CLIP_MEAN * 2)[:channels]).view(1, -1, 1, 1)
+    std = torch.tensor((OPENAI_CLIP_STD * 2)[:channels]).view(1, -1, 1, 1)
+    return (img - mean) / std

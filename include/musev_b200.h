@@ -96,6 +96,11 @@ typedef struct mvb_attention_desc {
 } mvb_attention_desc;
 
 int mvb_op_attention(const mvb_attention_desc* desc, void* stream);
+/* The same attention with a causal mask (since mvb_version 4): key k of a sequence is visible to query q only if k <= q,
+ * positions local to the sequence -- the self attention of transformers' CLIPTextTransformer (models/clip/modeling_clip.py,
+ * `_create_4d_causal_attention_mask`). Self attention only: nseg = 1, nk[0] = Nq, fdiv[0] = 1, fmul[0] = Nq, fadd[0] = 0;
+ * any other layout is rejected before a launch (MVB_ERR_CUDA with "causal" in mvb_last_error()). */
+int mvb_op_attention_causal(const mvb_attention_desc* desc, void* stream);
 /* Measurement aid (no reference equivalent): while `device_buffer` (>= 9*32*8 int64 on the device) is set, CTA (0,0,0) of every
  * ping-pong attention launch (head dim <= 64) writes the SM clock at each phase of its first 32 key/value tiles:
  * [role][tile][slot], role 4t+q = softmax warp of query tile t, lane quarter q (slots: 0 wait S, 1 S ready, 2 scores in registers, 3 row max,
@@ -242,7 +247,8 @@ const char* mvb_handle_error(mvb_handle* h);
 /* Debug aid for bisecting parity: layer outputs of the last forward, fp16 [rows, C] inside the caller's workspace. */
 int mvb_debug_num_taps(mvb_handle* h);
 int mvb_debug_tap(mvb_handle* h, int i, char* name, int name_cap, const void** ptr, long long* rows, int* C);
-/* LoRA merge into the packed weights of a UNet handle, after mvb_finalize. Replaces the in-place
+/* LoRA merge into the packed weights of a UNet handle or a CLIP text encoder handle (mvb_create_clip_text, since
+ * mvb_version 4; targets by the `CLIPTextModel.state_dict()` names), after mvb_finalize; other handles return MVB_ERR_STATE. Replaces the in-place
  * `curr_layer.weight.data += adding_weight` of musev/utils/model_util.py:update_pipeline_lora_model (:153-262) and, with
  * subtract = 1, the `layer.weight.data -= added_weight` of unload_lora (:468-475). For each i:
  *   up[i].name            the target, a reference weight name (`down_blocks.0.attentions.0.proj_in.weight`); a target may
@@ -408,6 +414,42 @@ int mvb_create_clip_vision(const mvb_config* cfg, int device, mvb_handle** out);
 long long mvb_clip_vision_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args);
 int mvb_clip_vision_forward(mvb_handle* h, const mvb_controlnet_args* args, void* workspace, long long workspace_bytes,
                             void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * CLIP text encoder, the prompt encoder, once per pipeline call before the denoise loop (since mvb_version 4).
+ * Reference: transformers `CLIPTextModel.forward(input_ids)` (models/clip/modeling_clip.py: CLIPTextEmbeddings,
+ * CLIPEncoderLayer, CLIPTextTransformer.forward) as `encode_weighted_prompt` runs it once per 77-token chunk
+ * (musev/utils/text_emb_util.py:178-215,352-420): token + position embeddings, pre-norm encoder layers with CAUSAL self
+ * attention (LayerNorm, q/k/v with bias, softmax(q k^T d^-0.5 + causal mask) v, out_proj + residual; LayerNorm, fc1,
+ * activation, fc2 + residual), final_layer_norm, and the pooled row. Tokenization stays with the caller; there is no padding
+ * mask. The handle is created from an `mvb_config` whose fields mean, for the CLIP text encoder:
+ *   block_out_channels    {hidden_size (multiple of 64, <= 2048), intermediate_size (multiple of 64),
+ *                          max_position_embeddings (<= 4096), vocab_size};
+ *   num_blocks            must be 4 (the four entries above);
+ *   layers_per_block      `num_hidden_layers`;
+ *   heads                 `num_attention_heads`; hidden_size / heads a multiple of 8 and at most 192;
+ *   norm_eps              `layer_norm_eps` of every LayerNorm;
+ *   norm_num_groups       the MLP activation `hidden_act`: 2 gelu (erf), 3 quick_gelu;
+ *   out_channels          `eos_token_id` (>= 0): 2 selects the legacy pooling rule i_n = argmax(input_ids[n]) (first
+ *                         occurrence), any other value the first position where input_ids[n] == eos_token_id (0 if none);
+ *   in_channels and the other fields are ignored.
+ * Weights by the `CLIPTextModel.state_dict()` names (`text_model.*`; `text_model.embeddings.position_ids` is not a weight).
+ * It takes `mvb_controlnet_args`, whose fields mean, for the CLIP text encoder:
+ *   sample                   input_ids [NF, L], int64 on the device; an id outside [0, vocab_size) is never read and embeds
+ *                            as a zero token row (callers should reject it first, as nn.Embedding does);
+ *   sample_is_f32            must be 0;
+ *   NF                       sequences, 1..1024;
+ *   H                        L, 1..max_position_embeddings;  W  must be 1;
+ *   n_out                    must be 2;
+ *   outs[0]                  last_hidden_state [NF, L, hidden_size] (after final_layer_norm), or NULL;
+ *   outs[1]                  pooler_output [NF, hidden_size], or NULL; at least one of the two must be given;
+ *   out_is_f32               both outputs fp32 (1) or fp16 (0);
+ *   other fields are ignored.
+ * Bad arguments are rejected before any launch (negative return, mvb_handle_error). LoRA: mvb_unet_merge_lora. */
+int mvb_create_clip_text(const mvb_config* cfg, int device, mvb_handle** out);
+long long mvb_clip_text_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args);
+int mvb_clip_text_forward(mvb_handle* h, const mvb_controlnet_args* args, void* workspace, long long workspace_bytes,
+                          void* stream);
 
 #ifdef __cplusplus
 }

@@ -6,7 +6,7 @@ importing this package does not load it, using any op does -- and fails loudly i
 from .schema import UNetConfig, preset_config, unet_param_shapes  # noqa: F401
 
 __all__ = ["UNetConfig", "preset_config", "unet_param_shapes", "UNet3DConditionModel", "DDIMScheduler",
-           "ParallelDenoiser", "CLIPVisionModelWithProjection"]
+           "ParallelDenoiser", "CLIPVisionModelWithProjection", "CLIPTextModel"]
 
 
 def __getattr__(name):
@@ -22,4 +22,7 @@ def __getattr__(name):
     if name == "CLIPVisionModelWithProjection":
         from .clip_vision import CLIPVisionModelWithProjection
         return CLIPVisionModelWithProjection
+    if name == "CLIPTextModel":
+        from .clip_text import CLIPTextModel
+        return CLIPTextModel
     raise AttributeError(name)

@@ -141,8 +141,8 @@ def _declare(l: C.CDLL) -> None:
     l.mvb_op_small_conv.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                     C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     l.mvb_op_small_conv.restype = C.c_int
-    l.mvb_op_attention.argtypes = [C.POINTER(AttentionDesc), C.c_void_p]
-    l.mvb_op_attention.restype = C.c_int
+    for att in ("mvb_op_attention", "mvb_op_attention_causal"):
+        fn(att, C.c_int, C.POINTER(AttentionDesc), C.c_void_p)
     l.mvb_debug_attention_trace.argtypes = [C.c_void_p]
     l.mvb_debug_attention_trace.restype = C.c_int
     l.mvb_tensor_map_cache_stats.argtypes = [C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]
@@ -180,7 +180,8 @@ def _declare(l: C.CDLL) -> None:
     # whole-model handles
     H, I, LL, P = C.c_void_p, C.c_int, C.c_longlong, C.POINTER
     for create in ("mvb_create", "mvb_create_controlnet", "mvb_create_referencenet", "mvb_create_vae_decoder",
-                   "mvb_create_vae_encoder", "mvb_create_pose_guider", "mvb_create_clip_vision"):
+                   "mvb_create_vae_encoder", "mvb_create_pose_guider", "mvb_create_clip_vision",
+                   "mvb_create_clip_text"):
         fn(create, I, P(MvbConfig), I, P(C.c_void_p))
     fn("mvb_destroy", None, H)
     fn("mvb_load_weight", I, H, C.c_char_p, C.c_void_p, I, P(LL), I)
@@ -198,7 +199,8 @@ def _declare(l: C.CDLL) -> None:
                           ("mvb_vae_decode_workspace_bytes", "mvb_vae_decode", MvbVaeDecodeArgs),
                           ("mvb_vae_encode_workspace_bytes", "mvb_vae_encode", MvbVaeDecodeArgs),
                           ("mvb_pose_guider_workspace_bytes", "mvb_pose_guider_forward", MvbVaeDecodeArgs),
-                          ("mvb_clip_vision_workspace_bytes", "mvb_clip_vision_forward", MvbControlnetArgs)):
+                          ("mvb_clip_vision_workspace_bytes", "mvb_clip_vision_forward", MvbControlnetArgs),
+                          ("mvb_clip_text_workspace_bytes", "mvb_clip_text_forward", MvbControlnetArgs)):
         fn(ws, LL, H, P(args))
         fn(run, I, H, P(args), C.c_void_p, LL, C.c_void_p)
 
@@ -405,6 +407,24 @@ class EngineModel:
             self._launch(a)
         self._keep = x   # the input must outlive the asynchronous launches
         return out
+
+    def _merge_lora(self, targets: Sequence[str], ups: Sequence[torch.Tensor], downs: Sequence[torch.Tensor],
+                    scales: Sequence[float], subtract: bool = False) -> None:
+        """W16 = fp16(W16 +- fp16(scale * (up @ down))) for every target (reference weight names), one `mvb_unet_merge_lora`
+        call (UNet and CLIP text encoder handles). The factors must be contiguous fp16 / fp32 tensors on this model's device."""
+        n = len(targets)
+        if not (len(ups) == len(downs) == len(scales) == n):
+            raise ValueError("targets, ups, downs and scales differ in length")
+        for t in list(ups) + list(downs):
+            if t.device != self.device or not t.is_contiguous():
+                raise ValueError(f"LoRA factors must be contiguous tensors on {self.device}")
+        up_arr = (MvbNamedTensor * max(n, 1))(*[_named(nm, u) for nm, u in zip(targets, ups)])
+        down_arr = (MvbNamedTensor * max(n, 1))(*[_named(nm, d) for nm, d in zip(targets, downs)])
+        sc = (C.c_float * max(n, 1))(*[float(s) for s in scales])
+        torch.cuda.current_stream(self.device).synchronize()      # the factors may still be in flight
+        rc = lib().mvb_unet_merge_lora(self._h, up_arr, down_arr, sc, n, int(bool(subtract)))
+        if rc != 0:
+            raise MvbError(f"mvb_unet_merge_lora ({rc}): {self._error()}")
 
     def debug_weight(self, name: str) -> torch.Tensor:
         """The packed matrix / convolution weight `name` read back into its reference shape, fp16 on the device."""

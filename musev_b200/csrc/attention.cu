@@ -1,4 +1,5 @@
-// wgmma flash attention (see attention.cuh). One kernel, templated on the padded head dim dp (the N of the P.V MMA).
+// wgmma flash attention (see attention.cuh). One kernel, templated on the padded head dim dp (the N of the P.V MMA) and on
+// the causal mask (CLIP text self attention: key tiles past the diagonal are skipped, the diagonal tile is masked).
 //
 // CTA = 384 threads = 3 warpgroups = 128 queries of one (frame, head):
 //   warpgroup 0, warp 0 : TMA producer -- Q once, then K and V tiles of 128 keys through their own smem rings (boxes of
@@ -67,7 +68,16 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b, float& back_sum
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-template <int DP>
+// Key tiles CTA blockIdx.x visits. The producer warp and both consumer warpgroups take their loop bound from this one
+// function: a disagreement would leave a warp waiting on an mbarrier that is never signalled. CAUSAL (one segment, the
+// query rows' own keys): query tile x needs key tiles 0..x only.
+template <bool CAUSAL>
+__device__ __forceinline__ int kv_tile_count(const AttnParams& p) {
+  const int n = (p.nk[0] + 127) / 128 + (p.nseg > 1 ? (p.nk[1] + 127) / 128 : 0);
+  return CAUSAL ? min(n, (int)blockIdx.x + 1) : n;
+}
+
+template <int DP, bool CAUSAL>
 __global__ void __launch_bounds__(384, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
                  const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
@@ -90,7 +100,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   const int q0 = blockIdx.x * 128;
   const int h = blockIdx.y;
   const int f = blockIdx.z;
-  const int ntiles = (p.nk[0] + 127) / 128 + (p.nseg > 1 ? (p.nk[1] + 127) / 128 : 0);
+  const int ntiles = kv_tile_count<CAUSAL>(p);
   const bool traced = p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
 
   if (threadIdx.x == 0) {
@@ -178,11 +188,31 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     att_stamp(tr, j, 0);
 
     // ---- online softmax on the two rows
-    if (valid < 128) {
+    if constexpr (!CAUSAL) {
+      if (valid < 128) {
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        if (8 * i + cq >= valid) { s[4 * i] = -INFINITY; s[4 * i + 2] = -INFINITY; }
-        if (8 * i + cq + 1 >= valid) { s[4 * i + 1] = -INFINITY; s[4 * i + 3] = -INFINITY; }
+        for (int i = 0; i < 16; ++i) {
+          if (8 * i + cq >= valid) { s[4 * i] = -INFINITY; s[4 * i + 2] = -INFINITY; }
+          if (8 * i + cq + 1 >= valid) { s[4 * i + 1] = -INFINITY; s[4 * i + 3] = -INFINITY; }
+        }
+      }
+    } else {
+      // the diagonal tile (k0 == q0) shows tile row r its keys 0..r only; column 0 is always kept, so no row (the tail
+      // rows past Nq included) is all -inf and the online softmax stays finite. Earlier tiles are whole.
+      int v0 = valid, v1 = valid;
+      if (j == (int)blockIdx.x) {
+        const int r0 = 64 * wg + 16 * wq + (lane >> 2);
+        v0 = min(valid, r0 + 1);
+        v1 = min(valid, r0 + 9);
+      }
+      if (v0 < 128 || v1 < 128) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          if (8 * i + cq >= v0) s[4 * i] = -INFINITY;
+          if (8 * i + cq + 1 >= v0) s[4 * i + 1] = -INFINITY;
+          if (8 * i + cq >= v1) s[4 * i + 2] = -INFINITY;
+          if (8 * i + cq + 1 >= v1) s[4 * i + 3] = -INFINITY;
+        }
       }
     }
     float mx0 = s[0], mx1 = s[2];
@@ -268,16 +298,26 @@ void set_attention_trace(long long* device_buffer) { g_attention_trace = device_
 
 typedef void (*AttnKernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                              const AttnParams);
-// instantiations for every padded head dim the launcher accepts (multiples of 16 up to 192)
-static const AttnKernelFn kAttnKernels[12] = {
-    attention_kernel<16>,  attention_kernel<32>,  attention_kernel<48>,  attention_kernel<64>,
-    attention_kernel<80>,  attention_kernel<96>,  attention_kernel<112>, attention_kernel<128>,
-    attention_kernel<144>, attention_kernel<160>, attention_kernel<176>, attention_kernel<192>};
+// instantiations for every padded head dim the launcher accepts (multiples of 16 up to 192), without and with the causal mask
+static const AttnKernelFn kAttnKernels[2][12] = {
+    {attention_kernel<16, false>,  attention_kernel<32, false>,  attention_kernel<48, false>,  attention_kernel<64, false>,
+     attention_kernel<80, false>,  attention_kernel<96, false>,  attention_kernel<112, false>, attention_kernel<128, false>,
+     attention_kernel<144, false>, attention_kernel<160, false>, attention_kernel<176, false>, attention_kernel<192, false>},
+    {attention_kernel<16, true>,  attention_kernel<32, true>,  attention_kernel<48, true>,  attention_kernel<64, true>,
+     attention_kernel<80, true>,  attention_kernel<96, true>,  attention_kernel<112, true>, attention_kernel<128, true>,
+     attention_kernel<144, true>, attention_kernel<160, true>, attention_kernel<176, true>, attention_kernel<192, true>}};
 
 cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char** err) {
   if (a.d % 8 || a.dp % 16 || a.dp < a.d || a.dp > 192 || a.nseg < 1 || a.nseg > 2 || a.heads < 1) {
     *err = "attention: head dim must be a multiple of 8, padded dim a multiple of 16 (<= 192), 1..2 KV segments";
     return cudaErrorInvalidValue;
+  }
+  if (a.causal) {
+    const AttnSegment& g = a.seg[0];
+    if (a.nseg != 1 || g.nk != a.Nq || g.fdiv != 1 || g.fmul != a.Nq || g.fadd != 0) {
+      *err = "attention: causal masking takes self attention only (one KV segment with nk = Nq, fdiv = 1, fmul = Nq, fadd = 0)";
+      return cudaErrorInvalidValue;
+    }
   }
   AttnParams p{};
   p.NF = a.NF; p.Nq = a.Nq; p.heads = a.heads; p.d = a.d; p.dp = a.dp;
@@ -299,11 +339,12 @@ cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char*
   else if (p.natoms == 2) { p.sk = 2; p.sv = 2; }
   else { p.sk = 2; p.sv = 1; }
   const int smem = (1 + p.sk + p.sv) * p.natoms * kAtomBytes + 1024 + 128 + 256;
-  const AttnKernelFn kernel = kAttnKernels[a.dp / 16 - 1];
-  static int max_set_dev[64][12] = {};     // per device (the attribute belongs to the device's context)
+  const int causal = a.causal ? 1 : 0;
+  const AttnKernelFn kernel = kAttnKernels[causal][a.dp / 16 - 1];
+  static int max_set_dev[64][2][12] = {};  // per device (the attribute belongs to the device's context)
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
-  int& max_set = max_set_dev[cur_dev & 63][a.dp / 16 - 1];
+  int& max_set = max_set_dev[cur_dev & 63][causal][a.dp / 16 - 1];
   if (smem > max_set) {
     cudaError_t e = cudaFuncSetAttribute(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(attention_kernel)"; return e; }
@@ -324,8 +365,8 @@ cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char*
   }
   static const bool trace = getenv("MVB_TRACE") != nullptr;
   if (trace)
-    fprintf(stderr, "MVB_TRACE attn NF=%d Nq=%d heads=%d d=%d nk0=%d nk1=%d acc=%d\n", a.NF, a.Nq, a.heads, a.d, p.nk[0],
-            p.nk[1], a.accumulate);
+    fprintf(stderr, "MVB_TRACE attn NF=%d Nq=%d heads=%d d=%d nk0=%d nk1=%d acc=%d causal=%d\n", a.NF, a.Nq, a.heads, a.d,
+            p.nk[0], p.nk[1], a.accumulate, causal);
   dim3 grid((a.Nq + 127) / 128, a.heads, a.NF);
   ProfScope prof(stream, KC_ATTENTION);
   kernel<<<grid, 384, smem, stream>>>(tq, tk0, tv0, tk1, tv1, p);

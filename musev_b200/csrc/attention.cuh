@@ -3,6 +3,7 @@
 //   * ReferEmbFuseAttention          (musev/models/attention_processor.py:629-750, K/V = reference tokens (+) own frame)
 //   * text / IP-Adapter cross attention (musev/models/attention_processor.py:176-359; diffusers attention_processor.py
 //     :1075-1250), the IP branch being a second call with accumulate = 1 and out_scale = ip_adapter_scale.
+//   * causal self attention of the CLIP text encoder (transformers models/clip/modeling_clip.py, CLIPTextTransformer).
 // out[f, q, h, :] = out_scale * softmax_k(Q K^T * scale) V   over the concatenation of up to two K/V segments.
 #pragma once
 #include <cuda_fp16.h>
@@ -34,6 +35,8 @@ struct AttnArgs {
   int accumulate;         // out += result
   int v_ones_col;         // every V row holds 1.0 at column h*dp + d (needs dp > d): row sums come from the MMA
   int variant = 0;        // accepted for ABI compatibility; every value runs the same kernel
+  int causal = 0;         // key k of a sequence is visible to query q only if k <= q (positions local to the sequence);
+                          // self attention only: nseg 1, nk = Nq, fdiv 1, fmul = Nq, fadd 0, anything else is rejected
 };
 
 cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char** err);

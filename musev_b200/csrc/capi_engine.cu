@@ -72,6 +72,18 @@ static bool clip_vision_config_ok(const mvb_config* cfg) {
   return cfg->norm_num_groups == 2 || cfg->norm_num_groups == 3;
 }
 
+// The CLIP text encoder (Engine::build_clip_text): the layer geometry of the vision tower; block_out_channels[2..3] =
+// max_position_embeddings (1..4096) and vocab_size (>= 1); out_channels = eos_token_id (>= 0).
+static bool clip_text_config_ok(const mvb_config* cfg) {
+  const int C = cfg->block_out_channels[0], I = cfg->block_out_channels[1], P = cfg->block_out_channels[2],
+            V = cfg->block_out_channels[3];
+  if (cfg->num_blocks != 4 || cfg->layers_per_block < 1 || P < 1 || P > 4096 || V < 1 || cfg->out_channels < 0) return false;
+  if (C < 64 || C > 2048 || C % 64 || cfg->heads < 1 || C % cfg->heads) return false;
+  const int d = C / cfg->heads;
+  if (d % 8 || d > 192 || I < 64 || I % 64 || !(cfg->norm_eps >= 0.f)) return false;
+  return cfg->norm_num_groups == 2 || cfg->norm_num_groups == 3;
+}
+
 // A handle of a validated configuration: MVB_ERR_STATE when out of host memory, MVB_ERR_CUDA when the device refused
 static int create(const mvb_config* cfg, int device, mvb::Kind kind, mvb_handle** out) {
   mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, kind);
@@ -183,6 +195,22 @@ int mvb_clip_vision_forward(mvb_handle* h, const mvb_controlnet_args* args, void
                             void* stream) {
   if (!h || !args) return MVB_ERR_INVALID;
   return h->e->clip_vision_forward(*args, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mvb_create_clip_text(const mvb_config* cfg, int device, mvb_handle** out) {
+  if (!cfg || !out || !clip_text_config_ok(cfg)) return MVB_ERR_INVALID;
+  return create(cfg, device, mvb::Kind::ClipText, out);
+}
+
+long long mvb_clip_text_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args) {
+  if (!h || !args) return -1;
+  return h->e->clip_text_workspace_bytes(*args);
+}
+
+int mvb_clip_text_forward(mvb_handle* h, const mvb_controlnet_args* args, void* workspace, long long workspace_bytes,
+                          void* stream) {
+  if (!h || !args) return MVB_ERR_INVALID;
+  return h->e->clip_text_forward(*args, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 void mvb_destroy(mvb_handle* h) {

@@ -33,7 +33,8 @@ extern "C" {
 
 const char* mvb_last_error(void) { return g_err; }
 
-int mvb_version(void) { return 3; }   // 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle
+// 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle; 4: the CLIP text handle, causal attention
+int mvb_version(void) { return 4; }
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   if (!d || !d->a0 || !d->weight || !d->out) return fail("mvb_op_conv_gemm: null pointer", cudaSuccess);
@@ -64,7 +65,7 @@ int mvb_op_small_conv(const void* x, int x_is_f32, int in_nchw, int cin, int H, 
   return e == cudaSuccess ? MVB_OK : fail(err, e);
 }
 
-int mvb_op_attention(const mvb_attention_desc* d, void* stream) {
+static int attention_op(const mvb_attention_desc* d, void* stream, int causal) {
   if (!d || !d->q || !d->out || !d->k[0] || !d->v[0]) return fail("mvb_op_attention: null pointer", cudaSuccess);
   AttnArgs a{};
   a.q = (const __half*)d->q; a.ldq = d->ldq; a.NF = d->NF; a.Nq = d->Nq; a.heads = d->heads; a.d = d->d; a.dp = d->dp;
@@ -75,11 +76,16 @@ int mvb_op_attention(const mvb_attention_desc* d, void* stream) {
     a.seg[s].fadd = d->fadd[s];
   }
   a.out = (__half*)d->out; a.ldo = d->ldo; a.out_scale = d->out_scale; a.accumulate = d->accumulate; a.v_ones_col = d->v_ones_col; a.variant = d->variant;
+  a.causal = causal;
   const char* err = nullptr;
   cudaError_t e = launch_attention((cudaStream_t)stream, a, &err);
   if (e != cudaSuccess) return fail(err, e);
   return MVB_OK;
 }
+
+int mvb_op_attention(const mvb_attention_desc* d, void* stream) { return attention_op(d, stream, 0); }
+
+int mvb_op_attention_causal(const mvb_attention_desc* d, void* stream) { return attention_op(d, stream, 1); }
 
 int mvb_tensor_map_cache_stats(unsigned long long* hits, unsigned long long* misses) {
   if (!hits || !misses) return fail("mvb_tensor_map_cache_stats: null pointer", cudaSuccess);

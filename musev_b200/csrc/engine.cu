@@ -10,6 +10,7 @@
 #include <algorithm>
 
 #include "attention.cuh"
+#include "clip_text.cuh"
 #include "clip_vision.cuh"
 #include "cond_embed.cuh"
 #include "conv_gemm.cuh"
@@ -284,6 +285,7 @@ void Engine::build() {
     case Kind::VaeEncoder: build_vae_encoder(); break;
     case Kind::PoseGuider: build_pose_guider(); break;
     case Kind::ClipVision: build_clip_vision(); break;
+    case Kind::ClipText: build_clip_text(); break;
   }
 }
 
@@ -374,7 +376,6 @@ void Engine::build_clip_vision() {
   const mvb_config& c = cfg_;
   const int C = c.block_out_channels[0], I = c.block_out_channels[1], p = c.block_out_channels[2], S = c.block_out_channels[3];
   const int P = (S / p) * (S / p), Kp = (c.in_channels * p * p + 63) / 64 * 64;
-  const int H = heads_, d = C / H, dp = pad16(d), hd = H * dp;
   const std::string e = "vision_model.embeddings.", v = "vision_model.";
   clip_patch_ = make_mat(C, Kp, false);
   reg_mat(e + "patch_embedding.weight", clip_patch_, 0, C, 0, 0, 0, C, c.in_channels * p * p);   // columns (c, ky, kx)
@@ -383,10 +384,19 @@ void Engine::build_clip_vision() {
   clip_pos_ = slab<float>((size_t)(P + 1) * C);
   reg_vec(e + "position_embedding.weight", clip_pos_, (P + 1) * C, (P + 1) * C);
   clip_pre_ = make_norm(v + "pre_layrnorm", C);
-  clip_.assign(c.layers_per_block, ClipLayer{});
-  for (int i = 0; i < c.layers_per_block; ++i) {
+  build_clip_layers(v + "encoder.layers.", C, I);
+  clip_post_ = make_norm(v + "post_layernorm", C);
+  reg_linear("visual_projection", clip_proj_, c.out_channels, C, false);
+}
+
+// cfg_.layers_per_block CLIPEncoderLayer (modeling_clip.py:354-386) under `<prefix><i>.`: q / k / v fused into one [3 H dp, C]
+// matrix with the heads padded to dp rows and the biases padded alike, out_proj, fc1 [I, C], fc2 [C, I] (all with bias)
+void Engine::build_clip_layers(const std::string& prefix, int C, int I) {
+  const int H = heads_, d = C / H, dp = pad16(d), hd = H * dp;
+  clip_.assign(cfg_.layers_per_block, ClipLayer{});
+  for (int i = 0; i < cfg_.layers_per_block; ++i) {
     ClipLayer& L = clip_[i];
-    const std::string q = v + "encoder.layers." + std::to_string(i) + ".";
+    const std::string q = prefix + std::to_string(i) + ".";
     L.ln1 = make_norm(q + "layer_norm1", C);
     L.qkv = make_mat(3 * hd, C, true);
     const char* proj[3] = {"q_proj", "k_proj", "v_proj"};
@@ -399,8 +409,22 @@ void Engine::build_clip_vision() {
     reg_linear(q + "mlp.fc1", L.fc1, I, C, true);
     reg_linear(q + "mlp.fc2", L.fc2, C, I, true);
   }
-  clip_post_ = make_norm(v + "post_layernorm", C);
-  reg_linear("visual_projection", clip_proj_, c.out_channels, C, false);
+}
+
+// CLIPTextModel.__init__ (transformers models/clip/modeling_clip.py: CLIPTextEmbeddings, CLIPEncoderLayer, CLIPTextTransformer
+// final_layer_norm). mvb_config: block_out_channels = {hidden, intermediate, max_position_embeddings, vocab_size},
+// layers_per_block = layers, heads, norm_eps, norm_num_groups = the MLP activation (conv_gemm act code 2 / 3),
+// out_channels = eos_token_id (read by the pooling only).
+void Engine::build_clip_text() {
+  const mvb_config& c = cfg_;
+  const int C = c.block_out_channels[0], I = c.block_out_channels[1], P = c.block_out_channels[2], V = c.block_out_channels[3];
+  const std::string e = "text_model.embeddings.", t = "text_model.";
+  clip_tok_ = make_mat(V, C, false);
+  reg_mat(e + "token_embedding.weight", clip_tok_, 0, V, 0, 0, 0, V, C);
+  clip_pos_ = slab<float>((size_t)P * C);
+  reg_vec(e + "position_embedding.weight", clip_pos_, P * C, P * C);
+  build_clip_layers(t + "encoder.layers.", C, I);
+  clip_final_ = make_norm(t + "final_layer_norm", C);
 }
 
 // AutoencoderKL decoder half: post_quant_conv + Decoder.__init__ (diffusers models/autoencoder_kl.py:102-104, vae.py:201-263):
@@ -777,6 +801,39 @@ struct Engine::Fwd {
   }
 
   // ---- stages shared by the model kinds
+  // CLIPEncoderLayer.forward (modeling_clip.py:363-386) for every layer, in place on the fp16 residual stream x [M = NFs Ts, C]:
+  // LN1, fused q / k / v (+ bias), softmax(q k^T d^-0.5) v per head over the Ts tokens of one sequence (causal: key k <= query
+  // q only, the text encoder's mask), out_proj + residual, LN2, fc1 + activation, fc2 + residual. Shared by both CLIP kinds.
+  void clip_encoder(__half* x, long long M, int NFs, int Ts, const std::vector<ClipLayer>& layers, bool causal) {
+    const mvb_config& c = E->cfg_;
+    const int C = c.block_out_channels[0], I = c.block_out_channels[1];
+    const int Hh = heads, d = C / Hh, dp = pad16(d), hd = Hh * dp;
+    const float eps = c.norm_eps;
+    for (size_t i = 0; i < layers.size(); ++i) {
+      const ClipLayer& L = layers[i];
+      const size_t mk = mark();
+      __half* nbuf = alloc_h(M, C);
+      ln(x, M, C, eps, L.ln1, nbuf);
+      __half* qkv = alloc_h(M, 3 * hd);
+      { Epilogue ep; ep.out = qkv; ep.ldc = 3 * hd; gemm(nbuf, M, C, L.qkv, ep); }
+      __half* ao = alloc_h(M, C);
+      AttnArgs aa{};   // eager_attention_forward (:261-280): softmax(q k^T d^-0.5) v per head over the Ts tokens of one sequence
+      aa.q = qkv; aa.ldq = 3 * hd; aa.NF = NFs; aa.Nq = Ts; aa.heads = Hh; aa.d = d; aa.dp = dp;
+      aa.scale = 1.f / sqrtf((float)d);
+      aa.nseg = 1;
+      aa.seg[0] = AttnSegment{qkv + hd, qkv + 2 * hd, 3 * hd, M, Ts, 1, Ts, 0};
+      aa.out = ao; aa.ldo = C; aa.out_scale = 1.f;
+      aa.causal = causal ? 1 : 0;
+      attn(aa);
+      { Epilogue ep; ep.out = x; ep.ldc = C; ep.res = x; ep.ld_res = C; gemm(ao, M, C, L.out, ep); }
+      ln(x, M, C, eps, L.ln2, nbuf);
+      __half* h = alloc_h(M, I);
+      { Epilogue ep; ep.out = h; ep.ldc = I; ep.act = c.norm_num_groups; gemm(nbuf, M, C, L.fc1, ep); }   // CLIPMLP :347-351
+      { Epilogue ep; ep.out = x; ep.ldc = C; ep.res = x; ep.ld_res = C; gemm(h, M, I, L.fc2, ep); }
+      release(mk);
+      tap("encoder.layers." + std::to_string(i), x, M, C);
+    }
+  }
   // conv_in at the full resolution: im2col of src (NCTHW [B, cin, T, H, W], 9 cin <= 64 columns) + one GEMM into x
   // [NF*H*W, m.N]; res (NCHW [NF, m.N, H, W]) or null is added in the epilogue
   void conv_in(__half* x, const void* src, int src_f32, int cin, const Mat& m, const void* res, int res_f32,
@@ -1590,9 +1647,8 @@ static const char* clip_vision_shape_error(const mvb_controlnet_args& a, const m
 bool Engine::run_clip_vision(const mvb_controlnet_args& a, Arena& ar, cudaStream_t s) {
   const mvb_config& c = cfg_;
   if (const char* bad = clip_vision_shape_error(a, c)) { err_ = bad; return false; }
-  const int C = c.block_out_channels[0], I = c.block_out_channels[1], p = c.block_out_channels[2], S = c.block_out_channels[3];
+  const int C = c.block_out_channels[0], p = c.block_out_channels[2], S = c.block_out_channels[3];
   const int P = (S / p) * (S / p), T = P + 1, Kp = clip_patch_.K, NF = a.NF;
-  const int Hh = heads_, d = C / Hh, dp = pad16(d), hd = Hh * dp;
   const float eps = c.norm_eps;
   const long long M = (long long)NF * T;
   mvb_unet_args ua{};
@@ -1618,29 +1674,7 @@ bool Engine::run_clip_vision(const mvb_controlnet_args& a, Arena& ar, cudaStream
   }
   f.tap("embeddings", x, M, C);
   // ---- encoder layers (CLIPEncoderLayer.forward :363-386)
-  for (size_t i = 0; i < clip_.size(); ++i) {
-    const ClipLayer& L = clip_[i];
-    const size_t mk = f.mark();
-    __half* nbuf = f.alloc_h(M, C);
-    f.ln(x, M, C, eps, L.ln1, nbuf);
-    __half* qkv = f.alloc_h(M, 3 * hd);
-    { Epilogue ep; ep.out = qkv; ep.ldc = 3 * hd; f.gemm(nbuf, M, C, L.qkv, ep); }
-    __half* ao = f.alloc_h(M, C);
-    AttnArgs aa{};   // eager_attention_forward (:261-280): softmax(q k^T d^-0.5) v per head over the T tokens of one image
-    aa.q = qkv; aa.ldq = 3 * hd; aa.NF = NF; aa.Nq = T; aa.heads = Hh; aa.d = d; aa.dp = dp;
-    aa.scale = 1.f / sqrtf((float)d);
-    aa.nseg = 1;
-    aa.seg[0] = AttnSegment{qkv + hd, qkv + 2 * hd, 3 * hd, M, T, 1, T, 0};
-    aa.out = ao; aa.ldo = C; aa.out_scale = 1.f;
-    f.attn(aa);
-    { Epilogue ep; ep.out = x; ep.ldc = C; ep.res = x; ep.ld_res = C; f.gemm(ao, M, C, L.out, ep); }
-    f.ln(x, M, C, eps, L.ln2, nbuf);
-    __half* h = f.alloc_h(M, I);
-    { Epilogue ep; ep.out = h; ep.ldc = I; ep.act = c.norm_num_groups; f.gemm(nbuf, M, C, L.fc1, ep); }   // CLIPMLP :347-351
-    { Epilogue ep; ep.out = x; ep.ldc = C; ep.res = x; ep.ld_res = C; f.gemm(h, M, I, L.fc2, ep); }
-    f.release(mk);
-    f.tap("encoder.layers." + std::to_string(i), x, M, C);
-  }
+  f.clip_encoder(x, M, NF, T, clip_, false);
   // ---- outputs: last_hidden_state is the encoder output (not post-normalised, :684); image_embeds = visual_projection(
   // post_layernorm(last_hidden_state[:, 0])) (:685-686, :1068-1069)
   if (a.outs[1] && !ar.dry && f.ok) {
@@ -1659,6 +1693,50 @@ bool Engine::run_clip_vision(const mvb_controlnet_args& a, Arena& ar, cudaStream
     f.ln(pooled, NF, C, eps, clip_post_, pn);
     Epilogue ep; ep.out = (__half*)a.outs[0]; ep.ldc = c.out_channels; ep.out_f32 = a.out_is_f32 ? 1 : 0;
     f.gemm(pn, NF, C, clip_proj_, ep, false);
+  }
+  return f.ok;
+}
+
+static const char* clip_text_shape_error(const mvb_controlnet_args& a, const mvb_config& c) {
+  if (a.sample_is_f32) return "clip text: sample holds int64 input_ids (sample_is_f32 must be 0)";
+  if (a.NF < 1 || a.NF > 1024) return "clip text: NF (sequences per call) must be in 1..1024";
+  if (a.H < 1 || a.H > c.block_out_channels[2] || a.W != 1)
+    return "clip text: H (sequence length) must be in 1..max_position_embeddings and W must be 1";
+  if (a.n_out != 2) return "clip text: n_out must be 2 (outs[0] = last_hidden_state, outs[1] = pooler_output)";
+  if (!a.outs[0] && !a.outs[1]) return "clip text: no output requested (outs[0] and outs[1] are both NULL)";
+  return nullptr;
+}
+
+// CLIPTextModel.forward (transformers models/clip/modeling_clip.py, CLIPTextTransformer.forward): a.sample = int64 input_ids
+// [NF, L]. Embeddings (token + position), the causal encoder layers, final_layer_norm -> last_hidden_state; pooler_output =
+// its row at the eos position (the config's eos_token_id picks the rule, clip_text.cuh).
+bool Engine::run_clip_text(const mvb_controlnet_args& a, Arena& ar, cudaStream_t s) {
+  const mvb_config& c = cfg_;
+  if (const char* bad = clip_text_shape_error(a, c)) { err_ = bad; return false; }
+  const int C = c.block_out_channels[0], V = c.block_out_channels[3], NF = a.NF, L = a.H;
+  const long long M = (long long)NF * L;
+  const int64_t* ids = (const int64_t*)a.sample;
+  mvb_unet_args ua{};
+  ua.B = NF; ua.T = 1; ua.H = 1; ua.W = 1;
+  Fwd f(this, ar, s, ua, true);
+  __half* x = f.alloc_h(M, C);
+  if (!ar.dry && f.ok) {
+    cudaError_t e = clip_text_embed(s, ids, NF, L, C, V, clip_tok_.w, clip_pos_, x);
+    if (e != cudaSuccess) f.fail("clip_text_embed", e);
+  }
+  f.tap("embeddings", x, M, C);
+  f.clip_encoder(x, M, NF, L, clip_, true);
+  __half* y = f.alloc_h(M, C);
+  f.ln(x, M, C, c.norm_eps, clip_final_, y);
+  f.tap("final_layer_norm", y, M, C);
+  if (a.outs[0] && !ar.dry && f.ok) {
+    cudaError_t e = a.out_is_f32 ? half_to_float(s, y, M * C, (float*)a.outs[0])
+                                 : cudaMemcpyAsync(a.outs[0], y, (size_t)M * C * sizeof(__half), cudaMemcpyDeviceToDevice, s);
+    if (e != cudaSuccess) f.fail("clip text last_hidden_state", e);
+  }
+  if (a.outs[1] && !ar.dry && f.ok) {
+    cudaError_t e = clip_text_pool(s, ids, NF, L, c.out_channels, y, C, a.outs[1], a.out_is_f32);
+    if (e != cudaSuccess) f.fail("clip_text_pool", e);
   }
   return f.ok;
 }
@@ -1739,6 +1817,14 @@ long long Engine::clip_vision_workspace_bytes(const mvb_controlnet_args& a) {
 int Engine::clip_vision_forward(const mvb_controlnet_args& a, void* ws, long long wbytes, cudaStream_t stream) {
   const char* bad = (!a.sample || !ws) ? kNullArg : clip_vision_shape_error(a, cfg_);
   return launch(&Engine::run_clip_vision, {Kind::ClipVision}, "not a CLIP vision handle", bad, a, ws, wbytes, stream);
+}
+
+long long Engine::clip_text_workspace_bytes(const mvb_controlnet_args& a) {
+  return dry_run(&Engine::run_clip_text, {Kind::ClipText}, "not a CLIP text handle", a);
+}
+int Engine::clip_text_forward(const mvb_controlnet_args& a, void* ws, long long wbytes, cudaStream_t stream) {
+  const char* bad = (!a.sample || !ws) ? kNullArg : clip_text_shape_error(a, cfg_);
+  return launch(&Engine::run_clip_text, {Kind::ClipText}, "not a CLIP text handle", bad, a, ws, wbytes, stream);
 }
 
 }  // namespace mvb

@@ -143,7 +143,8 @@ struct CondConv {
   bool act = true;       // SiLU after every conv except conv_out
 };
 
-// One pre-norm ViT encoder layer (transformers CLIPEncoderLayer, models/clip/modeling_clip.py:354-386)
+// One pre-norm CLIP encoder layer (transformers CLIPEncoderLayer, models/clip/modeling_clip.py:354-386), of the vision tower
+// and of the text encoder alike (Engine::build_clip_layers, Fwd::clip_encoder)
 struct ClipLayer {
   Norm ln1, ln2;
   Mat qkv;            // q | k | v projections, heads padded to dp columns (rowmode 1), biases padded alike
@@ -167,8 +168,9 @@ struct Arena {
 // ReferenceNet: ReferenceNet2D encoder + mid block (musev/models/referencenet.py);
 // VaeDecoder / VaeEncoder: the AutoencoderKL halves (diffusers models/autoencoder_kl.py, vae.py);
 // PoseGuider: musev/models/controlnet.py:326-371;
-// ClipVision: transformers CLIPVisionModelWithProjection (models/clip/modeling_clip.py), the IP-Adapter image encoder
-enum class Kind { UNet, ControlNet, ReferenceNet, VaeDecoder, VaeEncoder, PoseGuider, ClipVision };
+// ClipVision: transformers CLIPVisionModelWithProjection (models/clip/modeling_clip.py), the IP-Adapter image encoder;
+// ClipText: transformers CLIPTextModel, the prompt encoder
+enum class Kind { UNet, ControlNet, ReferenceNet, VaeDecoder, VaeEncoder, PoseGuider, ClipVision, ClipText };
 
 class Engine {
  public:
@@ -178,7 +180,7 @@ class Engine {
   int load_weights(const mvb_named_tensor* tensors, int n);
   int finalize();
   // LoRA merge into the packed weights (csrc/lora.cu; musev/utils/model_util.py:108-262,468-475). up[i].name names the
-  // target by its reference weight name; subtract = 1 removes a previous merge. UNet handles only, after finalize.
+  // target by its reference weight name; subtract = 1 removes a previous merge. UNet and CLIP text handles, after finalize.
   int merge_lora(const mvb_named_tensor* up, const mvb_named_tensor* down, const float* scale, int n, int subtract);
   // Packed matrix / convolution weight -> fp16 in the reference layout (device pointer, nsrc x ksrc elements)
   int read_weight(const char* name, void* dst_f16);
@@ -192,6 +194,8 @@ class Engine {
   int pose_guider_forward(const mvb_vae_decode_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long clip_vision_workspace_bytes(const mvb_controlnet_args& a);
   int clip_vision_forward(const mvb_controlnet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
+  long long clip_text_workspace_bytes(const mvb_controlnet_args& a);
+  int clip_text_forward(const mvb_controlnet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   long long controlnet_workspace_bytes(const mvb_controlnet_args& a);
   int controlnet_forward(const mvb_controlnet_args& a, void* workspace, long long workspace_bytes, cudaStream_t stream);
   Kind kind() const { return kind_; }
@@ -210,6 +214,8 @@ class Engine {
   void build_vae_mid(const std::string& p, int C);
   void build_pose_guider();
   void build_clip_vision();
+  void build_clip_text();
+  void build_clip_layers(const std::string& prefix, int C, int I);
   template <typename T> T* slab(size_t n);
   Mat make_mat(int N, int K, bool bias);
   Norm make_norm(const std::string& p, int C);
@@ -241,6 +247,7 @@ class Engine {
   bool run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
   bool run_pose_guider(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s);
   bool run_clip_vision(const mvb_controlnet_args& a, Arena& ar, cudaStream_t s);
+  bool run_clip_text(const mvb_controlnet_args& a, Arena& ar, cudaStream_t s);
 
   mvb_config cfg_;
   int device_ = 0, num_sms_ = 132;
@@ -292,7 +299,11 @@ class Engine {
   float* clip_cls_ = nullptr;
   float* clip_pos_ = nullptr;
   Norm clip_pre_, clip_post_;
-  std::vector<ClipLayer> clip_;
+  std::vector<ClipLayer> clip_;   // the encoder layers of either CLIP kind (build_clip_layers)
+  // ClipText (mvb_create_clip_text): token_embedding [vocab, C] fp16 (a Mat without bias), position_embedding in clip_pos_,
+  // the layers in clip_, final_layer_norm
+  Mat clip_tok_;
+  Norm clip_final_;
 };
 
 // Channel count a PoseGuider activation is stored with: 16 / 32 as is (small-channel kernel), others padded to 64k.

@@ -1,4 +1,4 @@
-// LoRA merge into the packed UNet weights, and read-back of a packed weight in the reference layout. Both map packed
+// LoRA merge into the packed UNet / CLIP text encoder weights, and read-back of a packed weight in the reference layout. Both map packed
 // elements to source elements with the packer's src_row / src_col (engine.cuh).
 // Reference arithmetic: musev/utils/model_util.py:153-262 (update_pipeline_lora_model) and :468-475 (unload_lora):
 //   delta32 = fl32(scale) * (up @ down)  (fp32),  delta16 = fp16(delta32),  W16 = fp16(float(W16) +- float(delta16)).
@@ -115,7 +115,10 @@ static std::string shape_str(const mvb_named_tensor& t) {
 }
 
 int Engine::merge_lora(const mvb_named_tensor* up, const mvb_named_tensor* down, const float* scale, int n, int subtract) {
-  if (kind_ != Kind::UNet) { err_ = "mvb_unet_merge_lora: LoRA weights merge into a UNet3DConditionModel handle only"; return MVB_ERR_STATE; }
+  if (kind_ != Kind::UNet && kind_ != Kind::ClipText) {
+    err_ = "mvb_unet_merge_lora: LoRA weights merge into a UNet3DConditionModel or CLIP text encoder handle only";
+    return MVB_ERR_STATE;
+  }
   if (!finalized_) { err_ = "mvb_unet_merge_lora: call mvb_finalize first"; return MVB_ERR_STATE; }
   if (n < 0 || (n > 0 && (!up || !down || !scale))) { err_ = "mvb_unet_merge_lora: bad arguments"; return MVB_ERR_INVALID; }
   if (n == 0) return MVB_OK;
@@ -129,7 +132,8 @@ int Engine::merge_lora(const mvb_named_tensor* up, const mvb_named_tensor* down,
     const std::string name = u.name;
     auto it = loaders_.find(name);
     if (it == loaders_.end() || it->second.kind != LK_MAT) {
-      err_ = "mvb_unet_merge_lora: " + name + " is not a mergeable (matrix or convolution) weight of this UNet";
+      err_ = "mvb_unet_merge_lora: " + name + " is not a mergeable (matrix or convolution) weight of this " +
+             (kind_ == Kind::UNet ? "UNet" : "text encoder");
       return MVB_ERR_INVALID;
     }
     if (!seen.insert(name).second) { err_ = "mvb_unet_merge_lora: target " + name + " appears twice in one call"; return MVB_ERR_INVALID; }

@@ -250,3 +250,19 @@ def clip_vision_flops(cfg, N: int) -> Dict[str, float]:
         lin(N * T, I, C)
     lin(N, C, cfg.projection_dim)
     return _vae_total(f)
+
+
+def clip_text_flops(cfg, N: int, L: int) -> Dict[str, float]:
+    """`CLIPTextModel.forward` on N sequences of L tokens (ClipTextConfig `cfg`; transformers models/clip/modeling_clip.py),
+    2 M N K per matrix product: q / k / v / out_proj / fc1 / fc2 per layer, and q k^T and P v per head over all L x L pairs
+    (the causal mask is an addend; the reference's eager attention multiplies the masked pairs too). SD-1.5 at L = 77:
+    13.30 GFLOP per sequence."""
+    f, conv, lin, attn = _vae_counters()
+    C, I = cfg.hidden_size, cfg.intermediate_size
+    for _ in range(cfg.num_hidden_layers):
+        for _ in range(4):                      # q, k, v, out_proj
+            lin(N * L, C, C)
+        attn(N * cfg.num_attention_heads, L, L, C // cfg.num_attention_heads)
+        lin(N * L, C, I)
+        lin(N * L, I, C)
+    return _vae_total(f)

@@ -5,8 +5,9 @@ Drop-ins for musev/utils/model_util.py:98-475 (`LORA_BLOCK_WEIGHT_MAP`, `update_
 base-model `lora_dict` and the LCM-LoRA of `lcm_lora_dct` (pipeline_controlnet_predictor.py:296-327).
 
 Keys are kohya style, the only format the reference reads: `<prefix>_<module path with "_">.lora_down.weight`,
-`.lora_up.weight` and an optional `.alpha`. UNet keys go to the engine (`mvb_unet_merge_lora`, musev_b200/csrc/lora.cu),
-keys containing "text" go to the torch text encoder with the reference's own arithmetic. Per target:
+`.lora_up.weight` and an optional `.alpha`. UNet keys go to the engine (`mvb_unet_merge_lora`, musev_b200/csrc/lora.cu).
+Keys containing "text" go to the engine too when `pipeline.text_encoder` is the engine `CLIPTextModel` (same entry point,
+same arithmetic), and otherwise to the torch text encoder with the reference's own arithmetic. Per target:
     scale = strength * (alpha / rank if alpha is present else 1)
     delta16 = fp16(fl32(scale) * (up @ down)) * LORA_BLOCK_WEIGHT_MAP[...][block]
     W16 = fp16(W16 + delta16), and W16 = fp16(W16 - delta16) on unload (not guaranteed to restore the original bits).
@@ -20,7 +21,7 @@ from typing import Dict, List, Optional, Tuple, Union
 
 import torch
 
-from .schema import UNetConfig, unet_param_shapes
+from .schema import ClipTextConfig, UNetConfig, clip_text_param_shapes, kohya_text_name_map, unet_param_shapes
 
 # musev/utils/model_util.py:98-104. Entry 0 is the text encoder, entries 1..16 follow LORA_UNET_LAYERS.
 LORA_BLOCK_WEIGHT_MAP = {
@@ -169,8 +170,9 @@ def update_pipeline_lora_model(pipeline, lora: Union[str, Dict[str, torch.Tensor
                                lora_unet_layers=LORA_UNET_LAYERS, lora_block_weight_str: str = "ALL",
                                need_unload: bool = False):
     """Drop-in for musev/utils/model_util.py:108-262 with `pipeline.unet` a musev_b200 `UNet3DConditionModel`: the UNet
-    targets of one LoRA are merged by one engine call; text-encoder targets are merged into `pipeline.text_encoder` in
-    torch. `alpha` is the strength. Everything is validated before any weight changes."""
+    targets of one LoRA are merged by one engine call. Text-encoder targets are merged by one more engine call when
+    `pipeline.text_encoder` is the engine `CLIPTextModel` (block weight `weights[0]`), and into the torch module otherwise.
+    `alpha` is the strength. Everything is validated before any weight changes."""
     weights = block_weights(lora_block_weight_str)
     sd = _load(lora)
     unet = pipeline.unet
@@ -179,9 +181,24 @@ def update_pipeline_lora_model(pipeline, lora: Union[str, Dict[str, torch.Tensor
     names = kohya_name_map(unet.cfg)
     shapes = unet_param_shapes(unet.cfg)
     dev = unet.device
-    eng, text = [], []
+    te = getattr(pipeline, "text_encoder", None)
+    te_engine = _is_engine_text_encoder(te)
+    te_names = kohya_text_name_map(te.cfg) if te_engine else None
+    te_shapes = clip_text_param_shapes(te.cfg) if te_engine else None
+    eng, text, te_eng = [], [], []
     for t in pair_keys(sd):
         key = t.up_key
+        if "text" in key and te_engine:
+            mod = t.module
+            name = te_names.get(mod[len(lora_prefix_text_encoder) + 1:]) if mod.startswith(lora_prefix_text_encoder + "_") else None
+            if name is None:
+                raise ValueError(f"LoRA key {key!r} names no linear-layer weight of this text encoder")
+            up, down, r = factors(sd, t, te_shapes[name])
+            if r > MAX_RANK:
+                raise ValueError(f"{mod}: rank {r} exceeds {MAX_RANK}")
+            s = target_scale(sd, t, alpha, r) * block_weight(key, weights, lora_unet_layers)
+            te_eng.append((name, _dev(up, te.device), _dev(down, te.device), s))
+            continue
         if "text" in key:
             up, down, r = factors(sd, t)
             text.append((t, up, down, r))
@@ -201,6 +218,10 @@ def update_pipeline_lora_model(pipeline, lora: Union[str, Dict[str, torch.Tensor
     if eng:
         unet._merge_lora([e[0] for e in eng], [e[1] for e in eng], [e[2] for e in eng], [e[3] for e in eng], subtract=False)
         unload += [{"layer": unet, "name": n, "up": u, "down": d, "scale": s} for n, u, d, s in eng]
+    if te_eng:
+        te._merge_lora([e[0] for e in te_eng], [e[1] for e in te_eng], [e[2] for e in te_eng], [e[3] for e in te_eng],
+                       subtract=False)
+        unload += [{"layer": te, "name": n, "up": u, "down": d, "scale": s} for n, u, d, s in te_eng]
     for layer, t, up, down, r in text_layers:
         p = layer.weight
         delta = text_delta(up.to(p.device), down.to(p.device), target_scale(sd, t, alpha, r),
@@ -251,6 +272,11 @@ def unload_lora(unload_dict: List[Dict]) -> None:
     flush()
     gc.collect()
     torch.cuda.empty_cache()
+
+
+def _is_engine_text_encoder(te) -> bool:
+    """The engine `CLIPTextModel` (or a stand-in with its surface): LoRA factors go to its `_merge_lora`."""
+    return te is not None and hasattr(te, "_merge_lora") and isinstance(getattr(te, "cfg", None), ClipTextConfig)
 
 
 def _dev(t: torch.Tensor, dev) -> torch.Tensor:

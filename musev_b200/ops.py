@@ -98,9 +98,11 @@ def small_conv(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tenso
     return out
 
 
-def attention(q, segs, NF, Nq, heads, d, dp, scale, out=None, out_scale=1.0, accumulate=False, v_ones_col=False, variant=0):
+def attention(q, segs, NF, Nq, heads, d, dp, scale, out=None, out_scale=1.0, accumulate=False, v_ones_col=False, variant=0,
+              causal=False):
     """q: [NF*Nq, >=heads*dp] fp16 (row stride taken from the tensor); segs: list of dicts
-    {k, v, nk, fdiv, fmul, fadd} with k/v [rows, >=heads*dp] views sharing a row stride."""
+    {k, v, nk, fdiv, fmul, fadd} with k/v [rows, >=heads*dp] views sharing a row stride. causal=True masks key k of a
+    sequence from query q unless k <= q (`mvb_op_attention_causal`; one segment of the queries' own sequence only)."""
     assert q.dtype == torch.float16 and q.stride(1) == 1
     if out is None:
         out = torch.zeros((NF * Nq, heads * d), dtype=torch.float16, device=q.device)
@@ -115,7 +117,8 @@ def attention(q, segs, NF, Nq, heads, d, dp, scale, out=None, out_scale=1.0, acc
     a.out, a.ldo, a.out_scale, a.accumulate = out.data_ptr(), out.stride(0), out_scale, int(accumulate)
     a.v_ones_col = int(v_ones_col)
     a.variant = int(variant)
-    _capi.check(_capi.lib().mvb_op_attention(C.byref(a), _stream()))
+    op = _capi.lib().mvb_op_attention_causal if causal else _capi.lib().mvb_op_attention
+    _capi.check(op(C.byref(a), _stream()))
     return out
 
 

@@ -496,20 +496,31 @@ class ClipVisionConfig:
         return (self.image_size // self.patch_size) ** 2
 
 
-def clip_vision_config(config) -> ClipVisionConfig:
-    """A `ClipVisionConfig` from a `ClipVisionConfig`, a `transformers.CLIPVisionConfig` or a dict (other keys are ignored).
-    Raises ValueError for an activation other than gelu / quick_gelu and for geometry the engine's kernels do not take."""
-    if isinstance(config, ClipVisionConfig):
-        cfg = ClipVisionConfig(**asdict(config))
-    else:
-        get = config.get if isinstance(config, dict) else (lambda k, d=None: getattr(config, k, d))
-        cfg = ClipVisionConfig(**{f.name: get(f.name, f.default) for f in fields(ClipVisionConfig)})
+def _read_config(config, cls):
+    """A `cls` dataclass from an instance of it, a transformers config object or a dict (other keys are ignored)."""
+    if isinstance(config, cls):
+        return cls(**asdict(config))
+    get = config.get if isinstance(config, dict) else (lambda k, d=None: getattr(config, k, d))
+    return cls(**{f.name: get(f.name, f.default) for f in fields(cls)})
+
+
+def _check_clip_layers(cfg) -> None:
+    """The encoder-layer geometry both CLIP towers share on the engine (conv_gemm K, the attention kernel's head dims)."""
     if cfg.hidden_act not in CLIP_ACT_CODES:
         raise ValueError(f"hidden_act {cfg.hidden_act!r} is not supported (the engine has {sorted(CLIP_ACT_CODES)})")
     C, H = cfg.hidden_size, cfg.num_attention_heads
     if C % 64 or not 64 <= C <= 2048 or H < 1 or C % H or (C // H) % 8 or C // H > 192:
         raise ValueError(f"hidden_size {C} / {H} heads: the hidden size must be a multiple of 64 (at most 2048) and the "
                          "head dim a multiple of 8, at most 192")
+    if cfg.intermediate_size % 64 or cfg.intermediate_size < 64 or cfg.num_hidden_layers < 1:
+        raise ValueError("intermediate_size must be a positive multiple of 64 and num_hidden_layers at least 1")
+
+
+def clip_vision_config(config) -> ClipVisionConfig:
+    """A `ClipVisionConfig` from a `ClipVisionConfig`, a `transformers.CLIPVisionConfig` or a dict (other keys are ignored).
+    Raises ValueError for an activation other than gelu / quick_gelu and for geometry the engine's kernels do not take."""
+    cfg = _read_config(config, ClipVisionConfig)
+    _check_clip_layers(cfg)
     if cfg.intermediate_size % 64 or cfg.projection_dim % 8 or cfg.image_size % cfg.patch_size or cfg.num_hidden_layers < 1:
         raise ValueError("intermediate_size must be a multiple of 64, projection_dim of 8, image_size of patch_size")
     if not 1 <= cfg.num_channels <= 4:
@@ -544,4 +555,74 @@ def clip_vision_param_shapes(cfg: ClipVisionConfig) -> "OrderedDict[str, Tuple[i
     out["vision_model.post_layernorm.weight"] = (C,)
     out["vision_model.post_layernorm.bias"] = (C,)
     out["visual_projection.weight"] = (cfg.projection_dim, C)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ CLIP text encoder
+@dataclass
+class ClipTextConfig:
+    """The `transformers.CLIPTextConfig` fields `CLIPTextModel` computes with. The defaults are SD-1.5's
+    `text_encoder/config.json` (OpenAI CLIP ViT-L/14 text tower): 123 M parameters, 77 positions, and the legacy
+    `eos_token_id = 2`, which makes the pooled row the argmax of the ids (the tokenizer's eos, 49407, is the largest id)."""
+    vocab_size: int = 49408
+    hidden_size: int = 768
+    intermediate_size: int = 3072
+    num_hidden_layers: int = 12
+    num_attention_heads: int = 12
+    max_position_embeddings: int = 77
+    hidden_act: str = "quick_gelu"
+    layer_norm_eps: float = 1e-5
+    bos_token_id: int = 0
+    eos_token_id: int = 2
+    pad_token_id: int = 1
+
+
+def clip_text_config(config) -> ClipTextConfig:
+    """A `ClipTextConfig` from a `ClipTextConfig`, a `transformers.CLIPTextConfig` or a dict (other keys are ignored). Raises
+    ValueError for an activation other than gelu / quick_gelu and for geometry the engine's kernels do not take."""
+    cfg = _read_config(config, ClipTextConfig)
+    _check_clip_layers(cfg)
+    if not 1 <= cfg.max_position_embeddings <= 4096 or cfg.vocab_size < 1:
+        raise ValueError(f"max_position_embeddings must be 1..4096 and vocab_size positive, got "
+                         f"{cfg.max_position_embeddings} / {cfg.vocab_size}")
+    if cfg.eos_token_id is None or cfg.eos_token_id < 0:
+        raise ValueError(f"eos_token_id must be a non-negative id, got {cfg.eos_token_id}")
+    return cfg
+
+
+def clip_text_param_shapes(cfg: ClipTextConfig) -> "OrderedDict[str, Tuple[int, ...]]":
+    """name -> shape of `transformers.CLIPTextModel.state_dict()` (models/clip/modeling_clip.py; the `position_ids` buffer is
+    not part of it)."""
+    out: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    C, I = cfg.hidden_size, cfg.intermediate_size
+    out["text_model.embeddings.token_embedding.weight"] = (cfg.vocab_size, C)
+    out["text_model.embeddings.position_embedding.weight"] = (cfg.max_position_embeddings, C)
+    for i in range(cfg.num_hidden_layers):
+        q = f"text_model.encoder.layers.{i}."
+        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
+            out[f"{q}self_attn.{n}.weight"] = (C, C)
+            out[f"{q}self_attn.{n}.bias"] = (C,)
+        out[q + "layer_norm1.weight"] = (C,)
+        out[q + "layer_norm1.bias"] = (C,)
+        out[q + "mlp.fc1.weight"] = (I, C)
+        out[q + "mlp.fc1.bias"] = (I,)
+        out[q + "mlp.fc2.weight"] = (C, I)
+        out[q + "mlp.fc2.bias"] = (C,)
+        out[q + "layer_norm2.weight"] = (C,)
+        out[q + "layer_norm2.bias"] = (C,)
+    out["text_model.final_layer_norm.weight"] = (C,)
+    out["text_model.final_layer_norm.bias"] = (C,)
+    return out
+
+
+def kohya_text_name_map(cfg: ClipTextConfig) -> "OrderedDict[str, str]":
+    """kohya module name (without the `lora_te_` prefix) -> reference weight name, for every linear-layer matrix of the text
+    encoder (q / k / v / out_proj, fc1, fc2: the modules kohya's text-encoder LoRAs target): the inverse of
+    `name[:-len(".weight")].replace(".", "_")`, which is injective over this schema (asserted)."""
+    out: "OrderedDict[str, str]" = OrderedDict()
+    for name, shape in clip_text_param_shapes(cfg).items():
+        if name.endswith(".weight") and len(shape) == 2 and ".encoder.layers." in name:
+            k = name[:-7].replace(".", "_")
+            assert k not in out, f"kohya names collide: {out[k]} and {name}"
+            out[k] = name
     return out

@@ -14,8 +14,8 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from .schema import (ClipVisionConfig, ControlNetConfig, ImageProjConfig, PoseGuiderConfig, ReferenceNetConfig, UNetConfig,
-                     VAEConfig, clip_vision_param_shapes, controlnet_param_shapes, image_proj_param_shapes, pose_guider_param_shapes, refer_emb_shapes,
+from .schema import (ClipTextConfig, ClipVisionConfig, ControlNetConfig, ImageProjConfig, PoseGuiderConfig, ReferenceNetConfig, UNetConfig,
+                     VAEConfig, clip_text_param_shapes, clip_vision_param_shapes, controlnet_param_shapes, image_proj_param_shapes, pose_guider_param_shapes, refer_emb_shapes,
                      referencenet_param_shapes, unet_param_shapes, vae_decoder_param_shapes, vae_encoder_param_shapes)
 
 _BRANCH_OUT = ("conv2.weight", "proj_out.weight", "to_out.0.weight", "ff.net.2.weight", "conv4.3.weight")
@@ -267,3 +267,58 @@ def make_clip_pixel_values(n: int, image_size: int = 224, seed: int = 3131, chan
     mean = torch.tensor((OPENAI_CLIP_MEAN * 2)[:channels]).view(1, -1, 1, 1)
     std = torch.tensor((OPENAI_CLIP_STD * 2)[:channels]).view(1, -1, 1, 1)
     return (img - mean) / std
+
+
+def make_clip_text_state_dict(cfg: ClipTextConfig, seed: int = 0, dtype: torch.dtype = torch.float32,
+                              outlier_channels: int = 0, outlier_offset: float = 40.0) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded weights for `CLIPTextModel` (`clip_text_param_shapes`), one generator per name as in `make_state_dict`.
+    Matrices have std 1 / sqrt(fan_in); the residual-branch outputs (`out_proj`, `fc2`) are scaled by
+    1 / sqrt(2 num_hidden_layers), so the residual stream stays O(1) over the layers. LayerNorm weights are 1 + 0.1 N(0, 1),
+    biases 0.02 N(0, 1), the token embedding N(0, 1) and the position embedding 0.5 N(0, 1).
+
+    `outlier_channels` > 0 picks that many channels (seeded) and adds `outlier_offset` to them in the position embedding and
+    in layer 0's fc2 bias, so every LayerNorm sees a few residual channels with a large constant offset."""
+    sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+    branch_gain = (2.0 * cfg.num_hidden_layers) ** -0.5
+    for name, shape in clip_text_param_shapes(cfg).items():
+        g = _gen(seed, "clip_text." + name)
+        if name.endswith("token_embedding.weight"):
+            t = torch.randn(shape, generator=g)
+        elif name.endswith("position_embedding.weight"):
+            t = torch.randn(shape, generator=g) * 0.5
+        elif len(shape) == 1:
+            t = torch.randn(shape, generator=g) * (0.1 if name.endswith(".weight") else 0.02)
+            if name.endswith(".weight"):
+                t = t + 1.0
+        else:
+            gain = branch_gain if name.endswith(("out_proj.weight", "fc2.weight")) else 1.0
+            t = torch.randn(shape, generator=g) * (gain / shape[1] ** 0.5)
+        sd[name] = t
+    if outlier_channels > 0:
+        ch = torch.randperm(cfg.hidden_size, generator=_gen(seed, "clip_text.outliers"))[:outlier_channels]
+        sd["text_model.embeddings.position_embedding.weight"][:, ch] += outlier_offset
+        sd["text_model.encoder.layers.0.mlp.fc2.bias"][ch] += outlier_offset
+    return OrderedDict((k, v.to(dtype)) for k, v in sd.items())
+
+
+def make_input_ids(n: int, L: int, cfg: ClipTextConfig, seed: int = 4747, lengths=None) -> torch.Tensor:
+    """Tokenizer-like `input_ids` [n, L] int64, as `pad_tokens_and_weights` (musev/utils/text_emb_util.py:153-175) builds
+    them with SD-1.5's tokenizer: bos, `lengths[i]` content ids, then eos up to the end (SD-1.5's pad token is its eos).
+    With the legacy `eos_token_id == 2` the tokenizer's ids are used (bos = vocab - 2, eos = vocab - 1, content below them);
+    otherwise bos / eos are the config's and content ids lie above both, so argmax and the eos rule pick different rows.
+    `lengths` defaults to seeded values in [0, L - 2]."""
+    g = torch.Generator().manual_seed(seed)
+    V = cfg.vocab_size
+    if cfg.eos_token_id == 2:
+        bos, eos, lo, hi = V - 2, V - 1, 0, V - 2
+    else:
+        bos, eos = cfg.bos_token_id, cfg.eos_token_id
+        lo, hi = max(bos, eos) + 1, V
+    if lengths is None:
+        lengths = torch.randint(0, max(1, L - 1), (n,), generator=g).tolist()
+    ids = torch.full((n, L), eos, dtype=torch.int64)
+    for i, k in enumerate(lengths):
+        k = max(0, min(int(k), L - 2))
+        ids[i, 0] = bos
+        ids[i, 1:1 + k] = torch.randint(lo, hi, (k,), generator=g)
+    return ids

@@ -217,24 +217,6 @@ class UNet3DConditionModel(EngineModel):
     __call__ = forward
 
     # ------------------------------------------------------------------ LoRA (musev_b200/lora.py is the public surface)
-    def _merge_lora(self, targets: Sequence[str], ups: Sequence[torch.Tensor], downs: Sequence[torch.Tensor],
-                    scales: Sequence[float], subtract: bool = False) -> None:
-        """W16 = fp16(W16 +- fp16(scale * (up @ down))) for every target (reference weight names), one `mvb_unet_merge_lora`
-        call. The factors must be contiguous fp16 / fp32 tensors on this model's device."""
-        n = len(targets)
-        if not (len(ups) == len(downs) == len(scales) == n):
-            raise ValueError("targets, ups, downs and scales differ in length")
-        for t in list(ups) + list(downs):
-            if t.device != self.device or not t.is_contiguous():
-                raise ValueError(f"LoRA factors must be contiguous tensors on {self.device}")
-        up_arr = (MvbNamedTensor * max(n, 1))(*[_named(nm, u) for nm, u in zip(targets, ups)])
-        down_arr = (MvbNamedTensor * max(n, 1))(*[_named(nm, d) for nm, d in zip(targets, downs)])
-        sc = (C.c_float * max(n, 1))(*[float(s) for s in scales])
-        torch.cuda.current_stream(self.device).synchronize()      # the factors may still be in flight
-        rc = lib().mvb_unet_merge_lora(self._h, up_arr, down_arr, sc, n, int(bool(subtract)))
-        if rc != 0:
-            raise MvbError(f"mvb_unet_merge_lora ({rc}): {self._error()}")
-
     # ------------------------------------------------------------------ debug
     def debug_taps(self) -> Dict[str, torch.Tensor]:
         """Layer outputs of the last forward as [(b t), C, h*w]-ordered channels-last copies (fp32, [rows, C])."""

@@ -8,8 +8,9 @@ two such output directories, every output that differs, every launch count that 
   python tools/gpu_compare_builds.py --compare /tmp/old /tmp/new
 
 The calls: the UNet (both presets, narrow and full width, with ControlNet residuals, reference embeddings and
-`pose_guider_emb`), the ControlNet, the ReferenceNet, VAE decode and encode, the PoseGuider (both configurations) and a
-LoRA merge, forward and unload on the UNet."""
+`pose_guider_emb`), the ControlNet, the ReferenceNet, VAE decode and encode, the PoseGuider (both configurations), a
+LoRA merge, forward and unload on the UNet, the CLIP vision tower (two narrow configurations and ViT-H/14) and, with a
+library that has it, the CLIP text encoder (two narrow configurations and SD-1.5)."""
 import argparse
 import json
 import os
@@ -156,13 +157,73 @@ def _lora_calls(rec):
         lambda: (model._merge_lora(targets, ups, downs, scales, subtract=True), [model.debug_weight(n) for n in probe])[1])
 
 
+def _clip_vision_calls(rec):
+    from musev_b200.clip_vision import CLIPVisionModelWithProjection
+    from musev_b200.schema import ClipVisionConfig
+    from musev_b200.synth import make_clip_pixel_values, make_clip_vision_state_dict
+    for tag, cfg, n in (("d64", ClipVisionConfig(hidden_size=128, intermediate_size=512, num_hidden_layers=2, num_attention_heads=2,
+                                                 image_size=56, patch_size=14, projection_dim=64), 3),
+                        ("d40", ClipVisionConfig(hidden_size=320, intermediate_size=640, num_hidden_layers=2, num_attention_heads=8,
+                                                 image_size=56, patch_size=14, projection_dim=64, hidden_act="quick_gelu"), 2),
+                        ("vit_h14", ClipVisionConfig(), 2)):
+        sd = {k: v.half() for k, v in make_clip_vision_state_dict(cfg, seed=6).items()}
+        m = CLIPVisionModelWithProjection.from_state_dict(sd, cfg, device=dev, dtype=torch.float16)
+        x = make_clip_pixel_values(n, cfg.image_size, seed=6).to(dev)
+        rec(f"clip_vision_{tag}", m, lambda: m(x).to_tuple())
+
+
+def _clip_text_calls(rec):
+    from musev_b200.clip_text import CLIPTextModel
+    from musev_b200.schema import ClipTextConfig
+    from musev_b200.synth import make_clip_text_state_dict, make_input_ids
+    for tag, cfg, n, L in (("d64", ClipTextConfig(vocab_size=1000, hidden_size=128, intermediate_size=512, num_hidden_layers=2,
+                                                  num_attention_heads=2), 3, 77),
+                           ("d40", ClipTextConfig(vocab_size=1000, hidden_size=320, intermediate_size=640, num_hidden_layers=2,
+                                                  num_attention_heads=8, max_position_embeddings=160, hidden_act="gelu",
+                                                  bos_token_id=6, eos_token_id=7), 2, 150),
+                           ("sd15", ClipTextConfig(), 6, 77)):
+        sd = {k: v.half() for k, v in make_clip_text_state_dict(cfg, seed=6).items()}
+        m = CLIPTextModel.from_state_dict(sd, cfg, device=dev, dtype=torch.float16)
+        ids = make_input_ids(n, L, cfg, seed=6).to(dev)
+        rec(f"clip_text_{tag}", m, lambda: m(ids).to_tuple())
+
+
+class _Missing:
+    def __init__(self, name):
+        self.name = name
+
+    def __call__(self, *args):
+        raise AttributeError(f"{self.name} is not exported by this library")
+
+
+class _TolerantLib:
+    """A library handle on which entry points a build does not export can still be declared (they raise when called), so
+    that an older library runs the calls it has."""
+
+    def __init__(self, path):
+        import ctypes
+        self._l = ctypes.CDLL(path)
+
+    def __getattr__(self, name):
+        try:
+            return getattr(self._l, name)
+        except AttributeError:
+            setattr(self, name, _Missing(name))
+            return getattr(self, name)
+
+
 def run(lib_path: str, out_dir: str) -> None:
     from musev_b200 import _capi
     _capi.LIB_PATH = os.path.abspath(lib_path)
-    _capi.lib()
+    tl = _TolerantLib(_capi.LIB_PATH)
+    _capi._declare(tl)
+    _capi._lib = tl
     rec = Recorder()
-    for calls in (_unet_calls, _encoder_calls, _vae_calls, _pose_guider_calls, _lora_calls):
-        calls(rec)
+    calls = [_unet_calls, _encoder_calls, _vae_calls, _pose_guider_calls, _lora_calls, _clip_vision_calls]
+    if hasattr(tl._l, "mvb_create_clip_text"):      # libraries before mvb_version 4 have no CLIP text handle
+        calls.append(_clip_text_calls)
+    for c in calls:
+        c(rec)
     os.makedirs(out_dir, exist_ok=True)
     torch.save(rec.results, os.path.join(out_dir, "results.pt"))
 

@@ -102,10 +102,9 @@ int mvb_op_attention(const mvb_attention_desc* desc, void* stream);
  * any other layout is rejected before a launch (MVB_ERR_CUDA with "causal" in mvb_last_error()). */
 int mvb_op_attention_causal(const mvb_attention_desc* desc, void* stream);
 /* Measurement aid (no reference equivalent): while `device_buffer` (>= 9*32*8 int64 on the device) is set, CTA (0,0,0) of every
- * ping-pong attention launch (head dim <= 64) writes the SM clock at each phase of its first 32 key/value tiles:
- * [role][tile][slot], role 4t+q = softmax warp of query tile t, lane quarter q (slots: 0 wait S, 1 S ready, 2 scores in registers, 3 row max,
- * 4 exponentials done, 5 previous P.V complete, 6 P published), role 8 = the MMA-issuing warp (per query tile t, slots 4t..4t+3:
- * S_t(j) freed, S_t(j+1) issued, P_t(j) ready, P_t(j)V(j) issued). NULL switches it off. tools/gpu_attention_trace.py. */
+ * attention launch writes the SM clock at each phase of its first 32 key/value tiles: [role][tile][8 slots], role 0 = the TMA
+ * producer (slots: 0 K tile issued, 1 V tile issued), role 1 + w = consumer warpgroup w, w < 3 for non-causal head dims <= 64
+ * and w < 2 otherwise (slots: 0 S in registers, 1 softmax done, 2 P.V complete). NULL switches it off. */
 int mvb_debug_attention_trace(long long* device_buffer);
 /* Encoded TMA descriptors (cuTensorMapEncodeTiled: 2-6 per GEMM / convolution, 5 per attention call) are memoized process-wide by
  * (address, extents, strides, box, swizzle); the engine's workspace arena reproduces its addresses on every forward of the same

@@ -1,15 +1,19 @@
-// wgmma flash attention (see attention.cuh). One kernel, templated on the padded head dim dp (the N of the P.V MMA) and on
-// the causal mask (CLIP text self attention: key tiles past the diagonal are skipped, the diagonal tile is masked).
+// wgmma flash attention (see attention.cuh). One kernel, templated on the padded head dim dp (the N of the P.V MMA), on
+// the causal mask (CLIP text self attention: key tiles past the diagonal are skipped, the diagonal tile is masked) and on
+// the number NWG of consumer warpgroups (attn_warpgroups: 3 for non-causal dp <= 64, else 2).
 //
-// CTA = 384 threads = 3 warpgroups = 128 queries of one (frame, head):
-//   warpgroup 0, warp 0 : TMA producer -- Q once, then K and V tiles of 128 keys through their own smem rings (boxes of
-//                         128 rows x 64 fp16, 128-byte swizzle); warp-uniform loop, elect.sync picks the issuing lane.
-//                         The warpgroup gives its registers to the other two (setmaxnreg).
-//   warpgroups 1, 2     : 64 query rows each. Per key tile: S = Q K^T (wgmma m64n128k16, both operands in smem) into
+// CTA = 128 (NWG + 1) threads = NWG + 1 warpgroups = 64 NWG queries of one (frame, head):
+//   warpgroup 0, warp 0 : TMA producer -- Q once (boxes of 64 NWG rows x 64 fp16), then K and V tiles of 128 keys through
+//                         their own smem rings (boxes of 128 rows x 64 fp16), all with the 128-byte swizzle;
+//                         warp-uniform loop, elect.sync picks the issuing lane. The warpgroup gives its registers to the
+//                         consumers (setmaxnreg).
+//   warpgroups 1..NWG   : 64 query rows each. Per key tile: S = Q K^T (wgmma m64n128k16, both operands in smem) into
 //                         registers; masked online softmax (row max / sum over the four lanes that share a row); P is
 //                         rounded to fp16 in registers and fed straight back as the A operand of O += P V (wgmma
 //                         m64n{dp}k16, V read MN-major from its row-major tile); O stays in registers until the end.
-// The two consumer warpgroups run independently, so one's softmax overlaps the other's MMAs.
+// The consumer warpgroups run independently, so one's softmax overlaps the others' MMAs, and every K / V tile brought
+// into shared memory serves all of them. A query row lands on the same lane and register of its warpgroup for either
+// NWG (64 divides both tile heights), so the warpgroup count does not change any output bit.
 #include "attention.cuh"
 
 #include <cuda.h>
@@ -35,7 +39,7 @@ struct AttnParams {
   long long ldo;
   int accumulate;
   long long* trace;   // measurement aid (mvb_debug_attention_trace): CTA (0,0,0) writes clock64 stamps of its phases
-                      // here, [role 0..2][KV tile j < 32][8 slots]; null in normal runs
+                      // here, [role 0..NWG][KV tile j < 32][8 slots]; null in normal runs
 };
 
 // clock64 stamp of one phase (only the traced CTA's reporting threads get a non-null pointer)
@@ -45,6 +49,11 @@ __device__ __forceinline__ void att_stamp(long long* tr, int j, int slot) {
 
 static constexpr int kAtomBytes = 128 * 128;  // 128 rows x 64 fp16
 static constexpr int kMaxRing = 4;
+
+// Consumer warpgroups per CTA. Three share each K / V tile when 128 registers a thread (65 536 / 512 threads) hold a
+// consumer's state without spilling: dp <= 64 (S 64 + P 32 + O dp / 2 fp32 / packed registers). The causal variant
+// stays at two: kv_tile_count<true> and the diagonal mask take query tiles and key tiles to be the same 128 rows.
+__host__ __device__ constexpr int attn_warpgroups(int dp, bool causal) { return (!causal && dp <= 64) ? 3 : 2; }
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -77,17 +86,23 @@ __device__ __forceinline__ int kv_tile_count(const AttnParams& p) {
   return CAUSAL ? min(n, (int)blockIdx.x + 1) : n;
 }
 
-template <int DP, bool CAUSAL>
-__global__ void __launch_bounds__(384, 1)
+template <int DP, bool CAUSAL, int NWG>
+__global__ void __launch_bounds__(128 * (NWG + 1), 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
                  const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
                  const __grid_constant__ CUtensorMap tmV1, const __grid_constant__ AttnParams p) {
+  static_assert(NWG == attn_warpgroups(DP, CAUSAL), "warpgroup count and instantiation disagree");
   constexpr int kAtoms = (DP + 63) / 64;
   constexpr int kTileBytes = kAtoms * kAtomBytes;
+  constexpr int kQRows = 64 * NWG;
+  constexpr int kQAtomBytes = kQRows * 128;          // kQRows rows x 64 fp16
+  // the producer warpgroup's registers go to the consumers; together they fit the SM's 65 536
+  constexpr int kProducerRegs = NWG == 2 ? 40 : 24, kConsumerRegs = NWG == 2 ? 232 : 160;
+  static_assert(128 * kProducerRegs + 128 * NWG * kConsumerRegs <= 65536, "setmaxnreg split exceeds the register file");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
-  uint8_t* sK = sQ + kTileBytes;
+  uint8_t* sK = sQ + kAtoms * kQAtomBytes;
   uint8_t* sV = sK + p.sk * kTileBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + p.sv * kTileBytes);
   uint64_t* bar_q = bars;                      // 1
@@ -97,7 +112,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   uint64_t* empty_v = full_v + kMaxRing;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 128;
+  const int q0 = blockIdx.x * kQRows;
   const int h = blockIdx.y;
   const int f = blockIdx.z;
   const int ntiles = kv_tile_count<CAUSAL>(p);
@@ -107,21 +122,21 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
     mbar_init(bar_q, 1);
     for (int s = 0; s < kMaxRing; ++s) {
-      mbar_init(&full_k[s], 1); mbar_init(&empty_k[s], 8);   // one arrival per consumer warp
-      mbar_init(&full_v[s], 1); mbar_init(&empty_v[s], 8);
+      mbar_init(&full_k[s], 1); mbar_init(&empty_k[s], 4 * NWG);   // one arrival per consumer warp
+      mbar_init(&full_v[s], 1); mbar_init(&empty_v[s], 4 * NWG);
     }
     fence_barrier_init();
   }
   __syncthreads();
 
   if (warp < 4) {
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<kProducerRegs>();
     if (warp == 0) {
       long long* tr = (traced && lane == 0) ? p.trace : nullptr;
       if (elect_one()) {
-        mbar_expect_tx(bar_q, (uint32_t)kTileBytes);
+        mbar_expect_tx(bar_q, (uint32_t)(kAtoms * kQAtomBytes));
         for (int a = 0; a < kAtoms; ++a)
-          tma_load_2d(sQ + a * kAtomBytes, &tmQ, bar_q, h * p.dp + a * 64, f * p.Nq + q0);
+          tma_load_2d(sQ + a * kQAtomBytes, &tmQ, bar_q, h * p.dp + a * 64, f * p.Nq + q0);
       }
       __syncwarp();
       for (int j = 0; j < ntiles; ++j) {
@@ -152,7 +167,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     return;
   }
 
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<kConsumerRegs>();
   const int wg = (warp - 4) >> 2;                  // query rows [64 wg, 64 wg + 64) of the tile
   const int wq = warp & 3;
   long long* tr = (traced && (threadIdx.x & 127) == 0) ? p.trace + (1 + wg) * 32 * 8 : nullptr;
@@ -177,8 +192,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < DP / 16; ++kk) {
-      const uint32_t off = (uint32_t)(kk >> 2) * kAtomBytes + (uint32_t)(kk & 3) * 32;
-      Wgmma<128>::ss(s, make_desc_k_sw128(aQ + off), make_desc_k_sw128(aK + off), kk != 0);
+      const uint32_t offq = (uint32_t)(kk >> 2) * kQAtomBytes + (uint32_t)(kk & 3) * 32;
+      const uint32_t offk = (uint32_t)(kk >> 2) * kAtomBytes + (uint32_t)(kk & 3) * 32;
+      Wgmma<128>::ss(s, make_desc_k_sw128(aQ + offq), make_desc_k_sw128(aK + offk), kk != 0);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -299,13 +315,15 @@ void set_attention_trace(long long* device_buffer) { g_attention_trace = device_
 typedef void (*AttnKernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                              const AttnParams);
 // instantiations for every padded head dim the launcher accepts (multiples of 16 up to 192), without and with the causal mask
+#define MVB_ATTN(dp, causal) attention_kernel<dp, causal, attn_warpgroups(dp, causal)>
 static const AttnKernelFn kAttnKernels[2][12] = {
-    {attention_kernel<16, false>,  attention_kernel<32, false>,  attention_kernel<48, false>,  attention_kernel<64, false>,
-     attention_kernel<80, false>,  attention_kernel<96, false>,  attention_kernel<112, false>, attention_kernel<128, false>,
-     attention_kernel<144, false>, attention_kernel<160, false>, attention_kernel<176, false>, attention_kernel<192, false>},
-    {attention_kernel<16, true>,  attention_kernel<32, true>,  attention_kernel<48, true>,  attention_kernel<64, true>,
-     attention_kernel<80, true>,  attention_kernel<96, true>,  attention_kernel<112, true>, attention_kernel<128, true>,
-     attention_kernel<144, true>, attention_kernel<160, true>, attention_kernel<176, true>, attention_kernel<192, true>}};
+    {MVB_ATTN(16, false),  MVB_ATTN(32, false),  MVB_ATTN(48, false),  MVB_ATTN(64, false),
+     MVB_ATTN(80, false),  MVB_ATTN(96, false),  MVB_ATTN(112, false), MVB_ATTN(128, false),
+     MVB_ATTN(144, false), MVB_ATTN(160, false), MVB_ATTN(176, false), MVB_ATTN(192, false)},
+    {MVB_ATTN(16, true),  MVB_ATTN(32, true),  MVB_ATTN(48, true),  MVB_ATTN(64, true),
+     MVB_ATTN(80, true),  MVB_ATTN(96, true),  MVB_ATTN(112, true), MVB_ATTN(128, true),
+     MVB_ATTN(144, true), MVB_ATTN(160, true), MVB_ATTN(176, true), MVB_ATTN(192, true)}};
+#undef MVB_ATTN
 
 cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char** err) {
   if (a.d % 8 || a.dp % 16 || a.dp < a.d || a.dp > 192 || a.nseg < 1 || a.nseg > 2 || a.heads < 1) {
@@ -334,12 +352,15 @@ cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char*
   }
   p.out = a.out; p.ldo = a.ldo; p.accumulate = a.accumulate;
   p.trace = g_attention_trace;
-  // ring depths: Q + sk K tiles + sv V tiles within the 227 KB of shared memory a block may use
+  const int causal = a.causal ? 1 : 0;
+  const int nwg = attn_warpgroups(a.dp, a.causal != 0);
+  const int q_rows = 64 * nwg;   // query rows per CTA
+  // ring depths: Q + sk K tiles + sv V tiles within the 227 KB of shared memory a block may use (three warpgroups only
+  // at natoms == 1: 24 KB of Q + 128 KB of ring)
   if (p.natoms == 1) { p.sk = 4; p.sv = 4; }
   else if (p.natoms == 2) { p.sk = 2; p.sv = 2; }
   else { p.sk = 2; p.sv = 1; }
-  const int smem = (1 + p.sk + p.sv) * p.natoms * kAtomBytes + 1024 + 128 + 256;
-  const int causal = a.causal ? 1 : 0;
+  const int smem = p.natoms * q_rows * 128 + (p.sk + p.sv) * p.natoms * kAtomBytes + 1024 + 128 + 256;
   const AttnKernelFn kernel = kAttnKernels[causal][a.dp / 16 - 1];
   static int max_set_dev[64][2][12] = {};  // per device (the attribute belongs to the device's context)
   int cur_dev = 0;
@@ -352,7 +373,7 @@ cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char*
   }
   CUtensorMap tq, tk0, tv0, tk1, tv1;
   const uint64_t cols = (uint64_t)a.heads * a.dp;
-  if (!encode_map_2d(&tq, a.q, cols, (uint64_t)a.NF * a.Nq, (uint64_t)a.ldq, 64, 128)) {
+  if (!encode_map_2d(&tq, a.q, cols, (uint64_t)a.NF * a.Nq, (uint64_t)a.ldq, 64, (uint32_t)q_rows)) {
     *err = "cuTensorMapEncodeTiled(Q) failed"; return cudaErrorInvalidValue;
   }
   const AttnSegment& s0 = a.seg[0];
@@ -367,9 +388,9 @@ cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char*
   if (trace)
     fprintf(stderr, "MVB_TRACE attn NF=%d Nq=%d heads=%d d=%d nk0=%d nk1=%d acc=%d causal=%d\n", a.NF, a.Nq, a.heads, a.d,
             p.nk[0], p.nk[1], a.accumulate, causal);
-  dim3 grid((a.Nq + 127) / 128, a.heads, a.NF);
+  dim3 grid((a.Nq + q_rows - 1) / q_rows, a.heads, a.NF);
   ProfScope prof(stream, KC_ATTENTION);
-  kernel<<<grid, 384, smem, stream>>>(tq, tk0, tv0, tk1, tv1, p);
+  kernel<<<grid, 128 * (nwg + 1), smem, stream>>>(tq, tk0, tv0, tk1, tv1, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) *err = "attention_kernel launch";
   return e;

@@ -40,7 +40,8 @@ struct AttnArgs {
 };
 
 cudaError_t launch_attention(cudaStream_t stream, const AttnArgs& a, const char** err);
-// measurement aid: CTA (0,0,0) of the following ping-pong launches writes 10 x 32 x 8 clock64 stamps to device_buffer (null = off)
+// measurement aid: CTA (0,0,0) of the following launches writes (1 + warpgroups) x 32 x 8 clock64 stamps to device_buffer
+// (null = off; layout in include/musev_b200.h)
 void set_attention_trace(long long* device_buffer);
 
 }  // namespace mvb

@@ -694,24 +694,32 @@ struct Engine::Fwd {
   Arena* ar;
   cudaStream_t s;
   bool dry;
-  const mvb_unet_args* a;
   int B, T, H, W, NF;
   int heads;
   float* gn_part = nullptr;            // GroupNorm partial sums scratch
   const float* temb_table = nullptr;   // [NF, temb_total] fp32
   const float* femb_table = nullptr;   // [NF, femb_total] fp32
-  const __half* enc = nullptr;         // [B*n_text, X] fp16
-  const __half* clip = nullptr;        // [B*n_clip, X] fp16 or null
+  // What spatial() and refer_tokens() condition on. run_unet sets all of it, run_controlnet the text part; the other kinds
+  // run neither layer and leave it empty.
+  struct Cond {
+    const __half* enc = nullptr;       // text tokens [B*n_text, X] fp16
+    int n_text = 0;
+    const __half* clip = nullptr;      // IP-Adapter image tokens [B*n_clip, X] fp16, or null
+    int n_clip = 0;
+    float ip_adapter_scale = 0.f;
+    int n_vis_cond = 0, vis_cond_first = 0;   // frames every frame's self attention also attends to
+    int refer_is_f32 = 0;              // dtype of the reference feature maps
+  } cond;
   bool skip_temporal;
   bool ok = true;
 
-  // `args` (B, T, H, W and what the layers read) must outlive the Fwd. Clears the taps of a real call and takes the
-  // GroupNorm scratch as the first allocation of the arena.
-  Fwd(Engine* e, Arena& arena, cudaStream_t st, const mvb_unet_args& args, bool skip_temporal_layers)
-      : E(e), ar(&arena), s(st), dry(arena.dry), a(&args), B(args.B), T(args.T), H(args.H), W(args.W), NF(args.B * args.T),
-        heads(e->heads_), skip_temporal(skip_temporal_layers) {
+  // Clears the taps of a real call. A kind that runs GroupNorm (`groupnorm`) takes its scratch as the first allocation of
+  // the arena.
+  Fwd(Engine* e, Arena& arena, cudaStream_t st, int B_, int T_, int H_, int W_, bool skip_temporal_layers, bool groupnorm)
+      : E(e), ar(&arena), s(st), dry(arena.dry), B(B_), T(T_), H(H_), W(W_), NF(B_ * T_), heads(e->heads_),
+        skip_temporal(skip_temporal_layers) {
     if (!dry) E->taps_.clear();
-    gn_part = alloc_f((long long)NF * (kGnMaxChunks + 1) * E->cfg_.norm_num_groups * 2);
+    if (groupnorm) gn_part = alloc_f((long long)NF * (kGnMaxChunks + 1) * E->cfg_.norm_num_groups * 2);
   }
 
   bool fail(const char* what, cudaError_t e) {
@@ -775,6 +783,7 @@ struct Engine::Fwd {
   }
   void gn(const __half* x0, int C0, const __half* x1, int C1, int HW, int fps, float eps, const Norm& n, int silu,
           __half* y) {
+    if (!gn_part) { fail("groupnorm: the forward reserved no scratch", cudaSuccess); return; }
     if (!ok || dry) return;
     if (E->gn_fused_) {
       cudaError_t e = gn_fused(s, x0, C0, x1, C1, NF, HW, E->cfg_.norm_num_groups, gn_part, fps, eps, n.g, n.b, silu, y,
@@ -801,6 +810,20 @@ struct Engine::Fwd {
   }
 
   // ---- stages shared by the model kinds
+  // TimestepEmbedding (diffusers models/embeddings.py) of n device values: sinusoid -> linear_1 + SiLU -> linear_2 with
+  // activation act2; returns the linear_2 output [n, l2.N]
+  __half* embed_mlp(const float* vals, int n, const Mat& l1, const Mat& l2, int act2) {
+    __half* sn = alloc_h(n, l1.K);
+    __half* h1 = alloc_h(n, l1.N);
+    __half* h2 = alloc_h(n, l2.N);
+    if (!dry && ok) {
+      cudaError_t e = sinusoid(s, vals, n, l1.K, sn, l1.K);
+      if (e != cudaSuccess) fail("sinusoid", e);
+    }
+    { Epilogue ep; ep.out = h1; ep.ldc = l1.N; ep.act = 1; gemm(sn, n, l1.K, l1, ep); }
+    { Epilogue ep; ep.out = h2; ep.ldc = l2.N; ep.act = act2; gemm(h1, n, l1.N, l2, ep); }
+    return h2;
+  }
   // CLIPEncoderLayer.forward (modeling_clip.py:363-386) for every layer, in place on the fp16 residual stream x [M = NFs Ts, C]:
   // LN1, fused q / k / v (+ bias), softmax(q k^T d^-0.5) v per head over the Ts tokens of one sequence (causal: key k <= query
   // q only, the text encoder's mask), out_proj + residual, LN2, fc1 + activation, fc2 + residual. Shared by both CLIP kinds.
@@ -979,10 +1002,10 @@ struct Engine::Fwd {
       aa.scale = 1.f / sqrtf((float)d);
       aa.nseg = 1;
       aa.seg[0] = AttnSegment{qkv + hd, qkv + 2 * hd, 3 * hd, M, HW, 1, HW, 0};
-      if (E->cfg_.need_t2i_ip_adapter && a->n_vis_cond > 0 && T > 1) {
+      if (E->cfg_.need_t2i_ip_adapter && cond.n_vis_cond > 0 && T > 1) {
         aa.nseg = 2;
-        aa.seg[1] = AttnSegment{qkv + hd, qkv + 2 * hd, 3 * hd, M, a->n_vis_cond * HW, T, (long long)T * HW,
-                                (long long)a->vis_cond_first * HW};
+        aa.seg[1] = AttnSegment{qkv + hd, qkv + 2 * hd, 3 * hd, M, cond.n_vis_cond * HW, T, (long long)T * HW,
+                                (long long)cond.vis_cond_first * HW};
       }
       aa.out = ao; aa.ldo = C; aa.out_scale = 1.f;
       attn(aa);
@@ -997,24 +1020,24 @@ struct Engine::Fwd {
       __half* q = alloc_h(M, hd);
       { Epilogue ep; ep.out = q; ep.ldc = hd; gemm(nbuf, M, C, b.q2, ep, false); }
       const int X = E->cfg_.cross_attention_dim;
-      const long long Mt = (long long)B * a->n_text;
+      const long long Mt = (long long)B * cond.n_text;
       __half* kv = alloc_h(Mt, 2 * hd);
-      { Epilogue ep; ep.out = kv; ep.ldc = 2 * hd; gemm(enc, Mt, X, b.kv2, ep, b.kv2.bias != nullptr); }
+      { Epilogue ep; ep.out = kv; ep.ldc = 2 * hd; gemm(cond.enc, Mt, X, b.kv2, ep, b.kv2.bias != nullptr); }
       __half* ao = alloc_h(M, C);
       AttnArgs aa{};
       aa.v_ones_col = b.kv2.bias != nullptr;
       aa.q = q; aa.ldq = hd; aa.NF = NF; aa.Nq = HW; aa.heads = Hh; aa.d = d; aa.dp = dp;
       aa.scale = 1.f / sqrtf((float)d);
       aa.nseg = 1;
-      aa.seg[0] = AttnSegment{kv, kv + hd, 2 * hd, Mt, a->n_text, T, a->n_text, 0};
+      aa.seg[0] = AttnSegment{kv, kv + hd, 2 * hd, Mt, cond.n_text, T, cond.n_text, 0};
       aa.out = ao; aa.ldo = C; aa.out_scale = 1.f;
       attn(aa);
-      if (b.has_ip && clip && a->ip_adapter_scale > 0.f) {
-        const long long Mc = (long long)B * a->n_clip;
+      if (b.has_ip && cond.clip && cond.ip_adapter_scale > 0.f) {
+        const long long Mc = (long long)B * cond.n_clip;
         __half* kvi = alloc_h(Mc, 2 * hd);
-        { Epilogue ep; ep.out = kvi; ep.ldc = 2 * hd; gemm(clip, Mc, X, b.kv2_ip, ep, b.kv2_ip.bias != nullptr); }
-        aa.seg[0] = AttnSegment{kvi, kvi + hd, 2 * hd, Mc, a->n_clip, T, a->n_clip, 0};
-        aa.out_scale = a->ip_adapter_scale; aa.accumulate = 1;
+        { Epilogue ep; ep.out = kvi; ep.ldc = 2 * hd; gemm(cond.clip, Mc, X, b.kv2_ip, ep, b.kv2_ip.bias != nullptr); }
+        aa.seg[0] = AttnSegment{kvi, kvi + hd, 2 * hd, Mc, cond.n_clip, T, cond.n_clip, 0};
+        aa.out_scale = cond.ip_adapter_scale; aa.accumulate = 1;
         attn(aa);
       }
       Epilogue ep; ep.out = h; ep.ldc = C; ep.res = h; ep.ld_res = C;
@@ -1098,7 +1121,7 @@ struct Engine::Fwd {
   __half* refer_tokens(const void* map, int C, int t, int h, int w) {
     __half* tok = alloc_h((long long)B * t * h * w, C);
     if (ok && !dry) {
-      cudaError_t e = ncthw_to_tokens(s, map, a->refer_is_f32, B, C, t, h * w, tok, C, 1.f);
+      cudaError_t e = ncthw_to_tokens(s, map, cond.refer_is_f32, B, C, t, h * w, tok, C, 1.f);
       if (e != cudaSuccess) fail("refer tokens", e);
     }
     return tok;
@@ -1163,7 +1186,7 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
     for (int i = 0; i < nb; ++i) expect += c.layers_per_block + (i == nb - 1 ? 0 : 1);
     if (a.n_refer != expect) { err_ = "down_block_refer_embs: wrong number of maps"; return false; }
   }
-  Fwd f(this, ar, s, a, a.skip_temporal_layers != 0);
+  Fwd f(this, ar, s, B, T, a.H, a.W, a.skip_temporal_layers != 0, true);
 
   // ---- embeddings (unet_3d_condition.py:887-937)
   __half* temb_rows = f.alloc_h(NF, temb);
@@ -1173,12 +1196,6 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
   f.temb_table = temb_table; f.femb_table = femb_table;
   {
     const size_t mk = f.mark();
-    __half* sin_t = f.alloc_h(B, c0);
-    __half* e1 = f.alloc_h(B, temb);
-    __half* e2 = f.alloc_h(B, temb);
-    __half* sin_f = f.alloc_h(T, c0);
-    __half* f1 = f.alloc_h(T, temb);
-    __half* f2 = f.alloc_h(T, temb);
     if (!ar.dry) {
       float vals[128];
       for (int i = 0; i < B && i < 64; ++i) vals[i] = a.timestep;
@@ -1191,13 +1208,9 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
       for (int i = 0; i < a.n_vis_cond && i < 64; ++i) zidx[i] = a.vis_cond_first + i;
       cudaMemcpyAsync(fidx_dev_, vals, sizeof(float) * 128, cudaMemcpyHostToDevice, s);
       cudaMemcpyAsync(zero_idx_dev_, zidx, sizeof(int) * 64, cudaMemcpyHostToDevice, s);
-      if (sinusoid(s, fidx_dev_, B, c0, sin_t, c0) != cudaSuccess) f.fail("sinusoid", cudaGetLastError());
-      if (sinusoid(s, fidx_dev_ + 64, T, c0, sin_f, c0) != cudaSuccess) f.fail("sinusoid", cudaGetLastError());
     }
-    { Epilogue ep; ep.out = e1; ep.ldc = temb; ep.act = 1; f.gemm(sin_t, B, c0, time_l1_, ep); }
-    { Epilogue ep; ep.out = e2; ep.ldc = temb; ep.act = c.use_anivv1_cfg ? 1 : 0; f.gemm(e1, B, temb, time_l2_, ep); }
-    { Epilogue ep; ep.out = f1; ep.ldc = temb; ep.act = 1; f.gemm(sin_f, T, c0, frame_l1_, ep); }
-    { Epilogue ep; ep.out = f2; ep.ldc = temb; ep.act = c.use_anivv1_cfg ? 1 : 0; f.gemm(f1, T, temb, frame_l2_, ep); }
+    const __half* e2 = f.embed_mlp(fidx_dev_, B, time_l1_, time_l2_, c.use_anivv1_cfg ? 1 : 0);
+    const __half* f2 = f.embed_mlp(fidx_dev_ + 64, T, frame_l1_, frame_l2_, c.use_anivv1_cfg ? 1 : 0);
     if (!ar.dry && f.ok) {
       const bool zero_vc = c.keep_vision_condtion && T > 1 && a.has_sample_index && a.n_vis_cond > 0;
       // rows of time_emb_proj input: [silu](emb) per frame, vision-condition frames zeroed (Q7)
@@ -1230,7 +1243,9 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
       if (e != cudaSuccess) f.fail("vision_clip_emb convert", e);
     }
   }
-  f.enc = enc; f.clip = clip;
+  Fwd::Cond& cd = f.cond;
+  cd.enc = enc; cd.n_text = a.n_text; cd.clip = clip; cd.n_clip = a.n_clip; cd.ip_adapter_scale = a.ip_adapter_scale;
+  cd.n_vis_cond = a.n_vis_cond; cd.vis_cond_first = a.vis_cond_first; cd.refer_is_f32 = a.refer_is_f32;
 
   // ---- conv_in (unet_3d_condition.py:1008-1009)
   int Hc = a.H, Wc = a.W;
@@ -1370,25 +1385,18 @@ bool Engine::run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_
   // output layout [out_b, C, out_t, h, w] with NF = out_b * out_t; ControlNet: (b t) c h w, i.e. out_t = 1
   const int out_t = (refnet && a.out_frames > 0) ? a.out_frames : 1;
   if (NF % out_t) { err_ = "referencenet: num_frames must divide the batch"; return false; }
-  mvb_unet_args ua{};                     // what the shared layer functions read
-  ua.B = NF; ua.T = 1; ua.H = a.H; ua.W = a.W; ua.n_text = a.n_text; ua.n_vis_cond = 0; ua.ip_adapter_scale = 0.f;
-  Fwd f(this, ar, s, ua, true);           // every frame is its own batch element (own text rows)
+  Fwd f(this, ar, s, NF, 1, a.H, a.W, true, true);   // every frame is its own batch element (own text rows)
   // ---- time embedding (:733-741): one timestep for all frames; ResnetBlock2D applies SiLU before time_emb_proj
   float* temb_table = f.alloc_f((long long)NF * temb_total_);
   f.temb_table = temb_table;
   {
     const size_t mk = f.mark();
-    __half* sin_t = f.alloc_h(1, c0);
-    __half* e1 = f.alloc_h(1, temb);
-    __half* e2 = f.alloc_h(1, temb);
-    __half* temb_rows = f.alloc_h(NF, temb);
     if (!ar.dry) {
       float v = a.timestep;
       cudaMemcpyAsync(fidx_dev_, &v, sizeof(float), cudaMemcpyHostToDevice, s);
-      if (sinusoid(s, fidx_dev_, 1, c0, sin_t, c0) != cudaSuccess) f.fail("sinusoid", cudaGetLastError());
     }
-    { Epilogue ep; ep.out = e1; ep.ldc = temb; ep.act = 1; f.gemm(sin_t, 1, c0, time_l1_, ep); }
-    { Epilogue ep; ep.out = e2; ep.ldc = temb; f.gemm(e1, 1, temb, time_l2_, ep); }
+    const __half* e2 = f.embed_mlp(fidx_dev_, 1, time_l1_, time_l2_, 0);
+    __half* temb_rows = f.alloc_h(NF, temb);
     if (!ar.dry && f.ok) {
       cudaError_t e = expand_rows(s, e2, 1, NF, temb, zero_idx_dev_, 0, 1, temb_rows);
       if (e != cudaSuccess) f.fail("expand_rows(temb)", e);
@@ -1403,7 +1411,7 @@ bool Engine::run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_
     cudaError_t e = ncthw_to_tokens(s, a.encoder_hidden_states, a.ehs_is_f32, 1, 1, 1, NF * a.n_text * X, enc, 1, 1.f);
     if (e != cudaSuccess) f.fail("encoder_hidden_states convert", e);
   }
-  f.enc = enc;
+  f.cond.enc = enc; f.cond.n_text = a.n_text;
   // ---- conv_in + condition embedding (:780-785)
   int Hc = a.H, Wc = a.W;
   __half* x = f.alloc_h((long long)NF * Hc * Wc, c0);
@@ -1468,9 +1476,7 @@ bool Engine::run_vae(const mvb_vae_decode_args& a, Arena& ar, cudaStream_t s) {
   if (((long long)a.h * a.w) % 64 || (long long)a.h * a.w > 8192) {
     err_ = "vae: latent h*w must be a multiple of 64 and at most 8192 (mid-block attention runs as GEMMs over the tokens)"; return false;
   }
-  mvb_unet_args ua{};
-  ua.B = NF; ua.T = 1; ua.H = a.h; ua.W = a.w;
-  Fwd f(this, ar, s, ua, true);
+  Fwd f(this, ar, s, NF, 1, a.h, a.w, true, true);
   int Hc = a.h, Wc = a.w;
   const long long M0 = (long long)NF * Hc * Wc;
   // ---- post_quant_conv + conv_in (autoencoder_kl.py:283, vae.py:268)
@@ -1527,10 +1533,8 @@ bool Engine::run_vae_encode(const mvb_vae_decode_args& a, Arena& ar, cudaStream_
   const int nb = c.num_blocks, c0 = c.block_out_channels[0], cm = c.block_out_channels[nb - 1];
   const int NF = a.N, zc2 = 2 * c.out_channels, f = 1 << (nb - 1);
   if (const char* bad = vae_encode_shape_error(a)) { err_ = bad; return false; }
-  mvb_unet_args ua{};
-  ua.B = NF; ua.T = 1; ua.H = a.h * f; ua.W = a.w * f;
-  Fwd fw(this, ar, s, ua, true);
-  int Hc = ua.H, Wc = ua.W;
+  int Hc = a.h * f, Wc = a.w * f;
+  Fwd fw(this, ar, s, NF, 1, Hc, Wc, true, true);
   // ---- conv_in (vae.py:136): im2col of the C-channel image (9 C of 64 columns) + one GEMM
   __half* x = fw.alloc_h((long long)NF * Hc * Wc, c0);
   fw.conv_in(x, a.latents, a.latents_is_f32, c.in_channels, conv_in_, nullptr, 0, "vae encode input");
@@ -1580,25 +1584,23 @@ bool Engine::run_pose_guider(const mvb_vae_decode_args& a, Arena& ar, cudaStream
   const int nb = c.num_blocks, NF = a.N;
   if (const char* bad = pose_guider_shape_error(a, nb)) { err_ = bad; return false; }
   int Hc = a.h << (nb - 1), Wc = a.w << (nb - 1);
-  size_t most = 0;
+  Fwd f(this, ar, s, NF, 1, Hc, Wc, true, false);
+  long long most = 0;   // elements of the largest activation
   {
     int hh = Hc, ww = Wc;
     for (const CondConv& L : pg_) {
       hh /= L.stride; ww /= L.stride;
-      const size_t b = (size_t)NF * hh * ww * L.cout_p * sizeof(__half);
-      if (b > most) most = b;
+      most = std::max(most, (long long)NF * hh * ww * L.cout_p);
     }
   }
-  __half* buf[2] = {(__half*)ar.alloc(most), (__half*)ar.alloc(most)};
-  if (!buf[0] || !buf[1]) { err_ = "workspace too small"; return false; }
-  if (!ar.dry) taps_.clear();
+  __half* buf[2] = {f.alloc_h(most, 1), f.alloc_h(most, 1)};
   const void* x = a.latents;
-  int cur = 0;
   for (size_t i = 0; i < pg_.size(); ++i) {
     const CondConv& L = pg_[i];
-    __half* y = buf[cur];
+    __half* y = buf[i & 1];
     const int Ho = Hc / L.stride, Wo = Wc / L.stride;
-    if (!ar.dry) {
+    const std::string name = i == 0 ? "conv_in" : i + 1 == pg_.size() ? "conv_out" : "blocks." + std::to_string(i - 1);
+    if (!ar.dry && f.ok) {
       const char* err = nullptr;
       cudaError_t e;
       if (L.small) {
@@ -1615,21 +1617,16 @@ bool Engine::run_pose_guider(const mvb_vae_decode_args& a, Arena& ar, cudaStream
           e = launch_conv_gemm(s, a0, nullptr, Wc, Hc, NF, 9, dy, dx, L.m.w, L.cout_p, ep, num_sms_, &err);
         }
       }
-      if (e != cudaSuccess) {
-        err_ = std::string(i == 0 ? "conv_in" : i + 1 == pg_.size() ? "conv_out" : "blocks." + std::to_string(i - 1)) +
-               ": " + (err ? err : "launch failed") + " (" + cudaGetErrorString(e) + ")";
-        return false;
-      }
-      taps_.push_back({i == 0 ? "conv_in" : i + 1 == pg_.size() ? "conv_out" : "blocks." + std::to_string(i - 1), y,
-                       (long long)NF * Ho * Wo, L.cout_p});
+      if (e != cudaSuccess) f.fail((name + ": " + (err ? err : "launch failed")).c_str(), e);
     }
-    x = y; cur ^= 1; Hc = Ho; Wc = Wo;
+    f.tap(name, y, (long long)NF * Ho * Wo, L.cout_p);
+    x = y; Hc = Ho; Wc = Wo;
   }
-  if (!ar.dry) {
+  if (!ar.dry && f.ok) {
     cudaError_t e = tokens_to_ncthw(s, (const __half*)x, pg_.back().cout_p, NF, c.out_channels, 1, Hc * Wc, a.out, a.out_is_f32);
-    if (e != cudaSuccess) { err_ = std::string("pose guider output: ") + cudaGetErrorString(e); return false; }
+    if (e != cudaSuccess) f.fail("pose guider output", e);
   }
-  return true;
+  return f.ok;
 }
 
 static const char* clip_vision_shape_error(const mvb_controlnet_args& a, const mvb_config& c) {
@@ -1651,9 +1648,7 @@ bool Engine::run_clip_vision(const mvb_controlnet_args& a, Arena& ar, cudaStream
   const int P = (S / p) * (S / p), T = P + 1, Kp = clip_patch_.K, NF = a.NF;
   const float eps = c.norm_eps;
   const long long M = (long long)NF * T;
-  mvb_unet_args ua{};
-  ua.B = NF; ua.T = 1; ua.H = 1; ua.W = 1;
-  Fwd f(this, ar, s, ua, true);
+  Fwd f(this, ar, s, NF, 1, 1, 1, true, false);
   // ---- embeddings (:202-218) + pre_layrnorm (:677): patch unfold, the patch conv as one GEMM into fp32, then one kernel
   __half* x = f.alloc_h(M, C);
   {
@@ -1716,9 +1711,7 @@ bool Engine::run_clip_text(const mvb_controlnet_args& a, Arena& ar, cudaStream_t
   const int C = c.block_out_channels[0], V = c.block_out_channels[3], NF = a.NF, L = a.H;
   const long long M = (long long)NF * L;
   const int64_t* ids = (const int64_t*)a.sample;
-  mvb_unet_args ua{};
-  ua.B = NF; ua.T = 1; ua.H = 1; ua.W = 1;
-  Fwd f(this, ar, s, ua, true);
+  Fwd f(this, ar, s, NF, 1, 1, 1, true, false);
   __half* x = f.alloc_h(M, C);
   if (!ar.dry && f.ok) {
     cudaError_t e = clip_text_embed(s, ids, NF, L, C, V, clip_tok_.w, clip_pos_, x);

@@ -159,6 +159,45 @@ int mvb_fuse_cfg_affine(const float* eps_sum, const float* counter, const void* 
                         int B, int C, int T, int HW, int cfg, float guidance_scale, float c_x, float c_e, float c_n,
                         const float* noise, float a_x, float a_e, float* aux_out, float* eps_out, void* stream);
 
+/* Fused overlap mean + classifier-free guidance + a MULTISTEP sampler step (since mvb_version() == 5). Per element
+ *   eps    = eps_sum / counter[t]; cfg: eps = uncond + g * (text - uncond)      (as mvb_fuse_cfg_affine)
+ *   m0     = a_x x + a_e eps, then clamp(m0, -clip, clip) when clip > 0
+ *   x_prev = c_x x + c0 m0 + c1 m1 + c2 m2 + c_n noise
+ * written to latents_out (fp16 / fp32 by is_f32) and, when m0_out is not NULL, m0 to m0_out (fp32). With host-computed
+ * scalars this stands in for
+ *   DPMSolverMultistepScheduler.step  musev/schedulers/scheduling_dpmsolver_multistep.py:655-769: m0 is
+ *                                     `convert_model_output` (:396-446, x0 for dpmsolver++, eps for dpmsolver); the
+ *                                     first / second / third order updates (:448-653) with D0 / D1 / D2 folded into c0..c2;
+ *                                     m1 / m2 are the converted outputs of the previous one / two steps (`model_outputs`);
+ *   EulerAncestralDiscreteScheduler.step  scheduling_euler_ancestral_discrete.py:220-323: m0 = pred_original_sample,
+ *                                     c_x = 1 + dt / sigma, c0 = -dt / sigma, c_n = sigma_up;
+ *   DDPMScheduler.step                scheduling_ddpm.py:124-262 (over diffusers scheduling_ddpm.py:280-318): m0 =
+ *                                     pred_original_sample with clip_sample, c0 / c_x = pred_original_sample_coeff /
+ *                                     current_sample_coeff, c_n = the standard deviation of the variance type.
+ * Aliasing: m0_out MAY BE m2 (the same pointer): every element reads m2 before it writes m0, so two history buffers rotate
+ * without a third. No other pair of the buffers may overlap -- in particular latents_out overlaps none of eps_sum, counter,
+ * latents_in, m1, m2, noise, m0_out, and m0_out overlaps none of them but m2 (exactly). Overlaps are rejected before a
+ * launch (MVB_ERR_INVALID, "overlap" in mvb_last_error()). HBM-bound: (4 or 8 with cfg) + 2 * (2 or 4) + 4 per non-NULL
+ * m1 / m2 / noise / m0_out bytes per element. */
+typedef struct mvb_multistep_args mvb_multistep_args;
+struct mvb_multistep_args {
+  const float* eps_sum;     /* fp32 [2B, C, T, HW] (cfg, uncond half first) or [B, C, T, HW] */
+  const float* counter;     /* fp32 [T] windows per frame, or NULL (= 1) */
+  const void* latents_in;   /* x, [B, C, T, HW], fp32 if is_f32 else fp16 */
+  void* latents_out;        /* x_prev, same shape and dtype */
+  const float* m1;          /* fp32 history of the previous step, or NULL (read as 0: pass NULL when c1 == 0) */
+  const float* m2;          /* fp32 history of the step before, or NULL (read as 0: pass NULL when c2 == 0) */
+  const float* noise;       /* fp32, or NULL */
+  float* m0_out;            /* fp32 m0 of this step, or NULL; may be m2 */
+  int is_f32, B, C, T, HW;
+  int cfg;                  /* 1: eps_sum holds both CFG halves; 0: one prediction (plain scheduler.step) */
+  float guidance_scale;     /* g */
+  float a_x, a_e;           /* m0 = a_x x + a_e eps */
+  float clip;               /* > 0: clamp m0 to [-clip, clip]; <= 0: no clamp */
+  float c_x, c0, c1, c2, c_n;   /* x_prev = c_x x + c0 m0 + c1 m1 + c2 m2 + c_n noise */
+};
+int mvb_fuse_cfg_multistep(const mvb_multistep_args* args, void* stream);
+
 /* eps_sum[:, :, frames[i]] += eps_window[:, :, src_t0 + i] (musev/pipelines/pipeline_controlnet.py:2068-2078).
  * eps_window [2B, C, Tw, HW] fp32/fp16; frames_dev: device int32[nframes]. */
 int mvb_accumulate_window(float* eps_sum, int B2, int C, int T, int HW, const void* eps_window, int is_f32, int Tw,

@@ -115,6 +115,16 @@ class MvbVaeDecodeArgs(C.Structure):
                 ("latent_scale", C.c_float), ("out", C.c_void_p), ("out_is_f32", C.c_int), ("postprocess", C.c_int)]
 
 
+class MvbMultistepArgs(C.Structure):
+    _fields_ = [
+        ("eps_sum", C.c_void_p), ("counter", C.c_void_p), ("latents_in", C.c_void_p), ("latents_out", C.c_void_p),
+        ("m1", C.c_void_p), ("m2", C.c_void_p), ("noise", C.c_void_p), ("m0_out", C.c_void_p),
+        ("is_f32", C.c_int), ("B", C.c_int), ("C", C.c_int), ("T", C.c_int), ("HW", C.c_int), ("cfg", C.c_int),
+        ("guidance_scale", C.c_float), ("a_x", C.c_float), ("a_e", C.c_float), ("clip", C.c_float),
+        ("c_x", C.c_float), ("c0", C.c_float), ("c1", C.c_float), ("c2", C.c_float), ("c_n", C.c_float),
+    ]
+
+
 def lib() -> C.CDLL:
     """Load libmusevb200.so (built in-tree by musev_b200.build). Raises if it is not there."""
     global _lib
@@ -168,6 +178,7 @@ def _declare(l: C.CDLL) -> None:
                                       C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_float,
                                       C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     l.mvb_fuse_cfg_affine.restype = C.c_int
+    fn("mvb_fuse_cfg_multistep", C.c_int, C.POINTER(MvbMultistepArgs), C.c_void_p)
     l.mvb_accumulate_window.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                         C.c_int, C.c_void_p, C.c_int, C.c_void_p]
     l.mvb_accumulate_window.restype = C.c_int

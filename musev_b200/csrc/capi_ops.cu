@@ -1,6 +1,7 @@
 // C-ABI entry points for the individual device ops (used by the per-op parity tests and by embedders that
 // only want one kernel). The whole-forward entry points live in capi_engine.cu.
 #include <cuda_runtime.h>
+#include <stdint.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -33,8 +34,9 @@ extern "C" {
 
 const char* mvb_last_error(void) { return g_err; }
 
-// 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle; 4: the CLIP text handle, causal attention
-int mvb_version(void) { return 4; }
+// 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle; 4: the CLIP text handle, causal attention;
+// 5: mvb_fuse_cfg_multistep
+int mvb_version(void) { return 5; }
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   if (!d || !d->a0 || !d->weight || !d->out) return fail("mvb_op_conv_gemm: null pointer", cudaSuccess);
@@ -159,6 +161,30 @@ int mvb_fuse_cfg_affine(const float* eps_sum, const float* counter, const void* 
   cudaError_t e = fuse_cfg_affine((cudaStream_t)stream, eps_sum, counter, latents_in, latents_out, is_f32, B, C, T, HW, cfg,
                                   guidance_scale, c_x, c_e, c_n, noise, a_x, a_e, aux_out, eps_out);
   if (e != cudaSuccess) return fail("mvb_fuse_cfg_affine", e);
+  return MVB_OK;
+}
+
+int mvb_fuse_cfg_multistep(const mvb_multistep_args* a, void* stream) {
+  if (!a || !a->eps_sum || !a->latents_in || !a->latents_out) return fail("mvb_fuse_cfg_multistep: null pointer", cudaSuccess);
+  if (a->B < 0 || a->C < 0 || a->T < 0 || a->HW < 0) return fail("mvb_fuse_cfg_multistep: negative extent", cudaSuccess);
+  const size_t n = (size_t)a->B * a->C * a->T * a->HW;
+  // [start, start + bytes) of every buffer; m0_out may be exactly m2, no other pair may overlap
+  struct Span { const void* p; size_t bytes; };
+  const Span lat_out{a->latents_out, n * (a->is_f32 ? 4 : 2)}, m0{a->m0_out, n * 4}, m2{a->m2, n * 4};
+  const Span others[] = {{a->eps_sum, n * 4 * (a->cfg ? 2 : 1)}, {a->counter, (size_t)a->T * 4},
+                         {a->latents_in, n * (a->is_f32 ? 4 : 2)}, {a->m1, n * 4}, {a->noise, n * 4}};
+  auto overlap = [](const Span& x, const Span& y) {
+    if (!x.p || !y.p || !x.bytes || !y.bytes) return false;
+    const uintptr_t x0 = (uintptr_t)x.p, y0 = (uintptr_t)y.p;
+    return x0 < y0 + y.bytes && y0 < x0 + x.bytes;
+  };
+  bool bad = overlap(lat_out, m0) || overlap(lat_out, m2) || (overlap(m0, m2) && a->m0_out != a->m2);
+  for (const Span& o : others) bad = bad || overlap(lat_out, o) || overlap(m0, o);
+  if (bad) return fail("mvb_fuse_cfg_multistep: buffers overlap (only m0_out == m2 is allowed)", cudaSuccess);
+  cudaError_t e = fuse_cfg_multistep((cudaStream_t)stream, a->eps_sum, a->counter, a->latents_in, a->latents_out, a->is_f32,
+                                     a->B, a->C, a->T, a->HW, a->cfg, a->guidance_scale, a->a_x, a->a_e, a->clip, a->c_x,
+                                     a->c0, a->c1, a->c2, a->c_n, a->m1, a->m2, a->noise, a->m0_out);
+  if (e != cudaSuccess) return fail("mvb_fuse_cfg_multistep", e);
   return MVB_OK;
 }
 

@@ -76,6 +76,12 @@ cudaError_t fuse_cfg_ddim(cudaStream_t s, const float* eps_sum, const float* cou
 cudaError_t fuse_cfg_affine(cudaStream_t s, const float* eps_sum, const float* counter, const void* latents_in,
                             void* latents_out, int is_f32, int B, int C, int T, int HW, int cfg, float guidance, float c_x,
                             float c_e, float c_n, const float* noise, float a_x, float a_e, float* aux_out, float* eps_out);
+// overlap mean + CFG + multistep sampler step (samplers.cu): m0 = clamp(a_x x + a_e eps, +-clip),
+// x_prev = c_x x + c0 m0 + c1 m1 + c2 m2 + c_n noise; m1 / m2 / noise / m0_out may be null, m0_out may alias m2
+cudaError_t fuse_cfg_multistep(cudaStream_t s, const float* eps_sum, const float* counter, const void* latents_in,
+                               void* latents_out, int is_f32, int B, int C, int T, int HW, int cfg, float guidance, float a_x,
+                               float a_e, float clip, float c_x, float c0, float c1, float c2, float c_n, const float* m1,
+                               const float* m2, const float* noise, float* m0_out);
 // eps_sum[:, :, frames[i]] += eps_window[:, :, src_t0 + i]   (pipeline_controlnet.py:2068-2078)
 cudaError_t accumulate_window(cudaStream_t s, float* eps_sum, int B2, int C, int T, int HW, const void* eps_win,
                               int is_f32, int Tw, int src_t0, const int* frames_dev, int nframes);

@@ -202,6 +202,30 @@ def fuse_cfg_affine(eps_sum, counter, latents, guidance, c_x, c_e, c_n=0.0, nois
     return out
 
 
+def fuse_cfg_multistep(eps_sum, counter, latents, guidance, a_x, a_e, clip, c_x, c0, c1=0.0, c2=0.0, c_n=0.0, m1=None,
+                       m2=None, noise=None, m0_out=None, cfg=True, out=None):
+    """m0 = clamp(a_x x + a_e eps, +-clip) (clip <= 0: none) -> m0_out; x_prev = c_x x + c0 m0 + c1 m1 + c2 m2 + c_n noise
+    (eps = overlap mean + CFG of eps_sum). m1 / m2 / noise / m0_out: fp32 like latents, or None; m0_out may be m2."""
+    B, Cc, T = latents.shape[:3]
+    HW = latents.shape[3] * latents.shape[4]
+    assert eps_sum.dtype == torch.float32 and eps_sum.is_contiguous() and latents.is_contiguous()
+    assert eps_sum.numel() == latents.numel() * (2 if cfg else 1), "eps_sum must be [2B,...] with cfg, [B,...] without"
+    assert latents.dtype in (torch.float16, torch.float32), f"latents must be fp16 or fp32, got {latents.dtype}"
+    assert counter is None or (counter.dtype == torch.float32 and counter.is_contiguous() and counter.numel() == T)
+    for t_ in (m1, m2, noise, m0_out):
+        assert t_ is None or (t_.dtype == torch.float32 and t_.is_contiguous() and t_.numel() == latents.numel())
+    if out is None:
+        out = torch.empty_like(latents)
+    a = _capi.MvbMultistepArgs()
+    a.eps_sum, a.counter, a.latents_in, a.latents_out = eps_sum.data_ptr(), _ptr(counter), latents.data_ptr(), out.data_ptr()
+    a.m1, a.m2, a.noise, a.m0_out = _ptr(m1), _ptr(m2), _ptr(noise), _ptr(m0_out)
+    a.is_f32, a.B, a.C, a.T, a.HW, a.cfg = int(latents.dtype == torch.float32), B, Cc, T, HW, int(cfg)
+    a.guidance_scale, a.a_x, a.a_e, a.clip = guidance, a_x, a_e, clip
+    a.c_x, a.c0, a.c1, a.c2, a.c_n = c_x, c0, c1, c2, c_n
+    _capi.check(_capi.lib().mvb_fuse_cfg_multistep(C.byref(a), _stream()))
+    return out
+
+
 def accumulate_window(eps_sum, eps_win, src_t0, frames_dev):
     B2, Cc, T = eps_sum.shape[:3]
     HW = eps_sum.shape[3] * eps_sum.shape[4]

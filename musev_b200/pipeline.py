@@ -17,6 +17,7 @@ import torch
 
 from . import ops
 from .context import assign_windows, prepare_global_context
+from .samplers import multistep_update
 from .scheduler import DDIMScheduler, _PRED, _variance_noise
 
 
@@ -29,9 +30,10 @@ class DenoiseOutput:
 
 class ParallelDenoiser:
     def __init__(self, unet, scheduler, process_group=None, device_ops=None):
-        """scheduler: musev_b200 `DDIMScheduler` (any prediction type / clipping / eta) or one of the affine samplers of
-        musev_b200.samplers (`EulerDiscreteScheduler`, the predictor's default; `LCMScheduler`)."""
-        # device_ops: module providing accumulate_window / fuse_cfg_ddim; the CUDA library unless a test injects a double
+        """scheduler: musev_b200 `DDIMScheduler` (any prediction type / clipping / eta), one of the affine samplers of
+        musev_b200.samplers (`EulerDiscreteScheduler`, the predictor's default; `LCMScheduler`) or any scheduler with a
+        `multistep_plan` (`DPMSolverMultistepScheduler`, `EulerAncestralDiscreteScheduler`, `DDPMScheduler`)."""
+        # device_ops: module providing accumulate_window / fuse_cfg_*; the CUDA library unless a test injects a double
         self.ops = device_ops if device_ops is not None else ops
         self.unet = unet
         self.scheduler = scheduler
@@ -130,13 +132,19 @@ class ParallelDenoiser:
         eps_sum = torch.zeros((2 * B, C, T, h, w), dtype=torch.float32, device=dev)
         latents = latents.contiguous()
         is_ddim = isinstance(sch, DDIMScheduler)
+        is_multistep = not is_ddim and hasattr(sch, "multistep_plan")
+        if is_multistep:
+            # m1 / m2 of the multistep kernel (DPM-Solver's `model_outputs`). Every rank applies the same plan and kernel to
+            # the same all-reduced eps, so the histories stay replicated bit-exactly, like the latents.
+            history = [torch.zeros((B, C, T, h, w), dtype=torch.float32, device=dev) for _ in range(2)]
         if is_ddim:
             pred = _PRED[sch.config.prediction_type]
             clip = sch.config.clip_sample_range if sch.config.clip_sample else 0.0
 
         def step_noise():
             """Per-step noise [B,C,T,h,w] fp32, identical on every rank (drawn on rank 0, broadcast): scheduling_ddim.py
-            :266-295, scheduling_euler_discrete.py:116-127, scheduling_lcm.py:291-300."""
+            :266-295, scheduling_euler_discrete.py:116-127, scheduling_lcm.py:291-300, scheduling_euler_ancestral_discrete.py
+            :303-314, scheduling_ddpm.py:220-241."""
             nz = _variance_noise(latents, generator, noise_type, w_ind_noise).float().contiguous()
             if self.world > 1:
                 self._dist.broadcast(nz, src=0, group=self.pg)
@@ -192,6 +200,10 @@ class ParallelDenoiser:
                                                      noise=step_noise())                 # eta > 0: scheduling_ddim.py:266-295
                 else:
                     latents = self.ops.fuse_cfg_ddim(eps_sum, counter, latents, float(g), a_t, a_p, pred, clip)  # :2079,2101-2117
+            elif is_multistep:
+                p = sch.multistep_plan(t)                                           # DPM-Solver / Euler ancestral / DDPM
+                latents = multistep_update(self.ops, p, eps_sum, counter, latents, g, history,
+                                           step_noise() if p.needs_noise else None)
             else:
                 a = sch.affine_step(t)                                              # Euler / LCM: scalars on the host
                 latents = self.ops.fuse_cfg_affine(eps_sum, counter, latents, float(g), a.c_x, a.c_e, a.c_n,

@@ -2,7 +2,7 @@
 
 Reference: diffusers/src/diffusers/models/controlnet.py:645-852, called from
 musev/pipelines/pipeline_controlnet.py:1238-1262. The SD-1.5 encoder half, the 12 + 1 zero convolutions and the output
-scaling run inside libmusevb200.so (`mvb_controlnet_forward`, musev_b200/csrc/engine.cu). The conditioning embedding
+scaling run inside libmusevb200.so (`mvb_controlnet_forward`, musev_b200/csrc/engine_encoder.cu). The conditioning embedding
 (controlnet.py:101-112) is a one-shot conv stack on the 8x larger condition image; the pipeline computes it once per
 call and passes `controlnet_cond_latents` on every step (pipeline_controlnet.py:1258), so it stays a handful of torch
 convolutions here, outside the per-step path.

@@ -12,78 +12,6 @@ struct mvb_handle {
   mvb::Engine* e;
 };
 
-// Validators of each model kind's mvb_config: the shapes its kernels take (MVB_ERR_INVALID otherwise)
-static bool unet_config_ok(const mvb_config* cfg) {
-  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->heads < 1 || cfg->norm_num_groups < 1) return false;
-  for (int i = 0; i < cfg->num_blocks; ++i) {
-    const int c = cfg->block_out_channels[i];
-    if (c % 64 || c % cfg->heads || (c / cfg->heads) % 8 || c % cfg->norm_num_groups) return false;
-  }
-  return cfg->cross_attention_dim % 64 == 0 && cfg->in_channels * 9 <= 64;
-}
-
-// The ControlNet / ReferenceNet encoder: the UNet's down blocks + mid block, one output map per layer
-static bool encoder_config_ok(const mvb_config* cfg) {
-  if (!unet_config_ok(cfg)) return false;
-  int n_out = 2;
-  for (int i = 0; i < cfg->num_blocks; ++i) n_out += cfg->layers_per_block + (i == cfg->num_blocks - 1 ? 0 : 1);
-  return n_out <= MVB_CONTROLNET_MAX_OUT;
-}
-
-// Either VAE half: conv_in is an im2col of 9 * in_channels <= 64 columns; conv_out writes 16 padded columns, which hold
-// out_channels image channels (decoder) or 2 * out_channels moments (encoder)
-static bool vae_config_ok(const mvb_config* cfg, int max_out_channels) {
-  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->norm_num_groups < 1 || cfg->layers_per_block < 1) return false;
-  for (int i = 0; i < cfg->num_blocks; ++i) {
-    const int c = cfg->block_out_channels[i];
-    if (c % 64 || c % cfg->norm_num_groups || (c / cfg->norm_num_groups) % 2) return false;
-  }
-  return cfg->in_channels >= 1 && cfg->in_channels <= 7 && cfg->out_channels >= 1 && cfg->out_channels <= max_out_channels;
-}
-
-// The layer split of Engine::build_pose_guider: conv_in and every layer reading 16 / 32 channels run on the small-channel
-// kernel, whose output is at most 128 (padded) channels.
-static bool pose_guider_config_ok(const mvb_config* cfg) {
-  if (cfg->num_blocks < 1 || cfg->num_blocks > 4 || cfg->in_channels < 1 || cfg->in_channels > 3) return false;
-  if (cfg->out_channels < 1 || cfg->out_channels > 4096) return false;
-  const int nb = cfg->num_blocks;
-  for (int i = 0; i < nb; ++i)
-    if (cfg->block_out_channels[i] < 1 || cfg->block_out_channels[i] > 4096) return false;
-  auto small = [](int cin) { return cin == 16 || cin == 32; };
-  if (mvb::cond_channels_padded(cfg->block_out_channels[0]) > 128) return false;                           // conv_in
-  for (int i = 0; i + 1 < nb; ++i) {
-    const int c = cfg->block_out_channels[i], n = cfg->block_out_channels[i + 1];
-    if (small(c) && mvb::cond_channels_padded(n) > 128) return false;                                       // blocks.2i+1
-  }
-  if (small(cfg->block_out_channels[nb - 1]) && cfg->out_channels > 128) return false;                      // conv_out
-  return true;
-}
-
-// The CLIP vision tower (Engine::build_clip_vision): hidden size a multiple of 64 (conv_gemm K), head dim a multiple of 8 and
-// at most 192 (attention kernel), the MLP width a multiple of 64, the image a whole number of patches, act 2 / 3.
-static bool clip_vision_config_ok(const mvb_config* cfg) {
-  const int C = cfg->block_out_channels[0], I = cfg->block_out_channels[1], p = cfg->block_out_channels[2],
-            S = cfg->block_out_channels[3];
-  if (cfg->num_blocks != 4 || cfg->in_channels < 1 || cfg->in_channels > 4 || cfg->layers_per_block < 1) return false;
-  if (C < 64 || C > 2048 || C % 64 || cfg->heads < 1 || C % cfg->heads) return false;
-  const int d = C / cfg->heads;
-  if (d % 8 || d > 192 || I < 64 || I % 64 || p < 1 || S < p || S % p || (S / p) * (S / p) > 4096) return false;
-  if (cfg->out_channels < 8 || cfg->out_channels % 8 || !(cfg->norm_eps >= 0.f)) return false;
-  return cfg->norm_num_groups == 2 || cfg->norm_num_groups == 3;
-}
-
-// The CLIP text encoder (Engine::build_clip_text): the layer geometry of the vision tower; block_out_channels[2..3] =
-// max_position_embeddings (1..4096) and vocab_size (>= 1); out_channels = eos_token_id (>= 0).
-static bool clip_text_config_ok(const mvb_config* cfg) {
-  const int C = cfg->block_out_channels[0], I = cfg->block_out_channels[1], P = cfg->block_out_channels[2],
-            V = cfg->block_out_channels[3];
-  if (cfg->num_blocks != 4 || cfg->layers_per_block < 1 || P < 1 || P > 4096 || V < 1 || cfg->out_channels < 0) return false;
-  if (C < 64 || C > 2048 || C % 64 || cfg->heads < 1 || C % cfg->heads) return false;
-  const int d = C / cfg->heads;
-  if (d % 8 || d > 192 || I < 64 || I % 64 || !(cfg->norm_eps >= 0.f)) return false;
-  return cfg->norm_num_groups == 2 || cfg->norm_num_groups == 3;
-}
-
 // A handle of a validated configuration: MVB_ERR_STATE when out of host memory, MVB_ERR_CUDA when the device refused
 static int create(const mvb_config* cfg, int device, mvb::Kind kind, mvb_handle** out) {
   mvb::Engine* e = new (std::nothrow) mvb::Engine(*cfg, device, kind);
@@ -98,17 +26,17 @@ static int create(const mvb_config* cfg, int device, mvb::Kind kind, mvb_handle*
 extern "C" {
 
 int mvb_create(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out || !unet_config_ok(cfg) || cfg->out_channels > 16) return MVB_ERR_INVALID;
+  if (!cfg || !out || !mvb::unet_config_ok(cfg) || cfg->out_channels > 16) return MVB_ERR_INVALID;
   return create(cfg, device, mvb::Kind::UNet, out);
 }
 
 int mvb_create_controlnet(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out || !encoder_config_ok(cfg)) return MVB_ERR_INVALID;
+  if (!cfg || !out || !mvb::encoder_config_ok(cfg)) return MVB_ERR_INVALID;
   return create(cfg, device, mvb::Kind::ControlNet, out);
 }
 
 int mvb_create_referencenet(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out || !encoder_config_ok(cfg)) return MVB_ERR_INVALID;
+  if (!cfg || !out || !mvb::encoder_config_ok(cfg)) return MVB_ERR_INVALID;
   return create(cfg, device, mvb::Kind::ReferenceNet, out);
 }
 
@@ -136,7 +64,7 @@ int mvb_controlnet_forward(mvb_handle* h, const mvb_controlnet_args* args, void*
 }
 
 int mvb_create_vae_decoder(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out || !vae_config_ok(cfg, 16)) return MVB_ERR_INVALID;
+  if (!cfg || !out || !mvb::vae_config_ok(cfg, 16)) return MVB_ERR_INVALID;
   return create(cfg, device, mvb::Kind::VaeDecoder, out);
 }
 
@@ -151,7 +79,7 @@ int mvb_vae_decode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspa
 }
 
 int mvb_create_vae_encoder(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out || !vae_config_ok(cfg, 8)) return MVB_ERR_INVALID;
+  if (!cfg || !out || !mvb::vae_config_ok(cfg, 8)) return MVB_ERR_INVALID;
   return create(cfg, device, mvb::Kind::VaeEncoder, out);
 }
 
@@ -166,7 +94,7 @@ int mvb_vae_encode(mvb_handle* h, const mvb_vae_decode_args* args, void* workspa
 }
 
 int mvb_create_pose_guider(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out || !pose_guider_config_ok(cfg)) return MVB_ERR_INVALID;
+  if (!cfg || !out || !mvb::pose_guider_config_ok(cfg)) return MVB_ERR_INVALID;
   return create(cfg, device, mvb::Kind::PoseGuider, out);
 }
 
@@ -182,7 +110,7 @@ int mvb_pose_guider_forward(mvb_handle* h, const mvb_vae_decode_args* args, void
 }
 
 int mvb_create_clip_vision(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out || !clip_vision_config_ok(cfg)) return MVB_ERR_INVALID;
+  if (!cfg || !out || !mvb::clip_vision_config_ok(cfg)) return MVB_ERR_INVALID;
   return create(cfg, device, mvb::Kind::ClipVision, out);
 }
 
@@ -198,7 +126,7 @@ int mvb_clip_vision_forward(mvb_handle* h, const mvb_controlnet_args* args, void
 }
 
 int mvb_create_clip_text(const mvb_config* cfg, int device, mvb_handle** out) {
-  if (!cfg || !out || !clip_text_config_ok(cfg)) return MVB_ERR_INVALID;
+  if (!cfg || !out || !mvb::clip_text_config_ok(cfg)) return MVB_ERR_INVALID;
   return create(cfg, device, mvb::Kind::ClipText, out);
 }
 

@@ -1,5 +1,7 @@
-// Whole-forward engine: owns the packed weights of one UNet3DConditionModel and launches the fixed kernel sequence
-// of musev/models/unet_3d_condition.py:773-1280 on a caller-provided stream and workspace.
+// Whole-forward engine: owns the packed weights of one model (a UNet3DConditionModel or one of the other kinds below) and
+// launches its fixed kernel sequence on a caller-provided stream and workspace. The core (packing, construction, the
+// shared layer builders) is engine.cu, the layer toolkit of every forward engine_fwd.cuh, and each kind has one file:
+// engine_unet.cu, engine_encoder.cu (ControlNet / ReferenceNet), engine_vae.cu, engine_pose_guider.cu, engine_clip.cu.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -7,6 +9,7 @@
 #include <initializer_list>
 #include <string>
 #include <unordered_map>
+#include <variant>
 #include <vector>
 
 #include "../../include/musev_b200.h"
@@ -144,11 +147,76 @@ struct CondConv {
 };
 
 // One pre-norm CLIP encoder layer (transformers CLIPEncoderLayer, models/clip/modeling_clip.py:354-386), of the vision tower
-// and of the text encoder alike (Engine::build_clip_layers, Fwd::clip_encoder)
+// and of the text encoder alike (engine_clip.cu: Engine::build_clip_layers, clip_encoder)
 struct ClipLayer {
   Norm ln1, ln2;
   Mat qkv;            // q | k | v projections, heads padded to dp columns (rowmode 1), biases padded alike
   Mat out, fc1, fc2;
+};
+
+// The time_emb_proj (or frame_emb_proj) of every layer concatenated into one matrix; while the model is built, `rows`
+// counts the rows registered so far, and each layer takes the next ones
+struct EmbProj {
+  Mat m;
+  int rows = 0;
+};
+
+// The weights of each model kind: an Engine holds the one of its own kind (Engine::model_)
+struct UNetWeights {          // engine_unet.cu
+  Mat conv_in, conv_out;
+  Norm norm_out;
+  Mat time_l1, time_l2, frame_l1, frame_l2;
+  EmbProj temb, femb;
+  bool has_tin = false;
+  TemporalT tin;
+  ReferAttn first_ref, mid_ref;
+  std::vector<Block> down, up;
+  Resnet mid_res[2];
+  TempConv mid_tc[2];
+  SpatialT mid_st;
+  TemporalT mid_tt;
+};
+struct EncoderWeights {       // engine_encoder.cu: ControlNet / ReferenceNet
+  Mat conv_in, time_l1, time_l2;
+  EmbProj temb;
+  std::vector<Block> down;
+  Resnet mid_res[2];
+  SpatialT mid_st;
+  Mat zero_convs[MVB_CONTROLNET_MAX_OUT];   // ControlNet: controlnet_down_blocks.* then controlnet_mid_block
+  int n_outs = 0;                           // output maps: one per down layer and downsampler, then the mid block
+};
+struct VaeWeights {           // engine_vae.cu: either AutoencoderKL half
+  Mat conv_in, conv_out;
+  Norm norm_out;
+  std::vector<Block> blocks;                // encoder down blocks / decoder up blocks
+  Resnet mid_res[2];                        // the mid block: resnet, single-head attention (GroupNorm + biased q/k/v/out), resnet
+  Norm attn_norm;
+  Mat q, k, v, o;
+  float* pq_w = nullptr;                    // post_quant_conv (decoder) / quant_conv (encoder), fp32 [C, C] + bias
+  float* pq_b = nullptr;
+};
+struct PoseGuiderWeights {    // engine_pose_guider.cu
+  std::vector<CondConv> layers;             // conv_in, blocks.0 .. blocks.{2 (num_blocks - 1) - 1}, conv_out
+};
+// engine_clip.cu: the vision tower (CLIPVisionModelWithProjection) or the text encoder (CLIPTextModel). mvb_config carries
+// their sizes in fields named for the UNet; build_clip_* decodes them into the named values here once.
+struct ClipWeights {
+  int hidden = 0, intermediate = 0;         // block_out_channels[0], [1]
+  int act = 0;                              // norm_num_groups: the MLP activation (conv_gemm act code 2 / 3)
+  float eps = 0.f;                          // norm_eps: every LayerNorm's
+  int patch_size = 0, image_size = 0;       // vision: block_out_channels[2], [3]
+  int positions = 0, vocab = 0;             // text: block_out_channels[2], [3] (max_position_embeddings, vocab_size)
+  int eos_token_id = 0;                     // text: out_channels
+  std::vector<ClipLayer> layers;
+  float* pos = nullptr;                     // position embeddings, fp32
+  // vision: patch embedding [C, Kp] (no bias), class embedding (fp32), pre_layrnorm / post_layernorm, visual_projection
+  // [out_channels, C] (no bias)
+  Mat patch, proj;
+  float* cls = nullptr;
+  Norm pre, post;
+  // text: token_embedding [vocab, C] fp16 (a Mat without bias), final_layer_norm
+  Mat tok;
+  Norm final_norm;
 };
 
 struct Arena {
@@ -204,35 +272,51 @@ class Engine {
   const std::vector<Tap>& taps() const { return taps_; }
   int num_params() const { return (int)loaders_.size(); }
 
+  // The layer toolkit every forward runs on (engine_fwd.cuh); public so that a kind's file can hold stages of its own
+  struct Fwd;
+
  private:
-  // construction
+  // construction (engine.cu), and each kind's build in its own file
   void build();
   void build_unet();
   void build_controlnet();
   void build_vae();
   void build_vae_encoder();
-  void build_vae_mid(const std::string& p, int C);
+  void build_vae_mid(VaeWeights& w, const std::string& p, int C);
   void build_pose_guider();
   void build_clip_vision();
   void build_clip_text();
-  void build_clip_layers(const std::string& prefix, int C, int I);
-  template <typename T> T* slab(size_t n);
+  void build_clip_layers(ClipWeights& w, const std::string& prefix);
+  template <typename T> T* slab(size_t n) {   // n elements of the weight slab; null while the first pass counts bytes
+    const size_t a = (slab_off_ + 255) & ~size_t(255);
+    slab_off_ = a + n * sizeof(T);
+    return slab_counting_ ? nullptr : reinterpret_cast<T*>(slab_ + a);
+  }
   Mat make_mat(int N, int K, bool bias);
   Norm make_norm(const std::string& p, int C);
-  void reg_mat(const std::string& name, Mat& m, int row0, int rows_dst, int rowmode, int p0, int p1, int nsrc, int ksrc,
-               int colmode = 0, int cin = 0, int taps = 1);
+  // The packed layouts of a matrix / convolution weight `name` in m (PackGeom, read by the packer, the LoRA merge and the
+  // read-back). Plain rows: source rows [0, rows) at packed rows [row0, row0 + rows), source columns [0, ksrc).
+  void reg_rows(const std::string& name, Mat& m, int rows, int ksrc, int row0 = 0);
+  // Head-padded rows (rowmode 1): heads_ heads of d source rows each, at dp packed rows each from packed row row0
+  void reg_head_rows(const std::string& name, Mat& m, int row0, int d, int dp);
+  // GEGLU-interleaved rows (rowmode 2): all m.N rows, value and gate halves in alternating chunks of 16 (geglu_src)
+  void reg_geglu_rows(const std::string& name, Mat& m);
+  // Convolution [nsrc, cin, taps] as tap-major columns tap * cin_dst + c (colmode 1; cin_dst 0: cin) in packed rows
+  // [0, rows), rows past nsrc zero
+  void reg_conv_cols(const std::string& name, Mat& m, int rows, int nsrc, int cin, int taps, int cin_dst = 0);
+  void reg_mat(const std::string& name, Mat& m, int row0, PackGeom g);
   void reg_vec(const std::string& name, float* dst, int n, int nsrc_expected, int vmode = 0, int p0 = 0, int p1 = 0);
   void reg_linear(const std::string& p, Mat& m, int N, int K, bool bias);
   void reg_conv(const std::string& p, Mat& m, int N, int Cin, int taps);
   void build_tblock(const std::string& p, TBlock& b, int C, bool cross);
-  void build_resnet(const std::string& p, Resnet& r, int cin, int C, bool has_temb = true);
+  // temb: the concatenated time_emb_proj the resnet takes its rows of, null for a resnet without one (the VAE)
+  void build_resnet(const std::string& p, Resnet& r, int cin, int C, EmbProj* temb);
   void build_tempconv(const std::string& p, TempConv& t, int C);
   void build_spatial(const std::string& p, SpatialT& s, int C);
-  void build_temporal(const std::string& p, TemporalT& t, int C);
+  void build_temporal(const std::string& p, TemporalT& t, int C, EmbProj& femb);
   void build_refer(const std::string& p, ReferAttn& r, int C);
 
   // forward helpers (all return false on error, message in err_)
-  struct Fwd;
   template <typename Args> using RunFn = bool (Engine::*)(const Args&, Arena&, cudaStream_t);
   // Every kind's workspace query: `run` on a dry arena, its peak + 4096 bytes; -1 on a handle of another kind
   template <typename Args>
@@ -264,49 +348,24 @@ class Engine {
   char* slab_ = nullptr;
   size_t slab_bytes_ = 0, slab_off_ = 0;
   bool slab_counting_ = true;
-
-  // model
-  Mat conv_in_, conv_out_;
-  Norm norm_out_;
-  Mat time_l1_, time_l2_, frame_l1_, frame_l2_;
-  Mat temb_all_, femb_all_;     // concatenated time_emb_proj / frame_emb_proj of every layer
-  int temb_total_ = 0, femb_total_ = 0;
-  bool has_tin_ = false;
-  TemporalT tin_;
-  ReferAttn first_ref_, mid_ref_;
-  std::vector<Block> down_, up_;
-  Resnet mid_res_[2];
-  TempConv mid_tc_[2];
-  SpatialT mid_st_;
-  TemporalT mid_tt_;
   unsigned int* gn_counter_dev_ = nullptr;   // grid-barrier word of the one-launch GroupNorm
   unsigned int gn_base_ = 0;                 // arrivals it has seen (host bookkeeping)
   bool gn_fused_ = false;                    // env MVB_GN_FUSED=1 selects the one-launch GroupNorm
   int* zero_idx_dev_ = nullptr;  // device int[32] scratch for vis-cond frame indices
   float* fidx_dev_ = nullptr;    // device float[64] scratch for timestep / frame index values
-  Mat zero_convs_[MVB_CONTROLNET_MAX_OUT];   // ControlNet: controlnet_down_blocks.* then controlnet_mid_block
-  int n_zero_convs_ = 0;
-  // VAE: post_quant_conv (decoder) / quant_conv (encoder), fp32 [C, C] + bias; the mid block's resnets are mid_res_ and
-  // its single-head attention is q/k/v/out with bias after a GroupNorm (build_vae_mid, Fwd::vae_mid)
-  float* vae_pq_w_ = nullptr;
-  float* vae_pq_b_ = nullptr;
-  Norm vae_attn_norm_;
-  Mat vae_q_, vae_k_, vae_v_, vae_o_;
-  std::vector<CondConv> pg_;   // PoseGuider: conv_in, blocks.0 .. blocks.{2 (num_blocks - 1) - 1}, conv_out
-  // ClipVision (mvb_create_clip_vision): patch embedding [C, Kp] (no bias), class / position embeddings (fp32), the layers,
-  // pre_layrnorm / post_layernorm and visual_projection [proj, C] (no bias)
-  Mat clip_patch_, clip_proj_;
-  float* clip_cls_ = nullptr;
-  float* clip_pos_ = nullptr;
-  Norm clip_pre_, clip_post_;
-  std::vector<ClipLayer> clip_;   // the encoder layers of either CLIP kind (build_clip_layers)
-  // ClipText (mvb_create_clip_text): token_embedding [vocab, C] fp16 (a Mat without bias), position_embedding in clip_pos_,
-  // the layers in clip_, final_layer_norm
-  Mat clip_tok_;
-  Norm clip_final_;
+
+  // the weights of this engine's kind (its build_* emplaces them)
+  std::variant<UNetWeights, EncoderWeights, VaeWeights, PoseGuiderWeights, ClipWeights> model_;
 };
 
-// Channel count a PoseGuider activation is stored with: 16 / 32 as is (small-channel kernel), others padded to 64k.
-inline int cond_channels_padded(int c) { return (c == 16 || c == 32) ? c : (c + 63) / 64 * 64; }
+// Validators of each kind's mvb_config, in the kind's file: the shapes its kernels take
+bool unet_config_ok(const mvb_config* cfg);
+bool encoder_config_ok(const mvb_config* cfg);
+bool vae_config_ok(const mvb_config* cfg, int max_out_channels);
+bool pose_guider_config_ok(const mvb_config* cfg);
+bool clip_vision_config_ok(const mvb_config* cfg);
+bool clip_text_config_ok(const mvb_config* cfg);
+
+inline int pad16(int d) { return (d + 15) / 16 * 16; }
 
 }  // namespace mvb

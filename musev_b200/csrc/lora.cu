@@ -1,5 +1,6 @@
 // LoRA merge into the packed UNet / CLIP text encoder weights, and read-back of a packed weight in the reference layout. Both map packed
-// elements to source elements with the packer's src_row / src_col (engine.cuh).
+// elements to source elements with the packer's src_row / src_col (engine.cuh); the layouts are registered by the builders
+// (engine.cu: reg_rows, reg_head_rows, reg_geglu_rows, reg_conv_cols).
 // Reference arithmetic: musev/utils/model_util.py:153-262 (update_pipeline_lora_model) and :468-475 (unload_lora):
 //   delta32 = fl32(scale) * (up @ down)  (fp32),  delta16 = fp16(delta32),  W16 = fp16(float(W16) +- float(delta16)).
 // `scale` already folds in the 0 / 1 block weight of LORA_BLOCK_WEIGHT_MAP (for finite products this gives the same

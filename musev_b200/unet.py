@@ -1,6 +1,6 @@
 """Drop-in host mirror of `musev.models.unet_3d_condition.UNet3DConditionModel` (reference file:line below).
 
-The forward runs entirely inside libmusevb200.so (musev_b200/csrc/engine.cu) on the tensors' device pointers; this
+The forward runs entirely inside libmusevb200.so (musev_b200/csrc/engine_unet.cu) on the tensors' device pointers; this
 class only marshals arguments. There is no PyTorch / CPU fallback: without the library or without a CUDA device it
 raises.
 """

@@ -4,7 +4,7 @@ Reference: `MusevControlNetPipeline.decode_latents` (musev/pipelines/pipeline_co
 :2157-2171) -> `decode_latents` of the diffusers img2img pipeline (pipeline_stable_diffusion_img2img.py:486-495) ->
 `AutoencoderKL.decode` (models/autoencoder_kl.py:275-302). post_quant_conv, the decoder's convolutions / GroupNorms /
 single-head mid-block attention and the `image / 2 + 0.5, clamp(0, 1)` post-processing run inside libmusevb200.so
-(`mvb_vae_decode`, musev_b200/csrc/engine.cu `Engine::run_vae`). Frames are decoded in chunks (the reference enables VAE
+(`mvb_vae_decode`, musev_b200/csrc/engine_vae.cu `Engine::run_vae`). Frames are decoded in chunks (the reference enables VAE
 slicing = one frame at a time, pipeline_controlnet_predictor.py:284) to bound the activation arena. No CPU fallback.
 
 Encode: `AutoencoderKL.encode` (models/autoencoder_kl.py:256-297) = `Encoder.forward` (models/vae.py:133-175) + quant_conv run

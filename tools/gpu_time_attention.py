@@ -50,7 +50,7 @@ def _head_padded(rows, heads, d, dp, g):
 
 
 def make_case(name, dev):
-    """The op's arguments for one shape, laid out as engine.cu lays them out (fused q / k / v rows for self attention,
+    """The op's arguments for one shape, laid out as the engine lays them out (engine_fwd.cuh) (fused q / k / v rows for self attention,
     q plus fused k / v of the B text sequences for cross attention). Returns (q, segs, Nq, d, dp, keys per query)."""
     Nq, d, dp, kind = SHAPES[name]
     hd = HEADS * dp

@@ -1,16 +1,20 @@
 // wgmma / TMA implicit-GEMM kernel. See conv_gemm.cuh for the math and the reference call sites.
 //
-// CTA = 384 threads = 3 warpgroups, persistent over output tiles of 128 rows x BN columns:
+// Persistent CTAs over output tiles of 128 rows x BN columns. BN <= 160: 512 threads = 4 warpgroups:
 //   warpgroup 0, warp 0 : TMA producer -- per K block (64 channels of one tap) loads the A box {64, bw, bh, bn}
 //                         (out-of-image taps are zero-filled by TMA = conv padding) and the weight tile {64, BN};
 //                         warp-uniform loop, elect.sync picks the issuing lane. The warpgroup gives its registers to
-//                         the other two (setmaxnreg).
-//   warpgroups 1, 2     : MMA + epilogue -- warpgroup g owns accumulator rows [64 g, 64 g + 64) of the tile: 4 x
-//                         wgmma m64nBNk16 per K block, one K block kept in flight; then the accumulator goes through a
-//                         padded fp32 smem slice (128 columns at a time) so that each thread finishes whole 32-column
-//                         runs of one output row: bias / time-embedding / residual / GEGLU / GELU (five template variants) ->
-//                         fp16 -> 16-byte global stores.
-// Pipeline: smem operand ring (full/empty mbarriers, 3..8 stages depending on BN).
+//                         the others (setmaxnreg).
+//   warpgroups 1, 2     : MMA -- warpgroup g owns accumulator rows [64 g, 64 g + 64) of the tile: 4 x wgmma m64nBNk16
+//                         per K block, one K block kept in flight; then the accumulator goes to the fp32 staging buffer
+//                         (128 x BN, XOR-swizzled) and the warpgroup starts the next tile's K loop.
+//   warpgroup 3         : epilogue -- one thread per accumulator row finishes whole 32-column runs of the staged tile:
+//                         bias / time-embedding / residual / GEGLU / GELU (five template variants) -> fp16 -> 16-byte
+//                         global stores, while the MMA warpgroups already run the next tile.
+// Pipeline: smem operand ring (full/empty mbarriers, 3..6 stages depending on BN); one staging buffer handed over by
+// acc_full (8 MMA warps arrive) / acc_empty (4 epilogue warps arrive), whose phases flip once per tile.
+// BN = 256: 384 threads, no epilogue warpgroup; the MMA warpgroups finish their own rows through padded fp32 slices
+// (inline_epilogue_tile) with the same per-run code (finish_run).
 #include "conv_gemm.cuh"
 
 #include <dlfcn.h>
@@ -25,15 +29,33 @@
 
 namespace mvb {
 
-static constexpr int kMaxStages = 8;   // ring depth is chosen per launch: as many (16 KB A + BN x 128 B) stages as fit
+static constexpr int kMaxStages = 8;   // ring depth is chosen per tile width: as many (16 KB A + BN x 128 B) stages as fit
 static constexpr int kBlockM = 128;
 static constexpr int kBlockK = 64;
 static constexpr int kABytes = kBlockM * kBlockK * 2;        // 16 KB
-static constexpr int kAccLd = 132;                            // fp32 accumulator slice row stride (conflict-free float4 reads)
-static constexpr int kAccBytes = 2 * 64 * kAccLd * 4;         // per consumer warpgroup: 64 rows x 128 columns
-static constexpr int kBiasBytes = 2 * 256 * 4;                // per consumer warpgroup: the bias of the tile's columns
-static constexpr int kRingBytes = 227 * 1024 - kAccBytes - kBiasBytes - 1024 /*align*/ - 256 /*barriers*/;
-static constexpr int kSmemBytes = kRingBytes + kAccBytes + kBiasBytes + 1024 + 256;
+static constexpr int kSmemBytes = 227 * 1024;
+// Tiles up to 160 columns hand the accumulator to an epilogue warpgroup through one staging buffer. A 256-column
+// tile's staging buffer would take 128 KB and leave the operand ring 2 stages, so BN = 256 keeps the epilogue in the
+// MMA warpgroups, each through its own padded 64-row x 128-column fp32 slice.
+constexpr bool inline_epilogue(int bn) { return bn == 256; }
+constexpr int conv_threads(int bn) { return inline_epilogue(bn) ? 384 : 512; }
+static constexpr int kMaxStagedN = 160;                        // the widest tile with the epilogue warpgroup
+static constexpr int kStagingBytes = kBlockM * kMaxStagedN * 4;   // the fp32 accumulator tile handed to the epilogue warpgroup
+static constexpr int kAccLd = 132;                             // in-line epilogue: fp32 slice row stride (conflict-free float4 reads)
+static constexpr int kAccBytes = 2 * 64 * kAccLd * 4;          // in-line epilogue: per MMA warpgroup 64 rows x 128 columns
+// the accumulator buffer (staging or the two slices) and the bias of the tile's columns (one copy, or one per warpgroup)
+constexpr int epi_buf_bytes(int bn) { return inline_epilogue(bn) ? kAccBytes : kStagingBytes; }
+constexpr int bias_buf_bytes(int bn) { return inline_epilogue(bn) ? 2 * 256 * 4 : kMaxStagedN * 4; }
+constexpr int ring_bytes(int bn) { return kSmemBytes - epi_buf_bytes(bn) - bias_buf_bytes(bn) - 1024 /*align*/ - 256 /*barriers*/; }
+// one ring stage: the A tile and the weight tile, rounded up to the 1 KB swizzle period
+constexpr int ring_stage_bytes(int bn) { return kABytes + (bn * kBlockK * 2 + 1023) / 1024 * 1024; }
+constexpr int ring_stages(int bn) {
+  return ring_bytes(bn) / ring_stage_bytes(bn) < kMaxStages ? ring_bytes(bn) / ring_stage_bytes(bn) : kMaxStages;
+}
+// 227 KB = 80 KB staging + 640 B bias + 1 KB alignment + 256 B barriers + the ring: 6 / 4 / 4 stages at BN 64 / 128 / 160;
+// at BN 256: 66 KB of slices + 2 KB bias + 1 KB + 256 B + the ring: 3 stages
+static_assert(ring_stages(64) == 6 && ring_stages(128) == 4 && ring_stages(160) == 4 && ring_stages(256) == 3,
+              "shared-memory budget per tile width");
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
 __device__ __forceinline__ float silu(float x) { return __fdividef(x, 1.f + __expf(-x)); }
 // exact-erf GELU (diffusers activations.py:89-102 uses F.gelu default) with erf from Abramowitz-Stegun 7.1.26
@@ -101,17 +123,269 @@ struct AMaps {
   CUtensorMap m[4];   // activation views: [0] source 0, [1] skip-concat source / stride-2 phases 1..3
 };
 
+// One 32-column output run of one row: accumulator columns [c0, c0 + 32) (GEGLU: [c0, c0 + 64)), read by ld32(col, v);
+// bias / time-embedding / residual / GEGLU / GELU -> fp16 (or fp32) -> 16-byte global stores. Both epilogue placements
+// (the epilogue warpgroup, and the MMA warpgroups at BN = 256) run this, so their outputs are the same bits.
+template <int kEpi, class Ld>
+__device__ __forceinline__ void finish_run(const ConvGemmParams& p, const Ld& ld32, int c0, int ncol0, const float* sbias,
+                                           const float* radd, const uint4 (&rcur)[4], bool row_ok, bool use_res,
+                                           long long m, __half* out_row) {
+  if constexpr (kEpi != kEpiGeneric && kEpi != kEpiAct) {
+    const int nbase = ncol0 + c0;
+    uint32_t v[32], vg[32];
+    ld32(c0, v);
+    if constexpr (kEpi == kEpiGeglu) ld32(c0 + 32, vg);
+    if (nbase < p.N && row_ok) {
+      const F2 alpha2 = f2_make(p.alpha, p.alpha);
+      const float* cbias = sbias + c0;           // this chunk's bias
+      const int oc = (kEpi == kEpiGeglu) ? nbase / 2 : nbase;
+#pragma unroll
+      for (int g = 0; g < 4; ++g) {      // 8 output columns = one 16-byte store
+        uint32_t o[4];
+        if constexpr (kEpi == kEpiGeglu) {
+          // output columns 8g..8g+7 of this chunk: accumulator block g/2 (va | vb), value j, gate 16 + j
+          const uint32_t* vv = (g < 2) ? v : vg;
+          const int j0 = (g & 1) * 8;
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int j = j0 + 2 * e;
+            // this chunk's 64 accumulator columns start at cbias; block g/2 holds [16 value | 16 gate]
+            const float2 bv = *reinterpret_cast<const float2*>(cbias + (g >> 1) * 32 + j);
+            const float2 bg = *reinterpret_cast<const float2*>(cbias + (g >> 1) * 32 + 16 + j);
+            const F2 val = f2_add(f2_make(__uint_as_float(vv[j]), __uint_as_float(vv[j + 1])), f2_make(bv.x, bv.y));
+            const F2 gat = f2_add(f2_make(__uint_as_float(vv[16 + j]), __uint_as_float(vv[16 + j + 1])),
+                                  f2_make(bg.x, bg.y));
+            float x0, x1;
+            f2_get(geglu2(val, gat), x0, x1);
+            const __half2 h2 = __floats2half2_rn(x0, x1);
+            o[e] = *reinterpret_cast<const uint32_t*>(&h2);
+          }
+        } else {
+          float4 b0 = *reinterpret_cast<const float4*>(cbias + 8 * g);
+          float4 b1 = *reinterpret_cast<const float4*>(cbias + 8 * g + 4);
+          if (radd) {
+            const float4 a0 = __ldg(reinterpret_cast<const float4*>(radd + nbase) + 2 * g);
+            const float4 a1 = __ldg(reinterpret_cast<const float4*>(radd + nbase) + 2 * g + 1);
+            b0.x += a0.x; b0.y += a0.y; b0.z += a0.z; b0.w += a0.w;
+            b1.x += a1.x; b1.y += a1.y; b1.z += a1.z; b1.w += a1.w;
+          }
+          const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+          const __half2* rh2 = reinterpret_cast<const __half2*>(&rcur[g]);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int j = g * 8 + 2 * e;
+            F2 x = f2_add(f2_make(__uint_as_float(v[j]), __uint_as_float(v[j + 1])), f2_make(bb[2 * e], bb[2 * e + 1]));
+            if constexpr (kEpi == kEpiResidual) {
+              const float2 rr = __half22float2(rh2[e]);
+              x = f2_fma(x, alpha2, f2_make(rr.x, rr.y));
+            }
+            float x0, x1;
+            f2_get(x, x0, x1);
+            const __half2 h2 = __floats2half2_rn(x0, x1);
+            o[e] = *reinterpret_cast<const uint32_t*>(&h2);
+          }
+        }
+        *reinterpret_cast<uint4*>(out_row + oc + 8 * g) = make_uint4(o[0], o[1], o[2], o[3]);
+      }
+    }
+  } else {
+    // accumulator -> f[32] = the 32 output columns of this chunk, bias / row-add applied
+    float f[32];
+    const int nbase = ncol0 + c0;
+    if (p.geglu) {
+      uint32_t va[32], vb[32];
+      ld32(c0, va);
+      ld32(c0 + 32, vb);
+      // packed columns: [16 value | 16 gate] per 32 accumulator columns
+#pragma unroll
+      for (int hsel = 0; hsel < 2; ++hsel) {
+        const uint32_t* v = hsel ? vb : va;
+        const int nb = nbase + hsel * 32;
+#pragma unroll
+        for (int j4 = 0; j4 < 4; ++j4) {
+          // bias of 4 value columns and their 4 gate columns (nb is a multiple of 32: 16-byte aligned float4)
+          const bool bok = p.bias && nb < p.N;
+          const float4 bv = bok ? __ldg(reinterpret_cast<const float4*>(p.bias + nb) + j4) : make_float4(0, 0, 0, 0);
+          const float4 bg = bok ? __ldg(reinterpret_cast<const float4*>(p.bias + nb + 16) + j4) : make_float4(0, 0, 0, 0);
+          const int j = j4 * 4;
+          const F2 v01 = f2_add(f2_make(__uint_as_float(v[j]), __uint_as_float(v[j + 1])), f2_make(bv.x, bv.y));
+          const F2 v23 = f2_add(f2_make(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3])), f2_make(bv.z, bv.w));
+          const F2 g01 = f2_add(f2_make(__uint_as_float(v[16 + j]), __uint_as_float(v[16 + j + 1])), f2_make(bg.x, bg.y));
+          const F2 g23 = f2_add(f2_make(__uint_as_float(v[16 + j + 2]), __uint_as_float(v[16 + j + 3])), f2_make(bg.z, bg.w));
+          f2_get(geglu2(v01, g01), f[hsel * 16 + j], f[hsel * 16 + j + 1]);
+          f2_get(geglu2(v23, g23), f[hsel * 16 + j + 2], f[hsel * 16 + j + 3]);
+        }
+      }
+    } else {
+      uint32_t v[32];
+      ld32(c0, v);      // BN is a multiple of 32
+      if (nbase + 32 <= p.N) {
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+          float4 b = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + nbase) + g) : make_float4(0, 0, 0, 0);
+          if (radd) {
+            const float4 a4 = __ldg(reinterpret_cast<const float4*>(radd + nbase) + g);
+            b.x += a4.x; b.y += a4.y; b.z += a4.z; b.w += a4.w;
+          }
+          f[g * 4 + 0] = __uint_as_float(v[g * 4 + 0]) + b.x;
+          f[g * 4 + 1] = __uint_as_float(v[g * 4 + 1]) + b.y;
+          f[g * 4 + 2] = __uint_as_float(v[g * 4 + 2]) + b.z;
+          f[g * 4 + 3] = __uint_as_float(v[g * 4 + 3]) + b.w;
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const int nn = nbase + j;
+          float x = __uint_as_float(v[j]);
+          if (nn < p.N) {
+            if (p.bias) x += __ldg(p.bias + nn);
+            if (radd) x += __ldg(radd + nn);
+          }
+          f[j] = x;
+        }
+      }
+    }
+    if (row_ok) {
+      if (p.out_f32) {
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+          const int nn = nbase + g * 4;
+          if (nn < p.N) {
+            float4 o4;
+            o4.x = f[g * 4 + 0] * p.alpha; o4.y = f[g * 4 + 1] * p.alpha;
+            o4.z = f[g * 4 + 2] * p.alpha; o4.w = f[g * 4 + 3] * p.alpha;
+            if (p.act == 1) { o4.x = silu(o4.x); o4.y = silu(o4.y); o4.z = silu(o4.z); o4.w = silu(o4.w); }
+            if constexpr (kEpi == kEpiAct) {
+              o4.x = gelu_act(o4.x, p.act); o4.y = gelu_act(o4.y, p.act);
+              o4.z = gelu_act(o4.z, p.act); o4.w = gelu_act(o4.w, p.act);
+            }
+            *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + m * p.ldc + nn) = o4;
+          }
+        }
+      } else {
+        // finish in fp32, round to fp16, store 8 columns at a time
+        const int oc = p.geglu ? nbase / 2 : nbase;
+        const int ncols = p.geglu ? p.N / 2 : p.N;
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          if (oc + 8 * g >= ncols) continue;
+          __align__(16) __half o[8];
+          const __half* rh8 = reinterpret_cast<const __half*>(&rcur[g]);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            float x = f[g * 8 + j];
+            if (!p.geglu) {
+              x *= p.alpha;
+              if (use_res) x = fmaf(p.beta, __half2float(rh8[j]), x);
+              if (p.act == 1) x = silu(x);
+              if constexpr (kEpi == kEpiAct) x = gelu_act(x, p.act);
+            }
+            o[j] = __float2half_rn(x);
+          }
+          *reinterpret_cast<uint4*>(out_row + oc + 8 * g) = *reinterpret_cast<const uint4*>(o);
+        }
+      }
+    }
+  }
+}
+
+// In-line epilogue of one tile (BN = 256): MMA warpgroup wg finishes its own 64 accumulator rows. The accumulator goes
+// through the warpgroup's padded fp32 slice 128 columns at a time; thread t takes row t % 64 and, with the other half
+// of the warpgroup, alternating 32-column runs.
 template <int kEpi, int BN>
-__global__ void __launch_bounds__(384, 1)
+__device__ __forceinline__ void inline_epilogue_tile(const ConvGemmParams& p, const float (&acc)[BN / 2], float* sacc,
+                                                     float* sbias, int unit, int wg, int t) {
+  const int lane = t & 31;
+  const int wq = t >> 5;
+  const int row_local = t & 63;
+  const int half = t >> 6;
+  const int r = 64 * wg + row_local;
+  float* acc_slice = sacc + wg * 64 * kAccLd;
+  float* wbias = sbias + wg * 256;
+  const bool use_res = (p.res != nullptr) && !p.geglu && !p.out_f32;
+  const int acc_step = p.geglu ? 64 : 32;             // accumulator columns consumed per 32 output columns
+  const int nt = unit % p.tiles_nn;
+  const int mt = unit / p.tiles_nn;
+  const int tw = mt % p.tiles_w;
+  const int th = (mt / p.tiles_w) % p.tiles_h;
+  const int tn = mt / (p.tiles_w * p.tiles_h);
+  const int ncol0 = nt * BN;
+  const int rw = r % p.bw;
+  const int rh = (r / p.bw) % p.bh;
+  const int rn = r / (p.bw * p.bh);
+  const int w = tw * p.bw + rw, h = th * p.bh + rh, n = tn * p.bn + rn;
+  const bool row_ok = (w < p.W) && (h < p.H) && (n < p.NF);
+  const long long m = ((long long)n * p.H + h) * p.W + w;
+  const float* radd = (p.rowadd && row_ok) ? p.rowadd + (long long)(m / p.rows_per_group) * p.ld_rowadd : nullptr;
+  const __half* res_row = use_res ? p.res + m * p.ld_res : nullptr;
+  __half* out_row = reinterpret_cast<__half*>(p.out) + m * p.ldc;
+
+  uint4 rcur[4] = {};
+  auto load_res = [&](int c0) {
+    if (!use_res || !row_ok) return;
+#pragma unroll
+    for (int g = 0; g < 4; ++g) {
+      const int nn = ncol0 + c0 + g * 8;
+      if (c0 + g * 8 < BN && nn < p.N) rcur[g] = __ldg(reinterpret_cast<const uint4*>(res_row + nn));
+    }
+  };
+  named_bar_sync(1 + wg, 128);                      // the previous tile's reads of the bias / accumulator slices are done
+  if constexpr (kEpi != kEpiGeneric && kEpi != kEpiAct) {
+    for (int c = t; c < BN; c += 128) wbias[c] = (p.bias && ncol0 + c < p.N) ? __ldg(p.bias + ncol0 + c) : 0.f;
+  }
+#pragma unroll
+  for (int u = 0; u < (BN + 127) / 128; ++u) {
+    if (u > 0) named_bar_sync(1 + wg, 128);         // previous slice consumed
+    // accumulator fragment (rows 16 wq + lane/4 (+8), columns 8 i + 2 (lane%4)) -> fp32 slice, columns [128 u, 128 u + 128)
+#pragma unroll
+    for (int i = 16 * u; i < 16 * u + 16 && i < BN / 8; ++i) {
+      const int rr = 16 * wq + (lane >> 2);
+      const int cc = 8 * (i - 16 * u) + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(acc_slice + rr * kAccLd + cc) = make_float2(acc[4 * i], acc[4 * i + 1]);
+      *reinterpret_cast<float2*>(acc_slice + (rr + 8) * kAccLd + cc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+    }
+    named_bar_sync(1 + wg, 128);
+    const int cend = (128 * u + 128 < BN) ? 128 * u + 128 : BN;
+    for (int c0 = 128 * u + half * acc_step; c0 < cend; c0 += 2 * acc_step) {
+      const float* srow = acc_slice + row_local * kAccLd - 128 * u;
+      auto ld32 = [&](int col, uint32_t (&v)[32]) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float4 x = *reinterpret_cast<const float4*>(srow + col + 4 * k);
+          v[4 * k] = __float_as_uint(x.x); v[4 * k + 1] = __float_as_uint(x.y);
+          v[4 * k + 2] = __float_as_uint(x.z); v[4 * k + 3] = __float_as_uint(x.w);
+        }
+      };
+      load_res(c0);
+      finish_run<kEpi>(p, ld32, c0, ncol0, wbias, radd, rcur, row_ok, use_res, m, out_row);
+    }
+  }
+}
+
+template <int kEpi, int BN>
+__global__ void __launch_bounds__(conv_threads(BN), 1)
 conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ ConvGemmParams p) {
+  constexpr bool kInline = inline_epilogue(BN);
+  static_assert(BN % 32 == 0 && (BN <= kMaxStagedN || kInline), "the staging swizzle and the epilogue take whole 32-column runs");
+  // the producer gives its registers away; an MMA thread holds BN / 2 accumulators (and, in line, runs the epilogue),
+  // an epilogue thread one row's 32- or 64-column run plus the next run's residual
+  constexpr int kProducerRegs = 40, kConsumerRegs = kInline ? 232 : 152, kEpilogueRegs = kInline ? 0 : 168;
+  static_assert(128 * (kProducerRegs + kEpilogueRegs) + 256 * kConsumerRegs <= 65536,
+                "setmaxnreg split exceeds the register file");
+  constexpr int kRingBytes = ring_bytes(BN);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* sacc = reinterpret_cast<float*>(smem + kRingBytes);               // [2 warpgroups][64][kAccLd]
-  float* sbias = reinterpret_cast<float*>(smem + kRingBytes + kAccBytes);  // [2 warpgroups][256]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes + kAccBytes + kBiasBytes);
+  // staging: [128 rows][BN] fp32; 16-byte chunk j of row r sits at chunk j ^ (r & 7), so that both the fragment writes
+  // (8 rows x 2 chunks per warp store) and the row reads (32 rows, one chunk each) are free of bank conflicts.
+  // In line (BN = 256): [2 warpgroups][64][kAccLd] slices.
+  float* stg = reinterpret_cast<float*>(smem + kRingBytes);
+  float* sbias = reinterpret_cast<float*>(smem + kRingBytes + epi_buf_bytes(BN));  // [BN], in line [2 warpgroups][256]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes + epi_buf_bytes(BN) + bias_buf_bytes(BN));
   uint64_t* full = bars;                       // [kMaxStages]
   uint64_t* empty = bars + kMaxStages;         // [kMaxStages]
+  uint64_t* acc_full = bars + 2 * kMaxStages;  // the staging holds a finished tile
+  uint64_t* acc_empty = acc_full + 1;          // the epilogue has read it
   const int nstages = p.nstages;
   const int stage_bytes = p.stage_bytes;
 
@@ -128,6 +402,8 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 8);                 // one arrival per consumer warp
     }
+    mbar_init(acc_full, 8);                    // one arrival per consumer warp
+    mbar_init(acc_empty, 4);                   // one arrival per epilogue warp
     fence_barrier_init();
   }
   __syncthreads();
@@ -139,7 +415,7 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
   const uint32_t stage_tx = kABytes + (uint32_t)BN * kBlockK * 2;
 
   if (warp < 4) {
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<kProducerRegs>();
     if (warp == 0) {
       // TMA producer: warp-uniform loop, one elected lane issues the copies of a stage
       int stage = 0;
@@ -178,33 +454,94 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
     return;
   }
 
-  setmaxnreg_inc<232>();
-  const int wg = (warp - 4) >> 2;                 // accumulator rows [64 wg, 64 wg + 64)
+  if (!kInline && warp >= 12) {
+    // ---- epilogue warpgroup: finishes tile i from the staging while the consumers run tile i + 1's K loop.
+    // Thread r owns accumulator row r and walks its 32-column runs: bias / time-embedding / residual / GEGLU / GELU
+    // (five template variants) -> fp16 -> 16-byte global stores.
+    setmaxnreg_inc<kEpilogueRegs>();
+    const int r = threadIdx.x - 384;
+    const float* srow = stg + r * BN;
+    const int sw = r & 7;
+    const bool use_res = (p.res != nullptr) && !p.geglu && !p.out_f32;
+    const int acc_step = p.geglu ? 64 : 32;             // accumulator columns consumed per 32 output columns
+    uint32_t acc_phase = 0;
+    for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+      const int nt = unit % p.tiles_nn;
+      const int mt = unit / p.tiles_nn;
+      const int tw = mt % p.tiles_w;
+      const int th = (mt / p.tiles_w) % p.tiles_h;
+      const int tn = mt / (p.tiles_w * p.tiles_h);
+      const int ncol0 = nt * BN;
+      const int rw = r % p.bw;
+      const int rh = (r / p.bw) % p.bh;
+      const int rn = r / (p.bw * p.bh);
+      const int w = tw * p.bw + rw, h = th * p.bh + rh, n = tn * p.bn + rn;
+      const bool row_ok = (w < p.W) && (h < p.H) && (n < p.NF);
+      const long long m = ((long long)n * p.H + h) * p.W + w;
+      const float* radd = (p.rowadd && row_ok) ? p.rowadd + (long long)(m / p.rows_per_group) * p.ld_rowadd : nullptr;
+      const __half* res_row = use_res ? p.res + m * p.ld_res : nullptr;
+      __half* out_row = reinterpret_cast<__half*>(p.out) + m * p.ldc;
+
+      uint4 rcur[4] = {}, rnext[4] = {};    // residual of this run / the next one
+      auto load_res = [&](int c0, uint4 (&dst)[4]) {
+        if (!use_res || !row_ok) return;
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          const int nn = ncol0 + c0 + g * 8;
+          if (c0 + g * 8 < BN && nn < p.N) dst[g] = __ldg(reinterpret_cast<const uint4*>(res_row + nn));
+        }
+      };
+      // what the tile needs besides the accumulator is fetched while its K loop still runs
+      if constexpr (kEpi != kEpiGeneric && kEpi != kEpiAct) {
+        named_bar_sync(1, 128);                         // every epilogue warp is done with the previous tile's bias
+        for (int c = r; c < BN; c += 128) sbias[c] = (p.bias && ncol0 + c < p.N) ? __ldg(p.bias + ncol0 + c) : 0.f;
+        named_bar_sync(1, 128);
+      }
+      load_res(0, rcur);
+      mbar_wait(acc_full, acc_phase);
+      for (int c0 = 0; c0 < BN; c0 += acc_step) {
+        // the residual variant loads the next run's residual ahead; the generic ones, short of registers, this run's
+        if constexpr (kEpi == kEpiResidual) load_res(c0 + acc_step, rnext);
+        else if (c0 > 0) load_res(c0, rcur);
+        // accumulator columns [col, col + 32) of row r (col is a multiple of 32: the swizzle stays inside the run)
+        auto ld32 = [&](int col, uint32_t (&v)[32]) {
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            const float4 x = *reinterpret_cast<const float4*>(srow + col + 4 * (k ^ sw));
+            v[4 * k] = __float_as_uint(x.x); v[4 * k + 1] = __float_as_uint(x.y);
+            v[4 * k + 2] = __float_as_uint(x.z); v[4 * k + 3] = __float_as_uint(x.w);
+          }
+        };
+        finish_run<kEpi>(p, ld32, c0, ncol0, sbias, radd, rcur, row_ok, use_res, m, out_row);
+        if constexpr (kEpi == kEpiResidual) {
+#pragma unroll
+          for (int g = 0; g < 4; ++g) rcur[g] = rnext[g];
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(acc_empty);
+      acc_phase ^= 1;
+    }
+    return;
+  }
+
+  // ---- MMA warpgroups 1, 2: warpgroup g owns accumulator rows [64 g, 64 g + 64) of the tile
+  setmaxnreg_inc<kConsumerRegs>();
+  const int wg = (warp - 4) >> 2;
   const int t = threadIdx.x - 128 * (1 + wg);     // thread in the warpgroup
   const int wq = t >> 5;
-  // epilogue mapping: one accumulator row per thread, the two halves of the warpgroup take alternating column chunks
-  const int row_local = t & 63;
-  const int half = t >> 6;
-  const int r = 64 * wg + row_local;
-  float* acc_slice = sacc + wg * 64 * kAccLd;
-  float* wbias = sbias + wg * 256;
-  const bool use_res = (p.res != nullptr) && !p.geglu && !p.out_f32;
-  const int acc_step = p.geglu ? 64 : 32;             // accumulator columns consumed per 32 output columns
   const uint64_t desc0_a = make_desc_k_sw128(smem_u32(smem) + (uint32_t)wg * 64 * 128);
   const uint64_t desc0_b = make_desc_k_sw128(smem_u32(smem) + kABytes);
   const uint32_t stage_step = (uint32_t)stage_bytes >> 4;     // descriptor address field counts 16-byte units
+  // fragment rows 16 wq + lane / 4 and + 8 of this warpgroup's 64 (both have row & 7 == lane / 4), column pairs
+  // 8 i + 2 (lane % 4) = chunk 2 i + (lane % 4) / 2, offset 2 (lane % 2) inside it
+  float* stg_row = stg + (64 * wg + 16 * wq + (lane >> 2)) * BN;
   int stage = 0;
   uint32_t phase = 0;
+  uint32_t acc_phase = 0;
   float acc[BN / 2];
 
   for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
-    const int nt = unit % p.tiles_nn;
-    const int mt = unit / p.tiles_nn;
-    const int tw = mt % p.tiles_w;
-    const int th = (mt / p.tiles_w) % p.tiles_h;
-    const int tn = mt / (p.tiles_w * p.tiles_h);
-    const int ncol0 = nt * BN;
-
     // ---- mainloop: one K block (4 wgmma) in flight while the next is issued
     int prev_stage = 0;
     for (int kb = 0; kb < num_kb; ++kb) {
@@ -232,212 +569,20 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[prev_stage]);
 
-    // ---- epilogue
-    const int rw = r % p.bw;
-    const int rh = (r / p.bw) % p.bh;
-    const int rn = r / (p.bw * p.bh);
-    const int w = tw * p.bw + rw, h = th * p.bh + rh, n = tn * p.bn + rn;
-    const bool row_ok = (w < p.W) && (h < p.H) && (n < p.NF);
-    const long long m = ((long long)n * p.H + h) * p.W + w;
-    const float* radd = (p.rowadd && row_ok) ? p.rowadd + (long long)(m / p.rows_per_group) * p.ld_rowadd : nullptr;
-    const __half* res_row = use_res ? p.res + m * p.ld_res : nullptr;
-    __half* out_row = reinterpret_cast<__half*>(p.out) + m * p.ldc;
-
-    uint4 rcur[4] = {};
-    auto load_res = [&](int c0, uint4 (&dst)[4]) {
-      if (!use_res || !row_ok) return;
+    if constexpr (kInline) {
+      inline_epilogue_tile<kEpi, BN>(p, acc, stg, sbias, unit, wg, t);
+    } else {
+      // ---- hand the tile to the epilogue warpgroup once it has read the previous one, then go on to the next tile
+      mbar_wait(acc_empty, acc_phase ^ 1);
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const int nn = ncol0 + c0 + g * 8;
-        if (c0 + g * 8 < BN && nn < p.N) dst[g] = __ldg(reinterpret_cast<const uint4*>(res_row + nn));
+      for (int i = 0; i < BN / 8; ++i) {
+        const int off = 4 * ((2 * i + ((lane & 3) >> 1)) ^ (lane >> 2)) + 2 * (lane & 1);
+        *reinterpret_cast<float2*>(stg_row + off) = make_float2(acc[4 * i], acc[4 * i + 1]);
+        *reinterpret_cast<float2*>(stg_row + 8 * BN + off) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
       }
-    };
-    named_bar_sync(1 + wg, 128);                      // the previous tile's reads of the bias / accumulator slices are done
-    if constexpr (kEpi != kEpiGeneric && kEpi != kEpiAct) {
-      for (int c = t; c < BN; c += 128) wbias[c] = (p.bias && ncol0 + c < p.N) ? __ldg(p.bias + ncol0 + c) : 0.f;
-    }
-#pragma unroll
-    for (int u = 0; u < (BN + 127) / 128; ++u) {
-      if (u > 0) named_bar_sync(1 + wg, 128);         // previous slice consumed
-      // accumulator fragment (rows 16 wq + lane/4 (+8), columns 8 i + 2 (lane%4)) -> fp32 slice, columns [128 u, 128 u + 128)
-#pragma unroll
-      for (int i = 16 * u; i < 16 * u + 16 && i < BN / 8; ++i) {
-        const int rr = 16 * wq + (lane >> 2);
-        const int cc = 8 * (i - 16 * u) + 2 * (lane & 3);
-        *reinterpret_cast<float2*>(acc_slice + rr * kAccLd + cc) = make_float2(acc[4 * i], acc[4 * i + 1]);
-        *reinterpret_cast<float2*>(acc_slice + (rr + 8) * kAccLd + cc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
-      }
-      named_bar_sync(1 + wg, 128);
-      const int cend = (128 * u + 128 < BN) ? 128 * u + 128 : BN;
-      for (int c0 = 128 * u + half * acc_step; c0 < cend; c0 += 2 * acc_step) {
-        const float* srow = acc_slice + row_local * kAccLd + (c0 - 128 * u);
-        auto ld32 = [&](const float* src, uint32_t (&v)[32]) {
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const float4 x = *reinterpret_cast<const float4*>(src + 4 * k);
-            v[4 * k] = __float_as_uint(x.x); v[4 * k + 1] = __float_as_uint(x.y);
-            v[4 * k + 2] = __float_as_uint(x.z); v[4 * k + 3] = __float_as_uint(x.w);
-          }
-        };
-        load_res(c0, rcur);
-        if constexpr (kEpi != kEpiGeneric && kEpi != kEpiAct) {
-          const int nbase = ncol0 + c0;
-          uint32_t v[32], vg[32];
-          ld32(srow, v);
-          if constexpr (kEpi == kEpiGeglu) ld32(srow + 32, vg);
-          if (nbase < p.N && row_ok) {
-            const F2 alpha2 = f2_make(p.alpha, p.alpha);
-            const float* cbias = wbias + c0;           // this chunk's bias
-            const int oc = (kEpi == kEpiGeglu) ? nbase / 2 : nbase;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {      // 8 output columns = one 16-byte store
-              uint32_t o[4];
-              if constexpr (kEpi == kEpiGeglu) {
-                // output columns 8g..8g+7 of this chunk: accumulator block g/2 (va | vb), value j, gate 16 + j
-                const uint32_t* vv = (g < 2) ? v : vg;
-                const int j0 = (g & 1) * 8;
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const int j = j0 + 2 * e;
-                  // this chunk's 64 accumulator columns start at cbias; block g/2 holds [16 value | 16 gate]
-                  const float2 bv = *reinterpret_cast<const float2*>(cbias + (g >> 1) * 32 + j);
-                  const float2 bg = *reinterpret_cast<const float2*>(cbias + (g >> 1) * 32 + 16 + j);
-                  const F2 val = f2_add(f2_make(__uint_as_float(vv[j]), __uint_as_float(vv[j + 1])), f2_make(bv.x, bv.y));
-                  const F2 gat = f2_add(f2_make(__uint_as_float(vv[16 + j]), __uint_as_float(vv[16 + j + 1])),
-                                        f2_make(bg.x, bg.y));
-                  float x0, x1;
-                  f2_get(geglu2(val, gat), x0, x1);
-                  const __half2 h2 = __floats2half2_rn(x0, x1);
-                  o[e] = *reinterpret_cast<const uint32_t*>(&h2);
-                }
-              } else {
-                float4 b0 = *reinterpret_cast<const float4*>(cbias + 8 * g);
-                float4 b1 = *reinterpret_cast<const float4*>(cbias + 8 * g + 4);
-                if (radd) {
-                  const float4 a0 = __ldg(reinterpret_cast<const float4*>(radd + nbase) + 2 * g);
-                  const float4 a1 = __ldg(reinterpret_cast<const float4*>(radd + nbase) + 2 * g + 1);
-                  b0.x += a0.x; b0.y += a0.y; b0.z += a0.z; b0.w += a0.w;
-                  b1.x += a1.x; b1.y += a1.y; b1.z += a1.z; b1.w += a1.w;
-                }
-                const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                const __half2* rh2 = reinterpret_cast<const __half2*>(&rcur[g]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const int j = g * 8 + 2 * e;
-                  F2 x = f2_add(f2_make(__uint_as_float(v[j]), __uint_as_float(v[j + 1])), f2_make(bb[2 * e], bb[2 * e + 1]));
-                  if constexpr (kEpi == kEpiResidual) {
-                    const float2 rr = __half22float2(rh2[e]);
-                    x = f2_fma(x, alpha2, f2_make(rr.x, rr.y));
-                  }
-                  float x0, x1;
-                  f2_get(x, x0, x1);
-                  const __half2 h2 = __floats2half2_rn(x0, x1);
-                  o[e] = *reinterpret_cast<const uint32_t*>(&h2);
-                }
-              }
-              *reinterpret_cast<uint4*>(out_row + oc + 8 * g) = make_uint4(o[0], o[1], o[2], o[3]);
-            }
-          }
-        } else {
-          // accumulator -> f[32] = the 32 output columns of this chunk, bias / row-add applied
-          float f[32];
-          const int nbase = ncol0 + c0;
-          if (p.geglu) {
-            uint32_t va[32], vb[32];
-            ld32(srow, va);
-            ld32(srow + 32, vb);
-            // packed columns: [16 value | 16 gate] per 32 accumulator columns
-#pragma unroll
-            for (int hsel = 0; hsel < 2; ++hsel) {
-              const uint32_t* v = hsel ? vb : va;
-              const int nb = nbase + hsel * 32;
-#pragma unroll
-              for (int j4 = 0; j4 < 4; ++j4) {
-                // bias of 4 value columns and their 4 gate columns (nb is a multiple of 32: 16-byte aligned float4)
-                const bool bok = p.bias && nb < p.N;
-                const float4 bv = bok ? __ldg(reinterpret_cast<const float4*>(p.bias + nb) + j4) : make_float4(0, 0, 0, 0);
-                const float4 bg = bok ? __ldg(reinterpret_cast<const float4*>(p.bias + nb + 16) + j4) : make_float4(0, 0, 0, 0);
-                const int j = j4 * 4;
-                const F2 v01 = f2_add(f2_make(__uint_as_float(v[j]), __uint_as_float(v[j + 1])), f2_make(bv.x, bv.y));
-                const F2 v23 = f2_add(f2_make(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3])), f2_make(bv.z, bv.w));
-                const F2 g01 = f2_add(f2_make(__uint_as_float(v[16 + j]), __uint_as_float(v[16 + j + 1])), f2_make(bg.x, bg.y));
-                const F2 g23 = f2_add(f2_make(__uint_as_float(v[16 + j + 2]), __uint_as_float(v[16 + j + 3])), f2_make(bg.z, bg.w));
-                f2_get(geglu2(v01, g01), f[hsel * 16 + j], f[hsel * 16 + j + 1]);
-                f2_get(geglu2(v23, g23), f[hsel * 16 + j + 2], f[hsel * 16 + j + 3]);
-              }
-            }
-          } else {
-            uint32_t v[32];
-            ld32(srow, v);      // BN is a multiple of 32
-            if (nbase + 32 <= p.N) {
-#pragma unroll
-              for (int g = 0; g < 8; ++g) {
-                float4 b = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + nbase) + g) : make_float4(0, 0, 0, 0);
-                if (radd) {
-                  const float4 a4 = __ldg(reinterpret_cast<const float4*>(radd + nbase) + g);
-                  b.x += a4.x; b.y += a4.y; b.z += a4.z; b.w += a4.w;
-                }
-                f[g * 4 + 0] = __uint_as_float(v[g * 4 + 0]) + b.x;
-                f[g * 4 + 1] = __uint_as_float(v[g * 4 + 1]) + b.y;
-                f[g * 4 + 2] = __uint_as_float(v[g * 4 + 2]) + b.z;
-                f[g * 4 + 3] = __uint_as_float(v[g * 4 + 3]) + b.w;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const int nn = nbase + j;
-                float x = __uint_as_float(v[j]);
-                if (nn < p.N) {
-                  if (p.bias) x += __ldg(p.bias + nn);
-                  if (radd) x += __ldg(radd + nn);
-                }
-                f[j] = x;
-              }
-            }
-          }
-          if (row_ok) {
-            if (p.out_f32) {
-#pragma unroll
-              for (int g = 0; g < 8; ++g) {
-                const int nn = nbase + g * 4;
-                if (nn < p.N) {
-                  float4 o4;
-                  o4.x = f[g * 4 + 0] * p.alpha; o4.y = f[g * 4 + 1] * p.alpha;
-                  o4.z = f[g * 4 + 2] * p.alpha; o4.w = f[g * 4 + 3] * p.alpha;
-                  if (p.act == 1) { o4.x = silu(o4.x); o4.y = silu(o4.y); o4.z = silu(o4.z); o4.w = silu(o4.w); }
-                  if constexpr (kEpi == kEpiAct) {
-                    o4.x = gelu_act(o4.x, p.act); o4.y = gelu_act(o4.y, p.act);
-                    o4.z = gelu_act(o4.z, p.act); o4.w = gelu_act(o4.w, p.act);
-                  }
-                  *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + m * p.ldc + nn) = o4;
-                }
-              }
-            } else {
-              // finish in fp32, round to fp16, store 8 columns at a time
-              const int oc = p.geglu ? nbase / 2 : nbase;
-              const int ncols = p.geglu ? p.N / 2 : p.N;
-#pragma unroll
-              for (int g = 0; g < 4; ++g) {
-                if (oc + 8 * g >= ncols) continue;
-                __align__(16) __half o[8];
-                const __half* rh8 = reinterpret_cast<const __half*>(&rcur[g]);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  float x = f[g * 8 + j];
-                  if (!p.geglu) {
-                    x *= p.alpha;
-                    if (use_res) x = fmaf(p.beta, __half2float(rh8[j]), x);
-                    if (p.act == 1) x = silu(x);
-                    if constexpr (kEpi == kEpiAct) x = gelu_act(x, p.act);
-                  }
-                  o[j] = __float2half_rn(x);
-                }
-                *reinterpret_cast<uint4*>(out_row + oc + 8 * g) = *reinterpret_cast<const uint4*>(o);
-              }
-            }
-          }
-        }
-      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(acc_full);
+      acc_phase ^= 1;
     }
   }
 }
@@ -651,9 +796,8 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   int bn_idx = 0;
   while (kBlockNs[bn_idx] != p.block_n) ++bn_idx;
   p.tiles_nn = ceil_div(p.N, p.block_n);
-  p.stage_bytes = kABytes + ((p.block_n * kBlockK * 2 + 1023) / 1024) * 1024;   // B tile rounded up to the swizzle period
-  p.nstages = kRingBytes / p.stage_bytes;
-  if (p.nstages > kMaxStages) p.nstages = kMaxStages;
+  p.stage_bytes = ring_stage_bytes(p.block_n);
+  p.nstages = ring_stages(p.block_n);
   p.out = ep.out; p.ldc = ep.ldc; p.bias = ep.bias; p.rowadd = ep.rowadd;
   p.rows_per_group = ep.rows_per_group > 0 ? ep.rows_per_group : 1;
   p.ld_rowadd = ep.ld_rowadd; p.res = ep.res; p.ld_res = ep.ld_res; p.alpha = ep.alpha; p.beta = ep.beta;
@@ -681,14 +825,24 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   }
   if (gelu) epi = kEpiAct;
   static const bool trace = getenv("MVB_TRACE") != nullptr;
-  if (trace)
-    fprintf(stderr, "MVB_TRACE gemm M=%lld N=%d K=%lld taps=%d block_n=%d tiles=%lld geglu=%d res=%d f32=%d epi=%d\n",
+  if (trace) {
+    // the trailing fields describe the launch fully enough to replay it (tools/gpu_gemm_census.py): output image, the
+    // channels of each A source, tap offsets, the stride-2 pad mode (0: not a stride-2 conv) and the epilogue options
+    char taps[9 * 10 + 1];                            // up to 9 x ",-128:-128" without the leading comma
+    int len = 0;
+    for (int i = 0; i < p.ntaps; ++i) len += snprintf(taps + len, sizeof(taps) - len, "%s%d:%d", i ? "," : "", p.dy[i], p.dx[i]);
+    int s2 = 0;
+    for (int i = 0; i < p.ntaps; ++i) if (p.tap_src[i]) s2 = p.dy[0] < 0 ? 1 : 2;
+    fprintf(stderr, "MVB_TRACE gemm M=%lld N=%d K=%lld taps=%d block_n=%d tiles=%lld geglu=%d res=%d f32=%d epi=%d "
+            "W=%d H=%d NF=%d c0=%d c1=%d offsets=%s s2=%d bias=%d rowadd=%d rpg=%d alpha=%.9g beta=%.9g act=%d\n",
             (long long)p.W * p.H * p.NF, p.N, ktot, p.ntaps, p.block_n, num_tiles, p.geglu, p.res != nullptr, p.out_f32,
-            epi);
+            epi, p.W, p.H, p.NF, p.kb0 * 64, p.kb1 * 64, taps, s2, p.bias != nullptr, p.rowadd != nullptr,
+            p.rows_per_group, p.alpha, p.beta, p.act);
+  }
   AMaps am;
   for (int i = 0; i < 4; ++i) am.m[i] = maps[i < nmaps ? i : 0];
   ProfScope prof(stream, KC_GEMM);
-  kernels[bn_idx][epi]<<<grid, 384, kSmemBytes, stream>>>(am, tmB, p);
+  kernels[bn_idx][epi]<<<grid, conv_threads(p.block_n), kSmemBytes, stream>>>(am, tmB, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) *err = "conv_gemm_kernel launch";
   return e;

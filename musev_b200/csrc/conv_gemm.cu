@@ -9,10 +9,14 @@
 //                         per K block, one K block kept in flight; then the accumulator goes to the fp32 staging buffer
 //                         (128 x BN, XOR-swizzled) and the warpgroup starts the next tile's K loop.
 //   warpgroup 3         : epilogue -- one thread per accumulator row finishes whole 32-column runs of the staged tile:
-//                         bias / time-embedding / residual / GEGLU / GELU (five template variants) -> fp16 -> 16-byte
-//                         global stores, while the MMA warpgroups already run the next tile.
-// Pipeline: smem operand ring (full/empty mbarriers, 3..6 stages depending on BN); one staging buffer handed over by
-// acc_full (8 MMA warps arrive) / acc_empty (4 epilogue warps arrive), whose phases flip once per tile.
+//                         bias / time-embedding / residual / GEGLU / GELU (five template variants) -> fp16, while the
+//                         MMA warpgroups already run the next tile. The plain / residual / GEGLU variants write each
+//                         run's fp16 outputs back into its staging and store them with one TMA box; the residual
+//                         variant reads residual runs that warp 1 loads with TMA into a 4-slot ring (full/empty
+//                         mbarriers). The generic / GELU variants use 16-byte global loads and stores per thread.
+// Pipeline: smem operand ring (full/empty mbarriers, 3..8 stages depending on BN); one staging buffer handed over by
+// acc_full (8 MMA warps arrive) / acc_empty (4 epilogue warps arrive, after the tile's TMA stores have read it), whose
+// phases flip once per tile.
 // BN = 256: 384 threads, no epilogue warpgroup; the MMA warpgroups finish their own rows through padded fp32 slices
 // (inline_epilogue_tile) with the same per-run code (finish_run).
 #include "conv_gemm.cuh"
@@ -40,21 +44,47 @@ static constexpr int kSmemBytes = 227 * 1024;
 constexpr bool inline_epilogue(int bn) { return bn == 256; }
 constexpr int conv_threads(int bn) { return inline_epilogue(bn) ? 384 : 512; }
 static constexpr int kMaxStagedN = 160;                        // the widest tile with the epilogue warpgroup
-static constexpr int kStagingBytes = kBlockM * kMaxStagedN * 4;   // the fp32 accumulator tile handed to the epilogue warpgroup
+static constexpr int kRunFloats = kBlockM * 32;                // one 32-column run of the fp32 staging (16 KB)
+static constexpr int kRunBytes = kBlockM * 32 * 2;             // one 32-column run of fp16 outputs or residuals (8 KB)
+static constexpr int kResSlots = 4;                            // residual ring: 32-column runs loaded ahead of the epilogue
 static constexpr int kAccLd = 132;                             // in-line epilogue: fp32 slice row stride (conflict-free float4 reads)
 static constexpr int kAccBytes = 2 * 64 * kAccLd * 4;          // in-line epilogue: per MMA warpgroup 64 rows x 128 columns
-// the accumulator buffer (staging or the two slices) and the bias of the tile's columns (one copy, or one per warpgroup)
-constexpr int epi_buf_bytes(int bn) { return inline_epilogue(bn) ? kAccBytes : kStagingBytes; }
+
+// Epilogue variants (template parameter kEpi). The generic one takes every option at run time; the three fast ones
+// cover the shapes that are epilogue-bound in the UNet (K <= 640) with packed f32x2 arithmetic and no per-element
+// branches: ~2-3 instructions per output element instead of ~14.
+enum : int {
+  kEpiGeneric = 0,
+  kEpiPlain = 1,      // fp16 out, bias / row-add optional, alpha == 1, no residual, no activation, N % 32 == 0
+  kEpiResidual = 2,   // fp16 out, alpha * (acc + bias) + residual (beta == 1), N % 32 == 0
+  kEpiGeglu = 3,      // fp16 out, value * gelu(gate) on the packed [16 value | 16 gate] column layout
+  kEpiAct = 4         // the generic epilogue followed by GELU (act 2) or quick-GELU (act 3): ViT MLPs (clip_vision.cu)
+};
+// The fast variants on the epilogue warpgroup move their outputs (and residuals) through shared memory with TMA, in
+// whole 32-column runs; the others, and BN = 256, read and write global memory from the epilogue threads.
+constexpr bool tma_epilogue(int epi, int bn) {
+  return !inline_epilogue(bn) && (epi == kEpiPlain || epi == kEpiResidual || epi == kEpiGeglu);
+}
+// the accumulator buffer (staging or the two slices), the residual ring and the bias of the tile's columns (one copy,
+// or one per warpgroup)
+constexpr int epi_buf_bytes(int bn) { return inline_epilogue(bn) ? kAccBytes : kBlockM * bn * 4; }
+constexpr int res_ring_bytes(int epi, int bn) { return tma_epilogue(epi, bn) && epi == kEpiResidual ? kResSlots * kRunBytes : 0; }
 constexpr int bias_buf_bytes(int bn) { return inline_epilogue(bn) ? 2 * 256 * 4 : kMaxStagedN * 4; }
-constexpr int ring_bytes(int bn) { return kSmemBytes - epi_buf_bytes(bn) - bias_buf_bytes(bn) - 1024 /*align*/ - 256 /*barriers*/; }
+constexpr int ring_bytes(int epi, int bn) {
+  return kSmemBytes - epi_buf_bytes(bn) - res_ring_bytes(epi, bn) - bias_buf_bytes(bn) - 1024 /*align*/ - 256 /*barriers*/;
+}
 // one ring stage: the A tile and the weight tile, rounded up to the 1 KB swizzle period
 constexpr int ring_stage_bytes(int bn) { return kABytes + (bn * kBlockK * 2 + 1023) / 1024 * 1024; }
-constexpr int ring_stages(int bn) {
-  return ring_bytes(bn) / ring_stage_bytes(bn) < kMaxStages ? ring_bytes(bn) / ring_stage_bytes(bn) : kMaxStages;
+constexpr int ring_stages(int epi, int bn) {
+  return ring_bytes(epi, bn) / ring_stage_bytes(bn) < kMaxStages ? ring_bytes(epi, bn) / ring_stage_bytes(bn) : kMaxStages;
 }
-// 227 KB = 80 KB staging + 640 B bias + 1 KB alignment + 256 B barriers + the ring: 6 / 4 / 4 stages at BN 64 / 128 / 160;
-// at BN 256: 66 KB of slices + 2 KB bias + 1 KB + 256 B + the ring: 3 stages
-static_assert(ring_stages(64) == 6 && ring_stages(128) == 4 && ring_stages(160) == 4 && ring_stages(256) == 3,
+// Shared memory, from the 1 KB-aligned base: the operand ring, the staging (128 x BN fp32), the residual ring
+// (4 x 8 KB, residual variant only), the bias, 256 B of barriers; 1 KB is kept for the alignment.
+// 227 KB at BN 64 / 128 / 160: 32 / 64 / 80 KB staging + 640 B bias + the ring: 8 / 5 / 4 stages, and with the
+// residual ring 6 / 4 / 3; at BN 256: 66 KB of slices + 2 KB bias + the ring: 3 stages
+static_assert(ring_stages(kEpiPlain, 64) == 8 && ring_stages(kEpiPlain, 128) == 5 && ring_stages(kEpiPlain, 160) == 4 &&
+              ring_stages(kEpiResidual, 64) == 6 && ring_stages(kEpiResidual, 128) == 4 &&
+              ring_stages(kEpiResidual, 160) == 3 && ring_stages(kEpiResidual, 256) == 3,
               "shared-memory budget per tile width");
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
 __device__ __forceinline__ float silu(float x) { return __fdividef(x, 1.f + __expf(-x)); }
@@ -104,16 +134,6 @@ __device__ __forceinline__ F2 geglu2(F2 val, F2 gate) {
   return f2_mul(val, gelu);
 }
 
-// Epilogue variants (template parameter kEpi). The generic one takes every option at run time; the three fast ones
-// cover the shapes that are epilogue-bound in the UNet (K <= 640) with packed f32x2 arithmetic and no per-element
-// branches: ~2-3 instructions per output element instead of ~14.
-enum : int {
-  kEpiGeneric = 0,
-  kEpiPlain = 1,      // fp16 out, bias / row-add optional, alpha == 1, no residual, no activation, N % 32 == 0
-  kEpiResidual = 2,   // fp16 out, alpha * (acc + bias) + residual (beta == 1), N % 32 == 0
-  kEpiGeglu = 3,      // fp16 out, value * gelu(gate) on the packed [16 value | 16 gate] column layout
-  kEpiAct = 4         // the generic epilogue followed by GELU (act 2) or quick-GELU (act 3): ViT MLPs (clip_vision.cu)
-};
 // act 2: exact-erf GELU (transformers ACT2FN["gelu"]); act 3: x * sigmoid(1.702 x) (ACT2FN["quick_gelu"], ViT-L CLIP)
 __device__ __forceinline__ float gelu_act(float x, int act) {
   return act == 2 ? gelu_erf(x) : act == 3 ? __fdividef(x, 1.f + __expf(-1.702f * x)) : x;
@@ -122,19 +142,27 @@ __device__ __forceinline__ float gelu_act(float x, int act) {
 struct AMaps {
   CUtensorMap m[4];   // activation views: [0] source 0, [1] skip-concat source / stride-2 phases 1..3
 };
+struct EpiMaps {      // fp16 {columns, W, H, NF} views with box {32, bw, bh, bn} (64-byte swizzle): TMA epilogue only
+  CUtensorMap out, res;
+};
 
 // One 32-column output run of one row: accumulator columns [c0, c0 + 32) (GEGLU: [c0, c0 + 64)), read by ld32(col, v);
-// bias / time-embedding / residual / GEGLU / GELU -> fp16 (or fp32) -> 16-byte global stores. Both epilogue placements
+// bias / time-embedding / residual / GEGLU / GELU -> fp16 (or fp32) -> 16-byte stores. Both epilogue placements
 // (the epilogue warpgroup, and the MMA warpgroups at BN = 256) run this, so their outputs are the same bits.
-template <int kEpi, class Ld>
-__device__ __forceinline__ void finish_run(const ConvGemmParams& p, const Ld& ld32, int c0, int ncol0, const float* sbias,
-                                           const float* radd, const uint4 (&rcur)[4], bool row_ok, bool use_res,
-                                           long long m, __half* out_row) {
+// The fast variants call loaded() once the run's accumulator is in registers (every thread of the caller reaches it)
+// and hand each 16-byte group g of output columns [col, col + 8) to st16(col, g, value); the generic ones store to
+// out_row themselves.
+template <int kEpi, class Ld, class Loaded, class St>
+__device__ __forceinline__ void finish_run(const ConvGemmParams& p, const Ld& ld32, const Loaded& loaded, const St& st16,
+                                           int c0, int ncol0, const float* sbias, const float* radd,
+                                           const uint4 (&rcur)[4], bool row_ok, bool use_res, long long m,
+                                           __half* out_row) {
   if constexpr (kEpi != kEpiGeneric && kEpi != kEpiAct) {
     const int nbase = ncol0 + c0;
     uint32_t v[32], vg[32];
     ld32(c0, v);
     if constexpr (kEpi == kEpiGeglu) ld32(c0 + 32, vg);
+    loaded();
     if (nbase < p.N && row_ok) {
       const F2 alpha2 = f2_make(p.alpha, p.alpha);
       const float* cbias = sbias + c0;           // this chunk's bias
@@ -185,7 +213,7 @@ __device__ __forceinline__ void finish_run(const ConvGemmParams& p, const Ld& ld
             o[e] = *reinterpret_cast<const uint32_t*>(&h2);
           }
         }
-        *reinterpret_cast<uint4*>(out_row + oc + 8 * g) = make_uint4(o[0], o[1], o[2], o[3]);
+        st16(oc + 8 * g, g, make_uint4(o[0], o[1], o[2], o[3]));
       }
     }
   } else {
@@ -357,7 +385,8 @@ __device__ __forceinline__ void inline_epilogue_tile(const ConvGemmParams& p, co
         }
       };
       load_res(c0);
-      finish_run<kEpi>(p, ld32, c0, ncol0, wbias, radd, rcur, row_ok, use_res, m, out_row);
+      finish_run<kEpi>(p, ld32, [] {}, [&](int col, int, uint4 o) { *reinterpret_cast<uint4*>(out_row + col) = o; },
+                       c0, ncol0, wbias, radd, rcur, row_ok, use_res, m, out_row);
     }
   }
 }
@@ -365,27 +394,38 @@ __device__ __forceinline__ void inline_epilogue_tile(const ConvGemmParams& p, co
 template <int kEpi, int BN>
 __global__ void __launch_bounds__(conv_threads(BN), 1)
 conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ ConvGemmParams p) {
+                 const __grid_constant__ EpiMaps tmE, const __grid_constant__ ConvGemmParams p) {
   constexpr bool kInline = inline_epilogue(BN);
+  constexpr bool kTma = tma_epilogue(kEpi, BN);
+  constexpr bool kResRing = res_ring_bytes(kEpi, BN) > 0;
   static_assert(BN % 32 == 0 && (BN <= kMaxStagedN || kInline), "the staging swizzle and the epilogue take whole 32-column runs");
   // the producer gives its registers away; an MMA thread holds BN / 2 accumulators (and, in line, runs the epilogue),
   // an epilogue thread one row's 32- or 64-column run plus the next run's residual
   constexpr int kProducerRegs = 40, kConsumerRegs = kInline ? 232 : 152, kEpilogueRegs = kInline ? 0 : 168;
   static_assert(128 * (kProducerRegs + kEpilogueRegs) + 256 * kConsumerRegs <= 65536,
                 "setmaxnreg split exceeds the register file");
-  constexpr int kRingBytes = ring_bytes(BN);
+  // the operand ring ends on a 1 KB boundary (stages are whole KB), so the staging runs and the residual slots that
+  // follow it keep the alignment the 64-byte TMA swizzle needs
+  constexpr int kRingEnd = ring_stages(kEpi, BN) * ring_stage_bytes(BN);
+  static_assert(kRingEnd % 1024 == 0 && kRingEnd + epi_buf_bytes(BN) + res_ring_bytes(kEpi, BN) + bias_buf_bytes(BN) + 256 + 1024 <=
+                kSmemBytes, "shared-memory layout");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // staging: [128 rows][BN] fp32; 16-byte chunk j of row r sits at chunk j ^ (r & 7), so that both the fragment writes
-  // (8 rows x 2 chunks per warp store) and the row reads (32 rows, one chunk each) are free of bank conflicts.
-  // In line (BN = 256): [2 warpgroups][64][kAccLd] slices.
-  float* stg = reinterpret_cast<float*>(smem + kRingBytes);
-  float* sbias = reinterpret_cast<float*>(smem + kRingBytes + epi_buf_bytes(BN));  // [BN], in line [2 warpgroups][256]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes + epi_buf_bytes(BN) + bias_buf_bytes(BN));
+  // staging: [BN / 32 runs][128 rows][32] fp32; 16-byte chunk j of row r sits at chunk j ^ (r & 7), so that both the
+  // fragment writes (8 rows x 2 chunks per warp store) and the row reads (32 rows, one chunk each) are free of bank
+  // conflicts. The TMA epilogue writes a run's fp16 outputs over the first 8 KB of that run's 16 KB once every row has
+  // been read. In line (BN = 256): [2 warpgroups][64][kAccLd] slices.
+  float* stg = reinterpret_cast<float*>(smem + kRingEnd);
+  uint8_t* sres = smem + kRingEnd + epi_buf_bytes(BN);                  // [kResSlots][128 rows][64 bytes], residual only
+  float* sbias = reinterpret_cast<float*>(sres + res_ring_bytes(kEpi, BN));  // [BN], in line [2 warpgroups][256]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sres + res_ring_bytes(kEpi, BN) + bias_buf_bytes(BN));
   uint64_t* full = bars;                       // [kMaxStages]
   uint64_t* empty = bars + kMaxStages;         // [kMaxStages]
   uint64_t* acc_full = bars + 2 * kMaxStages;  // the staging holds a finished tile
   uint64_t* acc_empty = acc_full + 1;          // the epilogue has read it
+  uint64_t* res_full = acc_full + 2;           // [kResSlots] a residual run has landed
+  uint64_t* res_empty = res_full + kResSlots;  // [kResSlots] the epilogue has read it
+  static_assert(2 * kMaxStages + 2 + 2 * kResSlots <= 256 / 8, "barrier area");
   const int nstages = p.nstages;
   const int stage_bytes = p.stage_bytes;
 
@@ -398,12 +438,18 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
     tma_prefetch_desc(&tmA.m[2]);
     tma_prefetch_desc(&tmA.m[3]);
     tma_prefetch_desc(&tmB);
+    if constexpr (kTma) tma_prefetch_desc(&tmE.out);
+    if constexpr (kResRing) tma_prefetch_desc(&tmE.res);
     for (int s = 0; s < kMaxStages; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 8);                 // one arrival per consumer warp
     }
     mbar_init(acc_full, 8);                    // one arrival per consumer warp
     mbar_init(acc_empty, 4);                   // one arrival per epilogue warp
+    for (int s = 0; s < kResSlots; ++s) {
+      mbar_init(&res_full[s], 1);
+      mbar_init(&res_empty[s], 1);             // the epilogue thread that stores the run
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -450,6 +496,28 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
           }
         }
       }
+    } else if (kResRing && warp == 1) {
+      // residual producer: the tile's 32-column residual runs, box {32, bw, bh, bn} = the tile's 128 rows, into the
+      // ring of kResSlots, running ahead of the epilogue into the next tile while warp 0 loads its operands
+      int slot = 0;
+      uint32_t phase = 0;
+      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+        const int nt = unit % p.tiles_nn;
+        const int mt = unit / p.tiles_nn;
+        const int tw = mt % p.tiles_w;
+        const int th = (mt / p.tiles_w) % p.tiles_h;
+        const int tn = mt / (p.tiles_w * p.tiles_h);
+        const int ncol0 = nt * BN;
+        for (int c0 = 0; c0 < BN && ncol0 + c0 < p.N; c0 += 32) {
+          mbar_wait(&res_empty[slot], phase ^ 1);
+          if (elect_one()) {
+            mbar_expect_tx(&res_full[slot], kRunBytes);
+            tma_load_4d(sres + slot * kRunBytes, &tmE.res, &res_full[slot], ncol0 + c0, tw * p.bw, th * p.bh, tn * p.bn);
+          }
+          __syncwarp();
+          if (++slot == kResSlots) { slot = 0; phase ^= 1; }
+        }
+      }
     }
     return;
   }
@@ -457,14 +525,19 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
   if (!kInline && warp >= 12) {
     // ---- epilogue warpgroup: finishes tile i from the staging while the consumers run tile i + 1's K loop.
     // Thread r owns accumulator row r and walks its 32-column runs: bias / time-embedding / residual / GEGLU / GELU
-    // (five template variants) -> fp16 -> 16-byte global stores.
+    // (five template variants) -> fp16. The fast variants (kTma) take each run's residual from the ring and write its
+    // outputs into the staging run they came from, which one thread then stores with TMA: every global access is a
+    // whole 8 KB box. The generic ones read residuals and store outputs from each thread, 16 bytes at a time.
     setmaxnreg_inc<kEpilogueRegs>();
     const int r = threadIdx.x - 384;
-    const float* srow = stg + r * BN;
+    const float* srow = stg + r * 32;
     const int sw = r & 7;
+    const int sw64 = (r >> 1) & 3;                      // 64-byte TMA swizzle of row r: 16-byte chunk g sits at g ^ sw64
     const bool use_res = (p.res != nullptr) && !p.geglu && !p.out_f32;
     const int acc_step = p.geglu ? 64 : 32;             // accumulator columns consumed per 32 output columns
     uint32_t acc_phase = 0;
+    int rslot = 0;
+    uint32_t rphase = 0;
     for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
       const int nt = unit % p.tiles_nn;
       const int mt = unit / p.tiles_nn;
@@ -482,13 +555,13 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
       const __half* res_row = use_res ? p.res + m * p.ld_res : nullptr;
       __half* out_row = reinterpret_cast<__half*>(p.out) + m * p.ldc;
 
-      uint4 rcur[4] = {}, rnext[4] = {};    // residual of this run / the next one
-      auto load_res = [&](int c0, uint4 (&dst)[4]) {
+      uint4 rcur[4] = {};                   // residual of this run
+      auto load_res = [&](int c0) {
         if (!use_res || !row_ok) return;
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
           const int nn = ncol0 + c0 + g * 8;
-          if (c0 + g * 8 < BN && nn < p.N) dst[g] = __ldg(reinterpret_cast<const uint4*>(res_row + nn));
+          if (c0 + g * 8 < BN && nn < p.N) rcur[g] = __ldg(reinterpret_cast<const uint4*>(res_row + nn));
         }
       };
       // what the tile needs besides the accumulator is fetched while its K loop still runs
@@ -497,31 +570,60 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
         for (int c = r; c < BN; c += 128) sbias[c] = (p.bias && ncol0 + c < p.N) ? __ldg(p.bias + ncol0 + c) : 0.f;
         named_bar_sync(1, 128);
       }
-      load_res(0, rcur);
+      if constexpr (!kTma) load_res(0);
       mbar_wait(acc_full, acc_phase);
       for (int c0 = 0; c0 < BN; c0 += acc_step) {
-        // the residual variant loads the next run's residual ahead; the generic ones, short of registers, this run's
-        if constexpr (kEpi == kEpiResidual) load_res(c0 + acc_step, rnext);
-        else if (c0 > 0) load_res(c0, rcur);
         // accumulator columns [col, col + 32) of row r (col is a multiple of 32: the swizzle stays inside the run)
         auto ld32 = [&](int col, uint32_t (&v)[32]) {
 #pragma unroll
           for (int k = 0; k < 8; ++k) {
-            const float4 x = *reinterpret_cast<const float4*>(srow + col + 4 * (k ^ sw));
+            const float4 x = *reinterpret_cast<const float4*>(srow + (col >> 5) * kRunFloats + 4 * (k ^ sw));
             v[4 * k] = __float_as_uint(x.x); v[4 * k + 1] = __float_as_uint(x.y);
             v[4 * k + 2] = __float_as_uint(x.z); v[4 * k + 3] = __float_as_uint(x.w);
           }
         };
-        finish_run<kEpi>(p, ld32, c0, ncol0, sbias, radd, rcur, row_ok, use_res, m, out_row);
-        if constexpr (kEpi == kEpiResidual) {
+        if constexpr (kTma) {
+          if (ncol0 + c0 >= p.N) break;                 // N % 32 == 0: the runs from here on lie wholly past N
+          if constexpr (kEpi == kEpiResidual) {
+            mbar_wait(&res_full[rslot], rphase);
+            const uint4* rrow = reinterpret_cast<const uint4*>(sres + rslot * kRunBytes + r * 64);
 #pragma unroll
-          for (int g = 0; g < 4; ++g) rcur[g] = rnext[g];
+            for (int g = 0; g < 4; ++g) rcur[g] = rrow[g ^ sw64];
+          }
+          // row r's 32 fp16 outputs go to bytes [64 r, 64 r + 64) of the run's staging, over accumulator rows < 64:
+          // they are written only once every row of the run has been read (loaded)
+          uint8_t* orun = reinterpret_cast<uint8_t*>(stg) + (c0 >> 5) * (kRunFloats * 4);
+          finish_run<kEpi>(p, ld32, [] { named_bar_sync(1, 128); },
+                           [&](int, int g, uint4 o) { *reinterpret_cast<uint4*>(orun + r * 64 + 16 * (g ^ sw64)) = o; },
+                           c0, ncol0, sbias, radd, rcur, row_ok, use_res, m, out_row);
+          // every thread's generic-proxy accesses of the run (its output writes, and its residual reads, which the
+          // arithmetic has consumed) are ordered before the TMA store reads the outputs and before the residual slot
+          // goes back to the producer. The slot is not released right after the reads are issued: they can still be
+          // in flight then, and the next TMA load would overwrite the slot under them.
+          fence_proxy_async();
+          named_bar_sync(1, 128);
+          if (r == 0) {                                 // rows outside the image are clipped by the tensor map
+            if constexpr (kEpi == kEpiResidual) mbar_arrive(&res_empty[rslot]);
+            tma_store_4d(&tmE.out, orun, kEpi == kEpiGeglu ? (ncol0 + c0) / 2 : ncol0 + c0, tw * p.bw, th * p.bh,
+                         tn * p.bn);
+            tma_store_commit();
+          }
+          if constexpr (kEpi == kEpiResidual) {
+            if (++rslot == kResSlots) { rslot = 0; rphase ^= 1; }
+          }
+        } else {
+          if (c0 > 0) load_res(c0);
+          finish_run<kEpi>(p, ld32, [] {}, [&](int col, int, uint4 o) { *reinterpret_cast<uint4*>(out_row + col) = o; },
+                           c0, ncol0, sbias, radd, rcur, row_ok, use_res, m, out_row);
         }
       }
+      // the MMA warpgroups overwrite the staging once every epilogue warp has arrived: the stores must have read it
+      if (kTma && r == 0) tma_store_wait_read<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(acc_empty);
       acc_phase ^= 1;
     }
+    if (kTma && r == 0) tma_store_wait_all();
     return;
   }
 
@@ -535,7 +637,7 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
   const uint32_t stage_step = (uint32_t)stage_bytes >> 4;     // descriptor address field counts 16-byte units
   // fragment rows 16 wq + lane / 4 and + 8 of this warpgroup's 64 (both have row & 7 == lane / 4), column pairs
   // 8 i + 2 (lane % 4) = chunk 2 i + (lane % 4) / 2, offset 2 (lane % 2) inside it
-  float* stg_row = stg + (64 * wg + 16 * wq + (lane >> 2)) * BN;
+  float* stg_row = stg + (64 * wg + 16 * wq + (lane >> 2)) * 32;
   int stage = 0;
   uint32_t phase = 0;
   uint32_t acc_phase = 0;
@@ -575,10 +677,10 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
       // ---- hand the tile to the epilogue warpgroup once it has read the previous one, then go on to the next tile
       mbar_wait(acc_empty, acc_phase ^ 1);
 #pragma unroll
-      for (int i = 0; i < BN / 8; ++i) {
-        const int off = 4 * ((2 * i + ((lane & 3) >> 1)) ^ (lane >> 2)) + 2 * (lane & 1);
+      for (int i = 0; i < BN / 8; ++i) {       // columns 8 i .. 8 i + 7 lie in run i / 4, chunks 2 (i % 4), + 1
+        const int off = (i >> 2) * kRunFloats + 4 * ((2 * (i & 3) + ((lane & 3) >> 1)) ^ (lane >> 2)) + 2 * (lane & 1);
         *reinterpret_cast<float2*>(stg_row + off) = make_float2(acc[4 * i], acc[4 * i + 1]);
-        *reinterpret_cast<float2*>(stg_row + 8 * BN + off) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+        *reinterpret_cast<float2*>(stg_row + 8 * 32 + off) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(acc_full);
@@ -694,7 +796,7 @@ void tensor_map_cache_stats(unsigned long long* hits, unsigned long long* misses
   *misses = g_map_misses;
 }
 
-// rank-4 fp16 map, inner box 64 elements, swizzle as given, zero fill out of bounds
+// rank-4 fp16 map, box and swizzle as given, zero fill out of bounds
 bool encode_map_4d_sw(CUtensorMap* m, const void* ptr, const uint64_t dims[4], const uint64_t strides_elems[3],
                       const uint32_t box[4], CUtensorMapSwizzle swz) {
   MapKey k;
@@ -767,7 +869,7 @@ static int pick_block_n(int N, int geglu, int gelu, long long tiles_m, int num_s
 static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, int nmaps, ConvGemmParams& p,
                                  const __half* wt, long long ktot, const Epilogue& ep, int num_sms, const char** err) {
   // kernel variants indexed [tile width][epilogue]
-  typedef void (*KernelFn)(const AMaps, const CUtensorMap, const ConvGemmParams);
+  typedef void (*KernelFn)(const AMaps, const CUtensorMap, const EpiMaps, const ConvGemmParams);
 #define MVB_GEMM_ROW(BN) \
   {conv_gemm_kernel<kEpiGeneric, BN>, conv_gemm_kernel<kEpiPlain, BN>, conv_gemm_kernel<kEpiResidual, BN>, \
    conv_gemm_kernel<kEpiGeglu, BN>, conv_gemm_kernel<kEpiAct, BN>}
@@ -796,8 +898,6 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   int bn_idx = 0;
   while (kBlockNs[bn_idx] != p.block_n) ++bn_idx;
   p.tiles_nn = ceil_div(p.N, p.block_n);
-  p.stage_bytes = ring_stage_bytes(p.block_n);
-  p.nstages = ring_stages(p.block_n);
   p.out = ep.out; p.ldc = ep.ldc; p.bias = ep.bias; p.rowadd = ep.rowadd;
   p.rows_per_group = ep.rows_per_group > 0 ? ep.rows_per_group : 1;
   p.ld_rowadd = ep.ld_rowadd; p.res = ep.res; p.ld_res = ep.ld_res; p.alpha = ep.alpha; p.beta = ep.beta;
@@ -805,6 +905,10 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   if (ep.out_f32 && (ep.geglu || ep.res)) { *err = "conv_gemm: fp32 output excludes geglu/residual"; return cudaErrorInvalidValue; }
   if ((ep.ldc % (ep.out_f32 ? 4 : 8)) || (reinterpret_cast<uintptr_t>(ep.out) % 16)) {
     *err = "conv_gemm: the output must be 16-byte aligned with a row stride of whole 16-byte vectors";
+    return cudaErrorInvalidValue;
+  }
+  if (ep.res && ((ep.ld_res % 8) || (reinterpret_cast<uintptr_t>(ep.res) % 16))) {
+    *err = "conv_gemm: the residual must be 16-byte aligned with a row stride of whole 16-byte vectors";
     return cudaErrorInvalidValue;
   }
   CUtensorMap tmB;
@@ -824,6 +928,31 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
     }
   }
   if (gelu) epi = kEpiAct;
+  p.stage_bytes = ring_stage_bytes(p.block_n);
+  p.nstages = ring_stages(epi, p.block_n);
+  // the TMA epilogue's output (and residual) views: {columns, W, H, NF} with the tile's pixel box, one 32-column run
+  // per box; out-of-image rows and columns past the tensor are clipped on store and zero-filled on load
+  const bool tma_epi = tma_epilogue(epi, p.block_n);
+  EpiMaps em;
+  memset(&em, 0, sizeof(em));
+  if (tma_epi) {
+    const uint32_t box[4] = {32u, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
+    const uint64_t ncols = (uint64_t)(ep.geglu ? p.N / 2 : p.N);
+    const uint64_t od[4] = {ncols, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.NF};
+    const uint64_t os[3] = {(uint64_t)ep.ldc, (uint64_t)ep.ldc * p.W, (uint64_t)ep.ldc * p.W * p.H};
+    if (!encode_map_4d_sw(&em.out, ep.out, od, os, box, CU_TENSOR_MAP_SWIZZLE_64B)) {
+      *err = "cuTensorMapEncodeTiled(out) failed";
+      return cudaErrorInvalidValue;
+    }
+    if (epi == kEpiResidual) {
+      const uint64_t rd[4] = {(uint64_t)p.N, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.NF};
+      const uint64_t rs[3] = {(uint64_t)ep.ld_res, (uint64_t)ep.ld_res * p.W, (uint64_t)ep.ld_res * p.W * p.H};
+      if (!encode_map_4d_sw(&em.res, ep.res, rd, rs, box, CU_TENSOR_MAP_SWIZZLE_64B)) {
+        *err = "cuTensorMapEncodeTiled(residual) failed";
+        return cudaErrorInvalidValue;
+      }
+    }
+  }
   static const bool trace = getenv("MVB_TRACE") != nullptr;
   if (trace) {
     // the trailing fields describe the launch fully enough to replay it (tools/gpu_gemm_census.py): output image, the
@@ -834,15 +963,15 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
     int s2 = 0;
     for (int i = 0; i < p.ntaps; ++i) if (p.tap_src[i]) s2 = p.dy[0] < 0 ? 1 : 2;
     fprintf(stderr, "MVB_TRACE gemm M=%lld N=%d K=%lld taps=%d block_n=%d tiles=%lld geglu=%d res=%d f32=%d epi=%d "
-            "W=%d H=%d NF=%d c0=%d c1=%d offsets=%s s2=%d bias=%d rowadd=%d rpg=%d alpha=%.9g beta=%.9g act=%d\n",
+            "epi_io=%s W=%d H=%d NF=%d c0=%d c1=%d offsets=%s s2=%d bias=%d rowadd=%d rpg=%d alpha=%.9g beta=%.9g act=%d\n",
             (long long)p.W * p.H * p.NF, p.N, ktot, p.ntaps, p.block_n, num_tiles, p.geglu, p.res != nullptr, p.out_f32,
-            epi, p.W, p.H, p.NF, p.kb0 * 64, p.kb1 * 64, taps, s2, p.bias != nullptr, p.rowadd != nullptr,
+            epi, tma_epi ? "tma" : "lsu", p.W, p.H, p.NF, p.kb0 * 64, p.kb1 * 64, taps, s2, p.bias != nullptr, p.rowadd != nullptr,
             p.rows_per_group, p.alpha, p.beta, p.act);
   }
   AMaps am;
   for (int i = 0; i < 4; ++i) am.m[i] = maps[i < nmaps ? i : 0];
   ProfScope prof(stream, KC_GEMM);
-  kernels[bn_idx][epi]<<<grid, conv_threads(p.block_n), kSmemBytes, stream>>>(am, tmB, p);
+  kernels[bn_idx][epi]<<<grid, conv_threads(p.block_n), kSmemBytes, stream>>>(am, tmB, em, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) *err = "conv_gemm_kernel launch";
   return e;

@@ -104,7 +104,10 @@ int mvb_op_temporal_attention(const void* qkv, int ld, int B, int T, int HW, int
                               void* out, int ldo, void* stream) {
   cudaError_t e = temporal_attention((cudaStream_t)stream, (const __half*)qkv, ld, B, T, HW, heads, d, dp, scale,
                                      (__half*)out, ldo);
-  if (e != cudaSuccess) return fail("mvb_op_temporal_attention", e == cudaErrorInvalidValue ? cudaSuccess : e);
+  if (e == cudaErrorInvalidValue)
+    return fail("mvb_op_temporal_attention: needs 1 <= T <= 32, d a multiple of 8, dp in {16, 32, 48, 64, 80, 96, 160} "
+                "with dp >= d, ld and ldo multiples of 8", cudaSuccess);
+  if (e != cudaSuccess) return fail("mvb_op_temporal_attention", e);
   return MVB_OK;
 }
 

@@ -128,9 +128,11 @@ static __half* vae_mid(Engine::Fwd& f, const VaeWeights& w, __half* x, int C, in
       Mat tok; tok.w = nbuf + (long long)n * HW * C; tok.N = HW; tok.K = C; tok.bias = nullptr;
       { Epilogue ep; ep.out = vt + (long long)n * C * HW; ep.ldc = HW; f.gemm(w.v.w, C, C, tok, ep, false); }
       Mat km; km.w = k + (long long)n * HW * C; km.N = HW; km.K = C; km.bias = nullptr;
-      { Epilogue ep; ep.out = sc; ep.ldc = HW; f.gemm(q + (long long)n * HW * C, HW, C, km, ep, false); }
+      // the scores are scaled by 1/sqrt(C) in fp32 before they are rounded to fp16, as diffusers' baddbmm(alpha = scale)
+      // does: raw q.k products overflow fp16 at sqrt(C) (22.6x for C = 512) smaller activations than the scaled ones
+      { Epilogue ep; ep.out = sc; ep.ldc = HW; ep.alpha = 1.f / sqrtf((float)C); f.gemm(q + (long long)n * HW * C, HW, C, km, ep, false); }
       if (!f.dry && f.ok) {
-        cudaError_t e = softmax_rows(f.s, sc, HW, HW, HW, 1.f / sqrtf((float)C));
+        cudaError_t e = softmax_rows(f.s, sc, HW, HW, HW, 1.f);
         if (e != cudaSuccess) f.fail("softmax_rows", e);
       }
       Mat vm; vm.w = vt + (long long)n * C * HW; vm.N = C; vm.K = HW; vm.bias = w.v.bias;

@@ -1136,8 +1136,10 @@ temporal_attention_mma_kernel(const __half* __restrict__ qkv, int ld, int B, int
 
 cudaError_t temporal_attention(cudaStream_t s, const __half* qkv, int ld, int B, int T, int HW, int heads, int d, int dp,
                                float scale, __half* out, int ldo) {
-  ProfScope prof(s, KC_TEMPORAL_ATTN);
-  if (T > 32 || T < 1 || (d % 8) || (dp % 16) || dp < d) return cudaErrorInvalidValue;
+  // rows are staged and written back as 16-byte vectors, so both row strides must be whole multiples of 8 halves
+  if (T > 32 || T < 1 || (d % 8) || (dp % 16) || dp < d || (ld % 8) || (ldo % 8)) return cudaErrorInvalidValue;
+  if (dp < 16 || (dp > 96 && dp != 160)) return cudaErrorInvalidValue;   // the instantiations below
+  ProfScope prof(s, KC_TEMPORAL_ATTN);   // after the checks: a refused call launches nothing and counts no launch
   const long long nprob = (long long)B * HW * heads;
   const int wpb = 4;
   const unsigned blocks = (unsigned)((nprob + wpb - 1) / wpb);

@@ -17,8 +17,11 @@
 // Pipeline: smem operand ring (full/empty mbarriers, 3..8 stages depending on BN); one staging buffer handed over by
 // acc_full (8 MMA warps arrive) / acc_empty (4 epilogue warps arrive, after the tile's TMA stores have read it), whose
 // phases flip once per tile.
-// BN = 256: 384 threads, no epilogue warpgroup; the MMA warpgroups finish their own rows through padded fp32 slices
-// (inline_epilogue_tile) with the same per-run code (finish_run).
+// BN = 256: 384 threads, no epilogue warpgroup (plain / residual / GEGLU only). The MMA warpgroups finish their own
+// accumulator fragments in registers (fragment_epilogue) with the same per-element helpers as finish_run, write the
+// fp16 results into one 128 x 256 output tile in shared memory and arrive on out_full; warp 1 of warpgroup 0 stores the
+// tile's runs with TMA, waits until they have read the tile, writes the next tile's bias, TMA-loads its residual runs
+// into the same tile and arrives on out_ready, which the MMA warpgroups wait on after their next K loop.
 #include "conv_gemm.cuh"
 
 #include <dlfcn.h>
@@ -39,16 +42,15 @@ static constexpr int kBlockK = 64;
 static constexpr int kABytes = kBlockM * kBlockK * 2;        // 16 KB
 static constexpr int kSmemBytes = 227 * 1024;
 // Tiles up to 160 columns hand the accumulator to an epilogue warpgroup through one staging buffer. A 256-column
-// tile's staging buffer would take 128 KB and leave the operand ring 2 stages, so BN = 256 keeps the epilogue in the
-// MMA warpgroups, each through its own padded 64-row x 128-column fp32 slice.
+// tile's staging buffer would take 128 KB and leave the operand ring 2 stages, and an MMA thread holding 128
+// accumulators leaves no registers for a fourth warpgroup, so BN = 256 keeps the epilogue in the MMA warpgroups, on
+// their accumulator fragments, with a 64 KB fp16 output tile in shared memory.
 constexpr bool inline_epilogue(int bn) { return bn == 256; }
 constexpr int conv_threads(int bn) { return inline_epilogue(bn) ? 384 : 512; }
 static constexpr int kMaxStagedN = 160;                        // the widest tile with the epilogue warpgroup
 static constexpr int kRunFloats = kBlockM * 32;                // one 32-column run of the fp32 staging (16 KB)
 static constexpr int kRunBytes = kBlockM * 32 * 2;             // one 32-column run of fp16 outputs or residuals (8 KB)
 static constexpr int kResSlots = 4;                            // residual ring: 32-column runs loaded ahead of the epilogue
-static constexpr int kAccLd = 132;                             // in-line epilogue: fp32 slice row stride (conflict-free float4 reads)
-static constexpr int kAccBytes = 2 * 64 * kAccLd * 4;          // in-line epilogue: per MMA warpgroup 64 rows x 128 columns
 
 // Epilogue variants (template parameter kEpi). The generic one takes every option at run time; the three fast ones
 // cover the shapes that are epilogue-bound in the UNet (K <= 640) with packed f32x2 arithmetic and no per-element
@@ -60,16 +62,16 @@ enum : int {
   kEpiGeglu = 3,      // fp16 out, value * gelu(gate) on the packed [16 value | 16 gate] column layout
   kEpiAct = 4         // the generic epilogue followed by GELU (act 2) or quick-GELU (act 3): ViT MLPs (clip_vision.cu)
 };
-// The fast variants on the epilogue warpgroup move their outputs (and residuals) through shared memory with TMA, in
-// whole 32-column runs; the others, and BN = 256, read and write global memory from the epilogue threads.
-constexpr bool tma_epilogue(int epi, int bn) {
-  return !inline_epilogue(bn) && (epi == kEpiPlain || epi == kEpiResidual || epi == kEpiGeglu);
+// The fast variants move their outputs (and residuals) through shared memory with TMA, in whole 32-column runs; the
+// generic and GELU ones read and write global memory from the epilogue threads and are not instantiated at BN = 256.
+constexpr bool tma_epilogue(int epi, int bn) { return epi == kEpiPlain || epi == kEpiResidual || epi == kEpiGeglu; }
+// the epilogue buffer (the fp32 staging, or at BN = 256 the fp16 output tile, which also takes the residual), the
+// residual ring and the bias of the tile's columns
+constexpr int epi_buf_bytes(int bn) { return inline_epilogue(bn) ? kBlockM * bn * 2 : kBlockM * bn * 4; }
+constexpr int res_ring_bytes(int epi, int bn) {
+  return !inline_epilogue(bn) && tma_epilogue(epi, bn) && epi == kEpiResidual ? kResSlots * kRunBytes : 0;
 }
-// the accumulator buffer (staging or the two slices), the residual ring and the bias of the tile's columns (one copy,
-// or one per warpgroup)
-constexpr int epi_buf_bytes(int bn) { return inline_epilogue(bn) ? kAccBytes : kBlockM * bn * 4; }
-constexpr int res_ring_bytes(int epi, int bn) { return tma_epilogue(epi, bn) && epi == kEpiResidual ? kResSlots * kRunBytes : 0; }
-constexpr int bias_buf_bytes(int bn) { return inline_epilogue(bn) ? 2 * 256 * 4 : kMaxStagedN * 4; }
+constexpr int bias_buf_bytes(int bn) { return inline_epilogue(bn) ? 256 * 4 : kMaxStagedN * 4; }
 constexpr int ring_bytes(int epi, int bn) {
   return kSmemBytes - epi_buf_bytes(bn) - res_ring_bytes(epi, bn) - bias_buf_bytes(bn) - 1024 /*align*/ - 256 /*barriers*/;
 }
@@ -78,13 +80,15 @@ constexpr int ring_stage_bytes(int bn) { return kABytes + (bn * kBlockK * 2 + 10
 constexpr int ring_stages(int epi, int bn) {
   return ring_bytes(epi, bn) / ring_stage_bytes(bn) < kMaxStages ? ring_bytes(epi, bn) / ring_stage_bytes(bn) : kMaxStages;
 }
-// Shared memory, from the 1 KB-aligned base: the operand ring, the staging (128 x BN fp32), the residual ring
-// (4 x 8 KB, residual variant only), the bias, 256 B of barriers; 1 KB is kept for the alignment.
+// Shared memory, from the 1 KB-aligned base: the operand ring, the staging (128 x BN fp32; at BN 256 the 128 x 256
+// fp16 output tile), the residual ring (4 x 8 KB, residual variant at BN <= 160 only), the bias, 256 B of barriers;
+// 1 KB is kept for the alignment.
 // 227 KB at BN 64 / 128 / 160: 32 / 64 / 80 KB staging + 640 B bias + the ring: 8 / 5 / 4 stages, and with the
-// residual ring 6 / 4 / 3; at BN 256: 66 KB of slices + 2 KB bias + the ring: 3 stages
+// residual ring 6 / 4 / 3; at BN 256: 64 KB output tile + 1 KB bias + the ring: 3 stages of 48 KB
 static_assert(ring_stages(kEpiPlain, 64) == 8 && ring_stages(kEpiPlain, 128) == 5 && ring_stages(kEpiPlain, 160) == 4 &&
               ring_stages(kEpiResidual, 64) == 6 && ring_stages(kEpiResidual, 128) == 4 &&
-              ring_stages(kEpiResidual, 160) == 3 && ring_stages(kEpiResidual, 256) == 3,
+              ring_stages(kEpiResidual, 160) == 3 && ring_stages(kEpiPlain, 256) == 3 &&
+              ring_stages(kEpiResidual, 256) == 3 && ring_stages(kEpiGeglu, 256) == 3,
               "shared-memory budget per tile width");
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
 __device__ __forceinline__ float silu(float x) { return __fdividef(x, 1.f + __expf(-x)); }
@@ -134,6 +138,27 @@ __device__ __forceinline__ F2 geglu2(F2 val, F2 gate) {
   return f2_mul(val, gelu);
 }
 
+// The per-element expressions of the fast variants. finish_run and fragment_epilogue both compute through these, so
+// an output gets the same bits whichever epilogue finishes it.
+__device__ __forceinline__ uint32_t half2_bits(F2 x) {
+  float x0, x1;
+  f2_get(x, x0, x1);
+  const __half2 h2 = __floats2half2_rn(x0, x1);
+  return *reinterpret_cast<const uint32_t*>(&h2);
+}
+// bias + time-embedding row
+__device__ __forceinline__ F2 epi_rowadd2(F2 bias, float2 radd) { return f2_add(bias, f2_make(radd.x, radd.y)); }
+__device__ __forceinline__ uint32_t epi_plain2(F2 acc, F2 bias) { return half2_bits(f2_add(acc, bias)); }
+// alpha * (acc + bias) + residual
+__device__ __forceinline__ uint32_t epi_residual2(F2 acc, F2 bias, F2 alpha2, uint32_t res) {
+  const float2 rr = __half22float2(*reinterpret_cast<const __half2*>(&res));
+  return half2_bits(f2_fma(f2_add(acc, bias), alpha2, f2_make(rr.x, rr.y)));
+}
+// (value + bias) * gelu(gate + bias)
+__device__ __forceinline__ uint32_t epi_geglu2(F2 val, F2 bval, F2 gate, F2 bgate) {
+  return half2_bits(geglu2(f2_add(val, bval), f2_add(gate, bgate)));
+}
+
 // act 2: exact-erf GELU (transformers ACT2FN["gelu"]); act 3: x * sigmoid(1.702 x) (ACT2FN["quick_gelu"], ViT-L CLIP)
 __device__ __forceinline__ float gelu_act(float x, int act) {
   return act == 2 ? gelu_erf(x) : act == 3 ? __fdividef(x, 1.f + __expf(-1.702f * x)) : x;
@@ -147,8 +172,8 @@ struct EpiMaps {      // fp16 {columns, W, H, NF} views with box {32, bw, bh, bn
 };
 
 // One 32-column output run of one row: accumulator columns [c0, c0 + 32) (GEGLU: [c0, c0 + 64)), read by ld32(col, v);
-// bias / time-embedding / residual / GEGLU / GELU -> fp16 (or fp32) -> 16-byte stores. Both epilogue placements
-// (the epilogue warpgroup, and the MMA warpgroups at BN = 256) run this, so their outputs are the same bits.
+// bias / time-embedding / residual / GEGLU / GELU -> fp16 (or fp32) -> 16-byte stores. The epilogue warpgroup
+// (BN <= 160) runs this.
 // The fast variants call loaded() once the run's accumulator is in registers (every thread of the caller reaches it)
 // and hand each 16-byte group g of output columns [col, col + 8) to st16(col, g, value); the generic ones store to
 // out_row themselves.
@@ -180,37 +205,28 @@ __device__ __forceinline__ void finish_run(const ConvGemmParams& p, const Ld& ld
             // this chunk's 64 accumulator columns start at cbias; block g/2 holds [16 value | 16 gate]
             const float2 bv = *reinterpret_cast<const float2*>(cbias + (g >> 1) * 32 + j);
             const float2 bg = *reinterpret_cast<const float2*>(cbias + (g >> 1) * 32 + 16 + j);
-            const F2 val = f2_add(f2_make(__uint_as_float(vv[j]), __uint_as_float(vv[j + 1])), f2_make(bv.x, bv.y));
-            const F2 gat = f2_add(f2_make(__uint_as_float(vv[16 + j]), __uint_as_float(vv[16 + j + 1])),
-                                  f2_make(bg.x, bg.y));
-            float x0, x1;
-            f2_get(geglu2(val, gat), x0, x1);
-            const __half2 h2 = __floats2half2_rn(x0, x1);
-            o[e] = *reinterpret_cast<const uint32_t*>(&h2);
+            o[e] = epi_geglu2(f2_make(__uint_as_float(vv[j]), __uint_as_float(vv[j + 1])), f2_make(bv.x, bv.y),
+                              f2_make(__uint_as_float(vv[16 + j]), __uint_as_float(vv[16 + j + 1])), f2_make(bg.x, bg.y));
           }
         } else {
-          float4 b0 = *reinterpret_cast<const float4*>(cbias + 8 * g);
-          float4 b1 = *reinterpret_cast<const float4*>(cbias + 8 * g + 4);
+          const float4 b0 = *reinterpret_cast<const float4*>(cbias + 8 * g);
+          const float4 b1 = *reinterpret_cast<const float4*>(cbias + 8 * g + 4);
+          F2 bb[4] = {f2_make(b0.x, b0.y), f2_make(b0.z, b0.w), f2_make(b1.x, b1.y), f2_make(b1.z, b1.w)};
           if (radd) {
             const float4 a0 = __ldg(reinterpret_cast<const float4*>(radd + nbase) + 2 * g);
             const float4 a1 = __ldg(reinterpret_cast<const float4*>(radd + nbase) + 2 * g + 1);
-            b0.x += a0.x; b0.y += a0.y; b0.z += a0.z; b0.w += a0.w;
-            b1.x += a1.x; b1.y += a1.y; b1.z += a1.z; b1.w += a1.w;
+            bb[0] = epi_rowadd2(bb[0], make_float2(a0.x, a0.y));
+            bb[1] = epi_rowadd2(bb[1], make_float2(a0.z, a0.w));
+            bb[2] = epi_rowadd2(bb[2], make_float2(a1.x, a1.y));
+            bb[3] = epi_rowadd2(bb[3], make_float2(a1.z, a1.w));
           }
-          const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-          const __half2* rh2 = reinterpret_cast<const __half2*>(&rcur[g]);
+          const uint32_t* rh2 = reinterpret_cast<const uint32_t*>(&rcur[g]);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const int j = g * 8 + 2 * e;
-            F2 x = f2_add(f2_make(__uint_as_float(v[j]), __uint_as_float(v[j + 1])), f2_make(bb[2 * e], bb[2 * e + 1]));
-            if constexpr (kEpi == kEpiResidual) {
-              const float2 rr = __half22float2(rh2[e]);
-              x = f2_fma(x, alpha2, f2_make(rr.x, rr.y));
-            }
-            float x0, x1;
-            f2_get(x, x0, x1);
-            const __half2 h2 = __floats2half2_rn(x0, x1);
-            o[e] = *reinterpret_cast<const uint32_t*>(&h2);
+            const F2 x = f2_make(__uint_as_float(v[j]), __uint_as_float(v[j + 1]));
+            if constexpr (kEpi == kEpiResidual) o[e] = epi_residual2(x, bb[e], alpha2, rh2[e]);
+            else o[e] = epi_plain2(x, bb[e]);
           }
         }
         st16(oc + 8 * g, g, make_uint4(o[0], o[1], o[2], o[3]));
@@ -317,76 +333,67 @@ __device__ __forceinline__ void finish_run(const ConvGemmParams& p, const Ld& ld
   }
 }
 
-// In-line epilogue of one tile (BN = 256): MMA warpgroup wg finishes its own 64 accumulator rows. The accumulator goes
-// through the warpgroup's padded fp32 slice 128 columns at a time; thread t takes row t % 64 and, with the other half
-// of the warpgroup, alternating 32-column runs.
+// Epilogue of one tile at BN = 256 (plain / residual / GEGLU), on the accumulator fragments of MMA thread (wq, lane) of
+// warpgroup wg: tile rows r0 = 64 wg + 16 wq + lane / 4 and r0 + 8, column pairs 8 i + 2 (lane % 4) of 8-column block
+// i (acc[4 i .. 4 i + 1] and acc[4 i + 2 .. 4 i + 3]). Every step is element-wise: a GEGLU value pair (block i, i % 4
+// < 2) and its gate pair (block i + 2) sit in the same thread. The fp16 results go to the output tile in the layout of
+// the TMA boxes: [runs of 32 output columns][128 rows][64 bytes], 16-byte chunk g of row r at g ^ ((r >> 1) & 3). A
+// warp's 4-byte writes of one block cover 8 rows x 4 lanes on 32 distinct banks. The residual variant reads its
+// residual from the location it then writes.
 template <int kEpi, int BN>
-__device__ __forceinline__ void inline_epilogue_tile(const ConvGemmParams& p, const float (&acc)[BN / 2], float* sacc,
-                                                     float* sbias, int unit, int wg, int t) {
-  const int lane = t & 31;
-  const int wq = t >> 5;
-  const int row_local = t & 63;
-  const int half = t >> 6;
-  const int r = 64 * wg + row_local;
-  float* acc_slice = sacc + wg * 64 * kAccLd;
-  float* wbias = sbias + wg * 256;
-  const bool use_res = (p.res != nullptr) && !p.geglu && !p.out_f32;
-  const int acc_step = p.geglu ? 64 : 32;             // accumulator columns consumed per 32 output columns
+__device__ __forceinline__ void fragment_epilogue(const ConvGemmParams& p, const float (&acc)[BN / 2], uint8_t* sout,
+                                                  const float* sbias, int unit, int r0, int q) {
   const int nt = unit % p.tiles_nn;
   const int mt = unit / p.tiles_nn;
-  const int tw = mt % p.tiles_w;
-  const int th = (mt / p.tiles_w) % p.tiles_h;
-  const int tn = mt / (p.tiles_w * p.tiles_h);
   const int ncol0 = nt * BN;
-  const int rw = r % p.bw;
-  const int rh = (r / p.bw) % p.bh;
-  const int rn = r / (p.bw * p.bh);
-  const int w = tw * p.bw + rw, h = th * p.bh + rh, n = tn * p.bn + rn;
-  const bool row_ok = (w < p.W) && (h < p.H) && (n < p.NF);
-  const long long m = ((long long)n * p.H + h) * p.W + w;
-  const float* radd = (p.rowadd && row_ok) ? p.rowadd + (long long)(m / p.rows_per_group) * p.ld_rowadd : nullptr;
-  const __half* res_row = use_res ? p.res + m * p.ld_res : nullptr;
-  __half* out_row = reinterpret_cast<__half*>(p.out) + m * p.ldc;
-
-  uint4 rcur[4] = {};
-  auto load_res = [&](int c0) {
-    if (!use_res || !row_ok) return;
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const int nn = ncol0 + c0 + g * 8;
-      if (c0 + g * 8 < BN && nn < p.N) rcur[g] = __ldg(reinterpret_cast<const uint4*>(res_row + nn));
-    }
+  auto dst = [&](int blk, int h) {          // output 8-column block blk of tile row r0 + 8 h, this lane's 4 bytes
+    const int r = r0 + 8 * h;
+    return reinterpret_cast<uint32_t*>(sout + (blk >> 2) * kRunBytes + r * 64 + 16 * ((blk & 3) ^ ((r >> 1) & 3)) + 4 * q);
   };
-  named_bar_sync(1 + wg, 128);                      // the previous tile's reads of the bias / accumulator slices are done
-  if constexpr (kEpi != kEpiGeneric && kEpi != kEpiAct) {
-    for (int c = t; c < BN; c += 128) wbias[c] = (p.bias && ncol0 + c < p.N) ? __ldg(p.bias + ncol0 + c) : 0.f;
-  }
+  if constexpr (kEpi == kEpiGeglu) {
 #pragma unroll
-  for (int u = 0; u < (BN + 127) / 128; ++u) {
-    if (u > 0) named_bar_sync(1 + wg, 128);         // previous slice consumed
-    // accumulator fragment (rows 16 wq + lane/4 (+8), columns 8 i + 2 (lane%4)) -> fp32 slice, columns [128 u, 128 u + 128)
+    for (int i = 0; i < BN / 8; ++i) {
+      if ((i & 2) || ncol0 + 64 * (i >> 3) >= p.N) continue;   // gate blocks; 64-column chunks wholly past N
+      const int col = 8 * i + 2 * q;
+      const float2 bv = *reinterpret_cast<const float2*>(sbias + col);
+      const float2 bg = *reinterpret_cast<const float2*>(sbias + col + 16);
 #pragma unroll
-    for (int i = 16 * u; i < 16 * u + 16 && i < BN / 8; ++i) {
-      const int rr = 16 * wq + (lane >> 2);
-      const int cc = 8 * (i - 16 * u) + 2 * (lane & 3);
-      *reinterpret_cast<float2*>(acc_slice + rr * kAccLd + cc) = make_float2(acc[4 * i], acc[4 * i + 1]);
-      *reinterpret_cast<float2*>(acc_slice + (rr + 8) * kAccLd + cc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+      for (int h = 0; h < 2; ++h)
+        *dst(2 * (i >> 2) + (i & 1), h) =
+            epi_geglu2(f2_make(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]), f2_make(bv.x, bv.y),
+                       f2_make(acc[4 * (i + 2) + 2 * h], acc[4 * (i + 2) + 2 * h + 1]), f2_make(bg.x, bg.y));
     }
-    named_bar_sync(1 + wg, 128);
-    const int cend = (128 * u + 128 < BN) ? 128 * u + 128 : BN;
-    for (int c0 = 128 * u + half * acc_step; c0 < cend; c0 += 2 * acc_step) {
-      const float* srow = acc_slice + row_local * kAccLd - 128 * u;
-      auto ld32 = [&](int col, uint32_t (&v)[32]) {
+  } else {
+    // time-embedding rows of the two tile rows; a row outside the image reads group 0 (its outputs are clipped)
+    const float* radd[2] = {nullptr, nullptr};
+    if (p.rowadd) {
+      const int tw = mt % p.tiles_w;
+      const int th = (mt / p.tiles_w) % p.tiles_h;
+      const int tn = mt / (p.tiles_w * p.tiles_h);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const float4 x = *reinterpret_cast<const float4*>(srow + col + 4 * k);
-          v[4 * k] = __float_as_uint(x.x); v[4 * k + 1] = __float_as_uint(x.y);
-          v[4 * k + 2] = __float_as_uint(x.z); v[4 * k + 3] = __float_as_uint(x.w);
-        }
-      };
-      load_res(c0);
-      finish_run<kEpi>(p, ld32, [] {}, [&](int col, int, uint4 o) { *reinterpret_cast<uint4*>(out_row + col) = o; },
-                       c0, ncol0, wbias, radd, rcur, row_ok, use_res, m, out_row);
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h;
+        const int w = tw * p.bw + r % p.bw, hh = th * p.bh + (r / p.bw) % p.bh, n = tn * p.bn + r / (p.bw * p.bh);
+        const bool row_ok = (w < p.W) && (hh < p.H) && (n < p.NF);
+        const long long m = ((long long)n * p.H + hh) * p.W + w;
+        radd[h] = p.rowadd + (row_ok ? m / p.rows_per_group : 0) * p.ld_rowadd + ncol0;
+      }
+    }
+    const F2 alpha2 = f2_make(p.alpha, p.alpha);
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      if (ncol0 + 32 * (i >> 2) >= p.N) continue;             // N % 32 == 0: runs wholly past N
+      const int col = 8 * i + 2 * q;
+      const float2 bs = *reinterpret_cast<const float2*>(sbias + col);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        F2 b = f2_make(bs.x, bs.y);
+        if (p.rowadd) b = epi_rowadd2(b, __ldg(reinterpret_cast<const float2*>(radd[h] + col)));
+        const F2 x = f2_make(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+        uint32_t* o = dst(i, h);
+        if constexpr (kEpi == kEpiResidual) *o = epi_residual2(x, b, alpha2, *o);
+        else *o = epi_plain2(x, b);
+      }
     }
   }
 }
@@ -399,6 +406,7 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
   constexpr bool kTma = tma_epilogue(kEpi, BN);
   constexpr bool kResRing = res_ring_bytes(kEpi, BN) > 0;
   static_assert(BN % 32 == 0 && (BN <= kMaxStagedN || kInline), "the staging swizzle and the epilogue take whole 32-column runs");
+  static_assert(!kInline || kTma, "BN = 256 has the fragment epilogue of the plain / residual / GEGLU variants only");
   // the producer gives its registers away; an MMA thread holds BN / 2 accumulators (and, in line, runs the epilogue),
   // an epilogue thread one row's 32- or 64-column run plus the next run's residual
   constexpr int kProducerRegs = 40, kConsumerRegs = kInline ? 232 : 152, kEpilogueRegs = kInline ? 0 : 168;
@@ -414,15 +422,17 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
   // staging: [BN / 32 runs][128 rows][32] fp32; 16-byte chunk j of row r sits at chunk j ^ (r & 7), so that both the
   // fragment writes (8 rows x 2 chunks per warp store) and the row reads (32 rows, one chunk each) are free of bank
   // conflicts. The TMA epilogue writes a run's fp16 outputs over the first 8 KB of that run's 16 KB once every row has
-  // been read. In line (BN = 256): [2 warpgroups][64][kAccLd] slices.
+  // been read. In line (BN = 256) the same place holds the fp16 output tile (fragment_epilogue).
   float* stg = reinterpret_cast<float*>(smem + kRingEnd);
   uint8_t* sres = smem + kRingEnd + epi_buf_bytes(BN);                  // [kResSlots][128 rows][64 bytes], residual only
-  float* sbias = reinterpret_cast<float*>(sres + res_ring_bytes(kEpi, BN));  // [BN], in line [2 warpgroups][256]
+  float* sbias = reinterpret_cast<float*>(sres + res_ring_bytes(kEpi, BN));  // [BN]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sres + res_ring_bytes(kEpi, BN) + bias_buf_bytes(BN));
   uint64_t* full = bars;                       // [kMaxStages]
   uint64_t* empty = bars + kMaxStages;         // [kMaxStages]
-  uint64_t* acc_full = bars + 2 * kMaxStages;  // the staging holds a finished tile
-  uint64_t* acc_empty = acc_full + 1;          // the epilogue has read it
+  uint64_t* acc_full = bars + 2 * kMaxStages;  // the staging holds a finished tile (in line: out_full)
+  uint64_t* acc_empty = acc_full + 1;          // the epilogue has read it (in line: out_ready)
+  uint64_t* out_full = acc_full;               // in line: the output tile holds a finished tile
+  uint64_t* out_ready = acc_empty;             // in line: its stores have read it; the next tile's bias (and residual) is in
   uint64_t* res_full = acc_full + 2;           // [kResSlots] a residual run has landed
   uint64_t* res_empty = res_full + kResSlots;  // [kResSlots] the epilogue has read it
   static_assert(2 * kMaxStages + 2 + 2 * kResSlots <= 256 / 8, "barrier area");
@@ -445,7 +455,7 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
       mbar_init(&empty[s], 8);                 // one arrival per consumer warp
     }
     mbar_init(acc_full, 8);                    // one arrival per consumer warp
-    mbar_init(acc_empty, 4);                   // one arrival per epilogue warp
+    mbar_init(acc_empty, kInline ? 1 : 4);     // one arrival per epilogue warp; in line, warp 1's storing lane
     for (int s = 0; s < kResSlots; ++s) {
       mbar_init(&res_full[s], 1);
       mbar_init(&res_empty[s], 1);             // the epilogue thread that stores the run
@@ -518,6 +528,61 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
           if (++slot == kResSlots) { slot = 0; phase ^= 1; }
         }
       }
+    } else if (kInline && warp == 1) {
+      // output warp (BN = 256): stores each finished tile's runs, then readies the output tile for the next tile: its
+      // bias, and for the residual variant its residual runs, TMA-loaded into the tile. Lane 0 issues every bulk copy,
+      // so that its bulk-group waits cover them.
+      const int runs = kEpi == kEpiGeglu ? BN / 64 : BN / 32;   // 32-column runs of outputs (and residuals)
+      const int run_cols = kEpi == kEpiGeglu ? 64 : 32;         // accumulator columns per run
+      uint8_t* sout = smem + kRingEnd;
+      auto ready = [&](int unit) {
+        const int nt = unit % p.tiles_nn;
+        const int mt = unit / p.tiles_nn;
+        const int tw = mt % p.tiles_w;
+        const int th = (mt / p.tiles_w) % p.tiles_h;
+        const int tn = mt / (p.tiles_w * p.tiles_h);
+        const int ncol0 = nt * BN;
+        for (int c = lane; c < BN; c += 32) sbias[c] = (p.bias && ncol0 + c < p.N) ? __ldg(p.bias + ncol0 + c) : 0.f;
+        __syncwarp();
+        if (lane == 0) {
+          if constexpr (kEpi == kEpiResidual) {
+            int nruns = 0;
+            while (nruns < runs && ncol0 + run_cols * nruns < p.N) ++nruns;
+            mbar_expect_tx(out_ready, nruns * kRunBytes);
+            for (int k = 0; k < nruns; ++k)
+              tma_load_4d(sout + k * kRunBytes, &tmE.res, out_ready, ncol0 + 32 * k, tw * p.bw, th * p.bh, tn * p.bn);
+          } else {
+            mbar_arrive(out_ready);
+          }
+        }
+        __syncwarp();
+      };
+      uint32_t phase = 0;
+      ready(blockIdx.x);
+      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+        mbar_wait(out_full, phase);
+        phase ^= 1;
+        if (lane == 0) {                          // rows outside the image are clipped by the tensor map
+          const int nt = unit % p.tiles_nn;
+          const int mt = unit / p.tiles_nn;
+          const int tw = mt % p.tiles_w;
+          const int th = (mt / p.tiles_w) % p.tiles_h;
+          const int tn = mt / (p.tiles_w * p.tiles_h);
+          const int ncol0 = nt * BN;
+          for (int k = 0; k < runs && ncol0 + run_cols * k < p.N; ++k)
+            tma_store_4d(&tmE.out, sout + k * kRunBytes, (kEpi == kEpiGeglu ? ncol0 / 2 : ncol0) + 32 * k, tw * p.bw,
+                         th * p.bh, tn * p.bn);
+          tma_store_commit();
+        }
+        if (unit + (int)gridDim.x < num_units) {
+          // the MMA warpgroups read this tile's bias before they arrived on out_full; the next tile's residual
+          // overwrites the output tile, so the stores must have read it
+          if (lane == 0) tma_store_wait_read<0>();
+          __syncwarp();
+          ready(unit + gridDim.x);
+        }
+      }
+      if (lane == 0) tma_store_wait_all();
     }
     return;
   }
@@ -672,7 +737,13 @@ conv_gemm_kernel(const __grid_constant__ AMaps tmA, const __grid_constant__ CUte
     if (lane == 0) mbar_arrive(&empty[prev_stage]);
 
     if constexpr (kInline) {
-      inline_epilogue_tile<kEpi, BN>(p, acc, stg, sbias, unit, wg, t);
+      // ---- finish the tile in registers once warp 1 has readied the output tile, and hand it to warp 1
+      mbar_wait(out_ready, acc_phase);
+      fragment_epilogue<kEpi, BN>(p, acc, smem + kRingEnd, sbias, unit, 64 * wg + 16 * wq + (lane >> 2), lane & 3);
+      fence_proxy_async();                       // the TMA stores read what this thread wrote
+      __syncwarp();
+      if (lane == 0) mbar_arrive(out_full);
+      acc_phase ^= 1;
     } else {
       // ---- hand the tile to the epilogue warpgroup once it has read the previous one, then go on to the next tile
       mbar_wait(acc_empty, acc_phase ^ 1);
@@ -847,15 +918,16 @@ static void pick_box(int W, int H, int NF, int* bw, int* bh, int* bn) {
 // channels exactly; the GEGLU epilogue needs whole 64-column [value | gate] chunks.
 static const int kBlockNs[4] = {64, 128, 160, 256};
 
-// The GELU epilogue (kEpiAct) is not instantiated at 256 columns, where the generic epilogue it extends spills 8 bytes.
-static int pick_block_n(int N, int geglu, int gelu, long long tiles_m, int num_sms) {
+// 256-column tiles finish on the accumulator fragments, which the plain / residual / GEGLU variants do (wide_ok); the
+// generic and GELU epilogues are not instantiated at that width.
+static int pick_block_n(int N, int geglu, bool wide_ok, long long tiles_m, int num_sms) {
   // prefer few padded columns, then fewer waves
   int best = 0;
   double best_cost = 1e30;
   for (int i = 3; i >= 0; --i) {
     const int bn = kBlockNs[i];
     if (geglu && (bn % 64)) continue;
-    if (gelu && bn == 256) continue;
+    if (!wide_ok && bn == 256) continue;
     const int tn = ceil_div(N, bn);
     const long long tiles = tiles_m * tn;
     const long long waves = (tiles + num_sms - 1) / num_sms;
@@ -874,8 +946,8 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   {conv_gemm_kernel<kEpiGeneric, BN>, conv_gemm_kernel<kEpiPlain, BN>, conv_gemm_kernel<kEpiResidual, BN>, \
    conv_gemm_kernel<kEpiGeglu, BN>, conv_gemm_kernel<kEpiAct, BN>}
   static const KernelFn kernels[4][5] = {MVB_GEMM_ROW(64), MVB_GEMM_ROW(128), MVB_GEMM_ROW(160),
-                                         {conv_gemm_kernel<kEpiGeneric, 256>, conv_gemm_kernel<kEpiPlain, 256>,
-                                          conv_gemm_kernel<kEpiResidual, 256>, conv_gemm_kernel<kEpiGeglu, 256>, nullptr}};
+                                         {nullptr, conv_gemm_kernel<kEpiPlain, 256>, conv_gemm_kernel<kEpiResidual, 256>,
+                                          conv_gemm_kernel<kEpiGeglu, 256>, nullptr}};
 #undef MVB_GEMM_ROW
   // the opt-in is per device: key the "already set" state by the current device ordinal
   static bool attr_set_dev[64] = {};
@@ -893,8 +965,17 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
     attr_set = true;
   }
   const long long tiles_m = (long long)p.tiles_w * p.tiles_h * p.tiles_n;
-  const int gelu = ep.act == 2 || ep.act == 3;
-  p.block_n = pick_block_n(p.N, ep.geglu, gelu, tiles_m, num_sms);
+  // epilogue variant: the fast ones need whole 32-column chunks and the common alpha / beta
+  int epi = kEpiGeneric;
+  if (!ep.out_f32 && ep.act == 0) {
+    if (ep.geglu) { if (p.N % 64 == 0 && !ep.rowadd) epi = kEpiGeglu; }
+    else if (p.N % 32 == 0) {
+      if (ep.res && ep.beta == 1.f) epi = kEpiResidual;
+      else if (!ep.res && ep.alpha == 1.f) epi = kEpiPlain;
+    }
+  }
+  if (ep.act == 2 || ep.act == 3) epi = kEpiAct;
+  p.block_n = pick_block_n(p.N, ep.geglu, tma_epilogue(epi, 256), tiles_m, num_sms);
   int bn_idx = 0;
   while (kBlockNs[bn_idx] != p.block_n) ++bn_idx;
   p.tiles_nn = ceil_div(p.N, p.block_n);
@@ -918,16 +999,6 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   }
   const long long num_tiles = tiles_m * p.tiles_nn;
   const int grid = (int)(num_tiles < num_sms ? num_tiles : num_sms);
-  // epilogue variant: the fast ones need whole 32-column chunks and the common alpha / beta
-  int epi = kEpiGeneric;
-  if (!ep.out_f32 && ep.act == 0) {
-    if (ep.geglu) { if (p.N % 64 == 0 && !ep.rowadd) epi = kEpiGeglu; }
-    else if (p.N % 32 == 0) {
-      if (ep.res && ep.beta == 1.f) epi = kEpiResidual;
-      else if (!ep.res && ep.alpha == 1.f) epi = kEpiPlain;
-    }
-  }
-  if (gelu) epi = kEpiAct;
   p.stage_bytes = ring_stage_bytes(p.block_n);
   p.nstages = ring_stages(epi, p.block_n);
   // the TMA epilogue's output (and residual) views: {columns, W, H, NF} with the tile's pixel box, one 32-column run

@@ -325,6 +325,12 @@ typedef struct mvb_controlnet_args {
   int out_is_f32;
   int out_frames;                                   /* ReferenceNet only (`num_frames`, referencenet.py:1041-1049): outputs are
                                                        [NF / out_frames, C_k, out_frames, h_k, w_k]; 0 or 1 = (b t) c h w */
+  int accumulate;                                   /* ControlNet only (since mvb_version 6): 0 writes outs[k]; 1 adds the
+                                                       scaled maps into the tensors already in outs[k] (fp32 sum, rounded
+                                                       once to the output dtype), the Multi-ControlNet sum of
+                                                       diffusers multicontrolnet.py:64-70 for the second and later nets.
+                                                       With 1, a ReferenceNet handle or a NULL outs[k] is MVB_ERR_INVALID
+                                                       and nothing is launched. */
 } mvb_controlnet_args;
 int mvb_create_controlnet(const mvb_config* cfg, int device, mvb_handle** out);
 long long mvb_controlnet_workspace_bytes(mvb_handle* h, const mvb_controlnet_args* args);

@@ -107,6 +107,7 @@ class MvbControlnetArgs(C.Structure):
         ("outs", C.c_void_p * MAX_OUT),
         ("out_is_f32", C.c_int),
         ("out_frames", C.c_int),
+        ("accumulate", C.c_int),
     ]
 
 

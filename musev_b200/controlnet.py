@@ -7,6 +7,10 @@ scaling run inside libmusevb200.so (`mvb_controlnet_forward`, musev_b200/csrc/en
 call and passes `controlnet_cond_latents` on every step (pipeline_controlnet.py:1258), so it stays a handful of torch
 convolutions here, outside the per-step path.
 
+`MultiControlNetModel` (diffusers pipelines/controlnet/multicontrolnet.py:15-72) runs several ControlNets on one input and
+sums their maps: the second and later nets add into the first net's output tensors inside the engine
+(`mvb_controlnet_args.accumulate`).
+
 `PoseGuider` (musev/models/controlnet.py:326-399) is the pose-guided video2video encoder: eight 3x3 convolutions run once per
 pipeline call on the pose images (`mvb_pose_guider_forward`, `Engine::run_pose_guider`); its output is the UNet's
 `pose_guider_emb`.
@@ -15,7 +19,7 @@ from __future__ import annotations
 
 from dataclasses import asdict
 from types import SimpleNamespace
-from typing import Any, Dict, List, Optional, Tuple, Union
+from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 import torch.nn.functional as F
@@ -100,8 +104,13 @@ class ControlNetModel(EngineModel):
         guess_mode: bool = False,
         return_dict: bool = True,
         controlnet_cond_latents: Optional[torch.Tensor] = None,
+        accumulate_into: Optional[Tuple[List[torch.Tensor], torch.Tensor]] = None,
     ):
-        """Reference: ControlNetModel.forward, diffusers models/controlnet.py:645-852."""
+        """Reference: ControlNetModel.forward, diffusers models/controlnet.py:645-852.
+
+        accumulate_into: the `(down, mid)` an earlier call returned. This call's scaled maps are then added into those
+        tensors on the device (fp32 sum, one rounding to their dtype) and they are returned: the Multi-ControlNet sum
+        `samples_prev + samples_curr` of diffusers multicontrolnet.py:64-70, without a second set of maps."""
         self._check_loaded()
         for name, v in (("class_labels", class_labels), ("timestep_cond", timestep_cond), ("attention_mask", attention_mask),
                         ("added_cond_kwargs", added_cond_kwargs)):
@@ -129,7 +138,17 @@ class ControlNetModel(EngineModel):
             scales = (torch.logspace(-1, 0, n_out) * scale).tolist()
         else:            # :831-833
             scales = [scale] * n_out
-        outs = [torch.empty((NF, c, H // ds, W // ds), device=dev, dtype=self.dtype) for c, ds in self._maps]
+        if accumulate_into is None:
+            outs = [torch.empty((NF, c, H // ds, W // ds), device=dev, dtype=self.dtype) for c, ds in self._maps]
+        else:
+            outs = list(accumulate_into[0]) + [accumulate_into[1]]
+            if len(outs) != n_out:
+                raise ValueError(f"accumulate_into holds {len(outs)} maps; this ControlNet has {n_out}")
+            for o, (c, ds) in zip(outs, self._maps):
+                if (tuple(o.shape) != (NF, c, H // ds, W // ds) or o.device != dev or o.dtype != outs[0].dtype
+                        or o.dtype not in (torch.float16, torch.float32) or not o.is_contiguous()):
+                    raise ValueError(f"accumulate_into: a map of shape {tuple(o.shape)} ({o.dtype}, {o.device}) is not the "
+                                     f"contiguous {(NF, c, H // ds, W // ds)} map on {dev} this call adds into")
         a = MvbControlnetArgs()
         a.sample, a.sample_is_f32 = sample.data_ptr(), _is_f32(sample)
         a.NF, a.H, a.W = NF, H, W
@@ -141,11 +160,91 @@ class ControlNetModel(EngineModel):
             a.scales[k] = scales[k]
             a.outs[k] = outs[k].data_ptr()
         a.out_is_f32 = _is_f32(outs[0])
+        a.accumulate = int(accumulate_into is not None)
         self._launch(a)
         down, mid = outs[:-1], outs[-1]
         if not return_dict:
             return (down, mid)
         return ControlNetOutput(down_block_res_samples=down, mid_block_res_sample=mid)
+
+    __call__ = forward
+
+
+def _geometry(net) -> Tuple:
+    """What fixes the shapes of a ControlNet's 12 + 1 residual maps (controlnet.py:181-447)."""
+    c = net.config
+    return (tuple(c.block_out_channels), c.layers_per_block, c.cross_attention_dim)
+
+
+class MultiControlNetModel:
+    """Several ControlNets whose residual maps are summed, behind the call surface of diffusers `MultiControlNetModel`
+    (diffusers/src/diffusers/pipelines/controlnet/multicontrolnet.py:15-72). The first net writes the 12 + 1 output
+    tensors; every later net adds its maps into them on the device (`accumulate_into`), in net order, so the sum rounds
+    as the reference's `samples_prev + samples_curr` does."""
+
+    def __init__(self, controlnets: Sequence[Any]):
+        nets = list(controlnets)
+        if not nets:
+            raise ValueError("For multiple controlnets: `controlnets` must hold at least one ControlNet")
+        for k, n in enumerate(nets[1:], 1):
+            if _geometry(n) != _geometry(nets[0]):
+                raise ValueError(f"For multiple controlnets: ControlNet {k} has block_out_channels / layers_per_block / "
+                                 f"cross_attention_dim {_geometry(n)}, ControlNet 0 has {_geometry(nets[0])}; their "
+                                 "residuals cannot be summed")
+            if torch.device(n.device) != torch.device(nets[0].device) or n.dtype != nets[0].dtype:
+                raise ValueError(f"For multiple controlnets: ControlNet {k} is on {n.device} in {n.dtype}, ControlNet 0 on "
+                                 f"{nets[0].device} in {nets[0].dtype}; every net must share one device and dtype")
+        self.nets = nets
+
+    @property
+    def dtype(self) -> torch.dtype:
+        return self.nets[0].dtype
+
+    @property
+    def device(self) -> torch.device:
+        return self.nets[0].device
+
+    def check_list(self, name: str, values) -> list:
+        """diffusers check_inputs (pipelines/controlnet/pipeline_controlnet.py:570-615): one entry per ControlNet."""
+        if not isinstance(values, (list, tuple)):
+            raise ValueError(f"For multiple controlnets: `{name}` must be type `list`")
+        if len(values) != len(self.nets):
+            raise ValueError(f"For multiple controlnets: `{name}` must have the same length as the number of controlnets, "
+                             f"but got {len(values)} entries and {len(self.nets)} ControlNets.")
+        return list(values)
+
+    @torch.no_grad()
+    def forward(
+        self,
+        sample: torch.Tensor,
+        timestep: Union[torch.Tensor, float, int],
+        encoder_hidden_states: torch.Tensor,
+        controlnet_cond: Optional[List[torch.Tensor]],
+        conditioning_scale: List[float],
+        class_labels: Optional[torch.Tensor] = None,
+        timestep_cond: Optional[torch.Tensor] = None,
+        attention_mask: Optional[torch.Tensor] = None,
+        added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None,
+        cross_attention_kwargs: Optional[Dict[str, Any]] = None,
+        guess_mode: bool = False,
+        return_dict: bool = True,
+        controlnet_cond_latents: Optional[List[torch.Tensor]] = None,
+    ):
+        """multicontrolnet.py:31-72. Returns `(down, mid)` whatever `return_dict` says, as the reference does. Without a
+        `controlnet_cond_latents` list each net embeds its own image (`controlnet_cond_embedding`); `controlnet_cond` may
+        be None when the list is given."""
+        n = len(self.nets)
+        scales = self.check_list("controlnet_conditioning_scale", conditioning_scale)
+        lats = self.check_list("controlnet_cond_latents", controlnet_cond_latents) \
+            if isinstance(controlnet_cond_latents, (list, tuple)) else [None] * n
+        images = self.check_list("image", controlnet_cond) if controlnet_cond is not None else [None] * n
+        res = None
+        for net, image, scale, lat in zip(self.nets, images, scales, lats):
+            res = net(sample, timestep, encoder_hidden_states, controlnet_cond=image, conditioning_scale=scale,
+                      class_labels=class_labels, timestep_cond=timestep_cond, attention_mask=attention_mask,
+                      added_cond_kwargs=added_cond_kwargs, cross_attention_kwargs=cross_attention_kwargs,
+                      guess_mode=guess_mode, return_dict=False, controlnet_cond_latents=lat, accumulate_into=res)
+        return res
 
     __call__ = forward
 

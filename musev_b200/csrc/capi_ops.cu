@@ -35,8 +35,8 @@ extern "C" {
 const char* mvb_last_error(void) { return g_err; }
 
 // 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle; 4: the CLIP text handle, causal attention;
-// 5: mvb_fuse_cfg_multistep
-int mvb_version(void) { return 5; }
+// 5: mvb_fuse_cfg_multistep; 6: mvb_controlnet_args.accumulate
+int mvb_version(void) { return 6; }
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   if (!d || !d->a0 || !d->weight || !d->out) return fail("mvb_op_conv_gemm: null pointer", cudaSuccess);

@@ -148,7 +148,9 @@ bool Engine::run_controlnet(const mvb_controlnet_args& a, Arena& ar, cudaStream_
     }
     if (!ar.dry && f.ok) {
       if (!a.outs[k]) { err_ = "controlnet: null output pointer"; return false; }
-      cudaError_t e = tokens_to_ncthw(s, o, t.C, NF / out_t, t.C, out_t, t.H * t.W, a.outs[k], a.out_is_f32);
+      cudaError_t e = a.accumulate   // Multi-ControlNet: outs[k] += this net's map (multicontrolnet.py:64-70)
+          ? tokens_to_ncthw_add(s, o, t.C, NF, t.C, 1, t.H * t.W, a.outs[k], a.out_is_f32)
+          : tokens_to_ncthw(s, o, t.C, NF / out_t, t.C, out_t, t.H * t.W, a.outs[k], a.out_is_f32);
       if (e != cudaSuccess) f.fail("controlnet output", e);
     }
     f.release(mk);
@@ -162,6 +164,13 @@ long long Engine::controlnet_workspace_bytes(const mvb_controlnet_args& a) {
 int Engine::controlnet_forward(const mvb_controlnet_args& a, void* ws, long long wbytes, cudaStream_t stream) {
   const bool cond_missing = kind_ == Kind::ControlNet && !a.cond_latents;
   const char* bad = (!a.sample || cond_missing || !a.encoder_hidden_states || !ws) ? kNullArg : nullptr;
+  // accumulate reads outs[k], so every output is checked before anything is launched
+  if (!bad && a.accumulate) {
+    if (a.accumulate != 1) bad = "controlnet: accumulate must be 0 or 1";
+    else if (kind_ != Kind::ControlNet) bad = "accumulate = 1 is a ControlNet option; a ReferenceNet writes its maps";
+    for (int k = 0; !bad && k < a.n_out && k < MVB_CONTROLNET_MAX_OUT; ++k)
+      if (!a.outs[k]) bad = "controlnet: accumulate = 1 needs every outs[k] (it adds into them); outs[k] is NULL";
+  }
   return launch(&Engine::run_controlnet, {Kind::ControlNet, Kind::ReferenceNet}, "not a ControlNet / ReferenceNet handle", bad,
                 a, ws, wbytes, stream);
 }

@@ -4,6 +4,8 @@
 
 #include <math.h>
 
+#include <type_traits>
+
 #include "stats.cuh"
 
 namespace mvb {
@@ -705,6 +707,72 @@ cudaError_t tokens_to_ncthw(cudaStream_t s, const __half* x, int ldx, int B, int
   dim3 grid((HW + 31) / 32, (C + 31) / 32, B * T), block(32, 8);
   if (is_f32) tokens_to_ncthw_kernel<float><<<grid, block, 0, s>>>(x, ldx, B, C, T, HW, (float*)y);
   else tokens_to_ncthw_kernel<__half><<<grid, block, 0, s>>>(x, ldx, B, C, T, HW, (__half*)y);
+  return cudaGetLastError();
+}
+
+// y += x with the layout change of tokens_to_ncthw, one 64-pixel x 64-channel tile per block. The sum is taken in fp32
+// and rounded once to TOut, which is what torch's fp16 / fp32 `a + b` does. VC: halves per load along C (8 = 16 bytes),
+// VP: elements per access of y along the pixels (16 bytes); 1 / 1 when the map's sizes or pointers do not allow it.
+constexpr int kAddTile = 64;
+template <typename TOut, int VC, int VP>
+__global__ void __launch_bounds__(256) tokens_to_ncthw_add_kernel(const __half* __restrict__ x, int ldx, int C, int T,
+                                                                  int HW, TOut* __restrict__ y) {
+  __shared__ float tile[kAddTile][kAddTile + 1];   // [pixel][channel]
+  const int bt = blockIdx.z;
+  const int b = bt / T, t = bt % T;
+  const int p0 = blockIdx.x * kAddTile, c0 = blockIdx.y * kAddTile;
+  constexpr int NCV = kAddTile / VC, NPV = kAddTile / VP;
+  for (int i = threadIdx.x; i < kAddTile * NCV; i += blockDim.x) {
+    const int py = i / NCV, c = c0 + (i % NCV) * VC, p = p0 + py;
+    if (p >= HW || c >= C) continue;
+    const __half* src = x + ((size_t)bt * HW + p) * ldx + c;
+    if constexpr (VC == 8) {
+      const uint4 v = *reinterpret_cast<const uint4*>(src);
+      const __half2* h2 = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = __half22float2(h2[j]);
+        tile[py][c - c0 + 2 * j] = f.x;
+        tile[py][c - c0 + 2 * j + 1] = f.y;
+      }
+    } else {
+      tile[py][c - c0] = __half2float(*src);
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < kAddTile * NPV; i += blockDim.x) {
+    const int cy = i / NPV, px = (i % NPV) * VP, c = c0 + cy, p = p0 + px;
+    if (p >= HW || c >= C) continue;
+    TOut* dst = y + (((size_t)b * C + c) * T + t) * HW + p;
+    if constexpr (VP == 1) {
+      *dst = (TOut)((float)*dst + tile[px][cy]);
+    } else {
+      uint4 v = *reinterpret_cast<const uint4*>(dst);
+      if constexpr (std::is_same<TOut, float>::value) {
+        float* f = reinterpret_cast<float*>(&v);
+#pragma unroll
+        for (int j = 0; j < VP; ++j) f[j] += tile[px + j][cy];
+      } else {
+        __half* h = reinterpret_cast<__half*>(&v);
+#pragma unroll
+        for (int j = 0; j < VP; ++j) h[j] = __float2half_rn(__half2float(h[j]) + tile[px + j][cy]);
+      }
+      *reinterpret_cast<uint4*>(dst) = v;
+    }
+  }
+}
+template <typename TOut>
+static void launch_tokens_to_ncthw_add(cudaStream_t s, const __half* x, int ldx, int B, int C, int T, int HW, TOut* y) {
+  constexpr int VP = 16 / sizeof(TOut);
+  const bool vec = C % 8 == 0 && ldx % 8 == 0 && HW % VP == 0 && ((uintptr_t)x % 16) == 0 && ((uintptr_t)y % 16) == 0;
+  dim3 grid((HW + kAddTile - 1) / kAddTile, (C + kAddTile - 1) / kAddTile, B * T);
+  if (vec) tokens_to_ncthw_add_kernel<TOut, 8, VP><<<grid, 256, 0, s>>>(x, ldx, C, T, HW, y);
+  else tokens_to_ncthw_add_kernel<TOut, 1, 1><<<grid, 256, 0, s>>>(x, ldx, C, T, HW, y);
+}
+cudaError_t tokens_to_ncthw_add(cudaStream_t s, const __half* x, int ldx, int B, int C, int T, int HW, void* y, int is_f32) {
+  ProfScope prof(s, KC_OTHER);
+  if (is_f32) launch_tokens_to_ncthw_add(s, x, ldx, B, C, T, HW, (float*)y);
+  else launch_tokens_to_ncthw_add(s, x, ldx, B, C, T, HW, (__half*)y);
   return cudaGetLastError();
 }
 

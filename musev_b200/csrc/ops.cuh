@@ -31,6 +31,10 @@ cudaError_t ncthw_to_tokens(cudaStream_t s, const void* x, int is_f32, int B, in
                             int ldy, float scale);
 cudaError_t tokens_to_ncthw(cudaStream_t s, const __half* x, int ldx, int B, int C, int T, int HW, void* y,
                             int is_f32);
+// y += x in the same layouts: fp32 sum of y and x, rounded once to y's dtype (a second ControlNet's residual map added
+// into the first's, multicontrolnet.py:64-70)
+cudaError_t tokens_to_ncthw_add(cudaStream_t s, const __half* x, int ldx, int B, int C, int T, int HW, void* y,
+                                int is_f32);
 // add an NCHW ((b t) c h w) residual (ControlNet) to channels-last tokens in place.
 cudaError_t add_nchw_residual(cudaStream_t s, __half* x, int NF, int C, int HW, const void* r, int is_f32);
 // im2col of the 4-channel latent for conv_in: x NCTHW -> A [B*T*H*W, 64] fp16 with column (tap*Cin + c), zero padded.

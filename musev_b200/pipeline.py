@@ -11,7 +11,7 @@ per step, every window -> UNet -> accumulate eps; overlap mean; CFG; scheduler.s
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Callable, Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, Optional, Sequence, Union
 
 import torch
 
@@ -214,28 +214,80 @@ class ParallelDenoiser:
 
 
 
-def make_controlnet_fn(controlnet, controlnet_latents: torch.Tensor, prompt_embeds: torch.Tensor, n_vision_cond: int,
-                       controlnet_conditioning_scale: float = 1.0, guess_mode: bool = False,
-                       controlnet_keep: Optional[Sequence[float]] = None) -> Callable:
+def controlnet_keep_schedule(num_inference_steps: int, control_guidance_start: Union[float, Sequence[float]] = 0.0,
+                             control_guidance_end: Union[float, Sequence[float]] = 1.0,
+                             num_controlnets: Optional[int] = None) -> list:
+    """`controlnet_keep` of the reference: per step, 1.0 while a net's guidance window [start, end] covers the step and 0.0
+    outside it (musev/pipelines/pipeline_controlnet.py:1700-1711), after the start / end lists are aligned
+    (:1060-1083). num_controlnets: None for one `ControlNetModel` (a float per step), N for a Multi-ControlNet of N nets
+    (a list of N per step). The checks and their wording are diffusers' check_inputs
+    (pipelines/controlnet/pipeline_controlnet.py:601-615)."""
+    start, end = control_guidance_start, control_guidance_end
+    if not isinstance(start, (list, tuple)) and isinstance(end, (list, tuple)):          # :1060-1083
+        start = len(end) * [start]
+    elif not isinstance(end, (list, tuple)) and isinstance(start, (list, tuple)):
+        end = len(start) * [end]
+    elif not isinstance(start, (list, tuple)) and not isinstance(end, (list, tuple)):
+        mult = 1 if num_controlnets is None else num_controlnets
+        start, end = mult * [start], mult * [end]
+    if len(start) != len(end):
+        raise ValueError(f"`control_guidance_start` has {len(start)} elements, but `control_guidance_end` has {len(end)} "
+                         "elements. Make sure to provide the same number of elements to each list.")
+    n = 1 if num_controlnets is None else num_controlnets
+    if len(start) != n:
+        raise ValueError(f"`control_guidance_start`: {list(start)} has {len(start)} elements but there are {n} controlnets "
+                         f"available. Make sure to provide {n}.")
+    for s, e in zip(start, end):
+        if s >= e:
+            raise ValueError(f"control guidance start: {s} cannot be larger or equal to control guidance end: {e}.")
+        if s < 0.0:
+            raise ValueError(f"control guidance start: {s} can't be smaller than 0.")
+        if e > 1.0:
+            raise ValueError(f"control guidance end: {e} can't be larger than 1.0.")
+    keep = []
+    for i in range(num_inference_steps):                                                  # :1700-1711
+        keeps = [1.0 - float(i / num_inference_steps < s or (i + 1) / num_inference_steps > e) for s, e in zip(start, end)]
+        keep.append(keeps[0] if num_controlnets is None else keeps)
+    return keep
+
+
+def make_controlnet_fn(controlnet, controlnet_latents, prompt_embeds: torch.Tensor, n_vision_cond: int,
+                       controlnet_conditioning_scale: Union[float, Sequence[float]] = 1.0, guess_mode: bool = False,
+                       controlnet_keep: Optional[Sequence] = None) -> Callable:
     """The per-window-step ControlNet call of the reference loop as a `controlnet_fn` for `ParallelDenoiser`
     (musev/pipelines/pipeline_controlnet.py:1992-2038 window slicing, :1202-1291 `get_controlnet_emb`).
 
     controlnet_latents: [2B, C0, n_vc + T, h, w] -- the condition embedding of every frame, vision-condition frame(s) first,
     already duplicated for CFG ([B, ...] in guess mode); computed once per call (`controlnet_cond_latents`, :1258).
-    Returns residuals shaped `(b t) c h w` with b = 2B, which is what `UNet3DConditionModel.forward` takes."""
+    Returns residuals shaped `(b t) c h w` with b = 2B, which is what `UNet3DConditionModel.forward` takes.
+
+    Several ControlNets (a `MultiControlNetModel` or a list of nets, the reference's multi-net branch): controlnet_latents
+    is a list with one such tensor per net, controlnet_conditioning_scale a float for every net (:1548-1553) or a list,
+    and controlnet_keep[i] a float or a list per net (`controlnet_keep_schedule`). Each net's slice of its own latents
+    is taken as for one net; the nets' maps are summed on the device. A net whose keep is 0 in a step is not run (the
+    reference runs it and scales its maps by 0, which only differs where a map is not finite); when every net is off the
+    function returns (None, None) and the UNet adds no residuals."""
+    from .controlnet import MultiControlNetModel
+    multi = isinstance(controlnet, (MultiControlNetModel, list, tuple))
+    if multi:
+        mc = controlnet if isinstance(controlnet, MultiControlNetModel) else MultiControlNetModel(controlnet)
+        nets = mc.nets
+        all_lat = mc.check_list("controlnet_latents", controlnet_latents)
+        scales = mc.check_list("controlnet_conditioning_scale", controlnet_conditioning_scale) \
+            if isinstance(controlnet_conditioning_scale, (list, tuple)) else [controlnet_conditioning_scale] * len(nets)
+    else:
+        nets, all_lat, scales = [controlnet], [controlnet_latents], [controlnet_conditioning_scale]
     vis = list(range(n_vision_cond))
 
     def fn(c, latent_model_input, t, i=0, rows=None):
         """rows: with `ParallelDenoiser(cfg_split=True)` the slice of the CFG batch this rank runs (`latent_model_input` then
         holds only those rows); the prompt and condition latents are sliced to match."""
         ctx = vis + [ci + n_vision_cond for ci in c]                                       # :1997-2000
-        idx = torch.tensor(ctx, dtype=torch.long, device=controlnet_latents.device)
-        lat_c = controlnet_latents.index_select(2, idx)                                    # :2008-2010
         b2 = latent_model_input.shape[0]
         if rows is not None:
             if guess_mode:
                 raise NotImplementedError("guess_mode runs the ControlNet on the conditional half only; not combined with cfg_split")
-            x, enc, lat_c = latent_model_input, prompt_embeds[rows], lat_c[rows]
+            x, enc = latent_model_input, prompt_embeds[rows]
         elif guess_mode:                                                                   # :1219-1225: cond half only
             x = latent_model_input[b2 // 2:]
             enc = prompt_embeds[prompt_embeds.shape[0] // 2:]
@@ -243,12 +295,35 @@ def make_controlnet_fn(controlnet, controlnet_latents: torch.Tensor, prompt_embe
             x, enc = latent_model_input, prompt_embeds
         nb, ch, tc, hh, ww = x.shape
         x2 = x.permute(0, 2, 1, 3, 4).reshape(nb * tc, ch, hh, ww)                           # b c t h w -> (b t) c h w
-        lat2 = lat_c.permute(0, 2, 1, 3, 4).reshape(nb * tc, lat_c.shape[1], hh, ww)
         enc2 = enc.repeat_interleave(tc, dim=0)                                            # align_repeat_tensor_single_dim
-        keep = 1.0 if controlnet_keep is None else float(controlnet_keep[i])
-        down, mid = controlnet(x2, t, enc2, controlnet_cond_latents=lat2,
-                               conditioning_scale=controlnet_conditioning_scale * keep, guess_mode=guess_mode,
-                               return_dict=False)
+
+        def net_latents(lat):
+            idx = torch.tensor(ctx, dtype=torch.long, device=lat.device)
+            lat_c = lat.index_select(2, idx)                                               # :2008-2010
+            if rows is not None:
+                lat_c = lat_c[rows]
+            return lat_c.permute(0, 2, 1, 3, 4).reshape(nb * tc, lat_c.shape[1], hh, ww)
+
+        if not multi:
+            keep = 1.0 if controlnet_keep is None else float(controlnet_keep[i])
+            down, mid = controlnet(x2, t, enc2, controlnet_cond_latents=net_latents(controlnet_latents),
+                                   conditioning_scale=controlnet_conditioning_scale * keep, guess_mode=guess_mode,
+                                   return_dict=False)
+        else:
+            keep = [1.0] * len(nets) if controlnet_keep is None else controlnet_keep[i]
+            if not isinstance(keep, (list, tuple)):
+                keep = [float(keep)] * len(nets)
+            if len(keep) != len(nets):
+                raise ValueError(f"controlnet_keep[{i}] has {len(keep)} entries for {len(nets)} ControlNets")
+            res = None
+            for net, lat, scale, kp in zip(nets, all_lat, scales, keep):                    # :1229-1235, cond_scale per net
+                if float(kp) == 0.0:
+                    continue
+                res = net(x2, t, enc2, controlnet_cond_latents=net_latents(lat), conditioning_scale=scale * float(kp),
+                          guess_mode=guess_mode, return_dict=False, accumulate_into=res)
+            if res is None:
+                return None, None
+            down, mid = res
         if guess_mode:                                                                     # :1275-1286: zeros for uncond
             def pad(r):
                 r5 = r.view(nb, tc, *r.shape[1:])

@@ -9,7 +9,8 @@
   3  image2video 48 frames 512x512, musev_referencenet + ReferenceNet one-shot + IP-Adapter tokens; window 16 overlap 4
      -> 4 windows (0-15, 12-27, 24-39, 36-47: the last one has 12 frames)
   4  pose video2video 128 frames 512x512, musev_referencenet + IP-Adapter + ControlNet encoder EVERY window-step;
-     window 16 overlap 4 -> 11 windows (the last one has 8 frames)
+     window 16 overlap 4 -> 11 windows (the last one has 8 frames); `--controlnets N` runs N ControlNets per
+     window-step with their residuals summed on the device (Multi-ControlNet, e.g. `--controlnet_name dwpose,depth`)
   5  512 frames 512x768 (64x96 latents), musev, window 16 stride 8 -> 63 windows
 Synthetic weights / inputs (no checkpoints offline). The one-shot side paths (ReferenceNet, image projection, ControlNet
 condition embedding) run before the timed region, as in the metric definition (SURVEY.md 8d); the ControlNet encoder itself
@@ -42,8 +43,12 @@ def main():
     ap.add_argument("--repeat", type=int, default=1)
     ap.add_argument("--cfg-split", action="store_true")
     ap.add_argument("--frames", type=int, default=0, help="override the video length (smoke runs)")
+    ap.add_argument("--controlnets", type=int, default=1,
+                    help="config 4: number of ControlNets per window-step (2 = e.g. `--controlnet_name dwpose,depth`)")
     a = ap.parse_args()
     c = dict(CONFIGS[a.config])
+    if a.controlnets != 1 and not c["controlnet"]:
+        ap.error("--controlnets applies to the ControlNet configuration (4)")
     if a.frames:
         c["T"] = a.frames
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
@@ -94,10 +99,16 @@ def main():
     if c["controlnet"]:
         from musev_b200.controlnet import ControlNetModel
         ccfg = ControlNetConfig()
-        cnet = ControlNetModel(ccfg, device=dev, dtype=torch.float16)
-        cnet.load_state_dict(make_state_dict(ccfg, seed=3, dtype=torch.float16))
-        cn_lat = (torch.randn(2, ccfg.block_out_channels[0], 1 + T, h, w, generator=g) * 0.3).half().to(dev)
-        cnet_fn = make_controlnet_fn(cnet, cn_lat, prompt, 1)
+        nets, lats = [], []
+        for k in range(a.controlnets):
+            cnet = ControlNetModel(ccfg, device=dev, dtype=torch.float16)
+            cnet.load_state_dict(make_state_dict(ccfg, seed=3 + 10 * k, dtype=torch.float16))
+            nets.append(cnet)
+            lats.append((torch.randn(2, ccfg.block_out_channels[0], 1 + T, h, w, generator=g) * 0.3).half().to(dev))
+        if a.controlnets == 1:
+            cnet_fn = make_controlnet_fn(nets[0], lats[0], prompt, 1)
+        else:                                        # Multi-ControlNet: the nets' residuals summed on the device
+            cnet_fn = make_controlnet_fn(nets, lats, prompt, 1)
     den = ParallelDenoiser(unet, DDIMScheduler(**SD15_DDIM_CONFIG))
 
     def run(steps):
@@ -132,7 +143,8 @@ def main():
             "balance": (sum(loads) / groups) / max(loads) if loads else None,
             "ms_per_denoise": float(ms.item()), "frames_per_s": T / (float(ms.item()) * 1e-3),
             "one_shot_ms": one_shot_ms, "finite": bool(torch.isfinite(res.latents).all().item()),
-            "referencenet": c["refnet"], "controlnet_per_window_step": c["controlnet"]}), flush=True)
+            "referencenet": c["refnet"], "controlnet_per_window_step": c["controlnet"],
+            "controlnets": a.controlnets if c["controlnet"] else 0}), flush=True)
     if world > 1:
         dist.destroy_process_group()
 

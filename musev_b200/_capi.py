@@ -1,17 +1,21 @@
 """ctypes binding of include/musev_b200.h. There is no fallback: if the library is missing, loading raises.
 
 Also the host side every whole-model wrapper shares (`EngineModel`): one engine handle, its weights by reference names,
-the workspace and the launch."""
+the workspace and the launch, and the frame chunking of the per-frame models (`launch_frame_chunks`), on one GPU or
+shared out over the ranks of a process group."""
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 import os
 from types import SimpleNamespace
-from typing import Dict, Iterable, Optional, Sequence, Tuple
+from typing import Callable, Dict, Iterable, Optional, Sequence, Tuple
 
 import torch
+import torch.distributed as dist
 
 from .build import LIB_PATH
+from .context import assign_windows
 
 _lib = None
 
@@ -311,6 +315,55 @@ def make_config(in_channels: int, out_channels: int, block_out_channels: Sequenc
     return c
 
 
+def frame_chunks(n: int, step: int) -> list:
+    """The launches of one frame-chunked call: [(0, step), (step, 2 step), ...], the last one possibly short."""
+    return [(n0, min(n0 + step, n)) for n0 in range(0, n, step)]
+
+
+def _check_same_call(x: torch.Tensor, out: torch.Tensor, step: int, group) -> None:
+    """All-gathers (N, step, digest of the per-frame shapes and dtypes) over the group and raises ValueError on every rank
+    when any rank's call differs, so that no rank enters a row exchange the others would never join."""
+    desc = f"per-frame input {list(x.shape[1:])} {x.dtype} -> output {list(out.shape[1:])} {out.dtype}"
+    digest = int.from_bytes(hashlib.blake2b(desc.encode(), digest_size=8).digest(), "little", signed=True)
+    # NCCL exchanges device tensors only; the other backends take host tensors
+    dev = out.device if dist.get_backend(group) == dist.Backend.NCCL else torch.device("cpu")
+    mine = torch.tensor([x.shape[0], step, digest], dtype=torch.int64, device=dev)
+    keys = [torch.empty_like(mine) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(keys, mine, group=group)
+    keys = [tuple(k.tolist()) for k in keys]
+    if len(set(keys)) > 1:
+        per_rank = ", ".join(f"rank {r}: N={k[0]} frames_per_call={k[1]}" for r, k in enumerate(keys))
+        same = "equal" if len({k[2] for k in keys}) == 1 else "not equal"
+        raise ValueError(f"the ranks of the process group made different frame-sharded calls ({per_rank}; per-frame "
+                         f"shapes / dtypes {same}); this rank: {desc}. Every rank must make the same call")
+
+
+def launch_frame_chunks(x: torch.Tensor, out: torch.Tensor, step: int, launch: Callable[[int, int], None],
+                        process_group=None) -> torch.Tensor:
+    """Runs `launch(n0, n1)` over the `frame_chunks(N, step)` of a per-frame model call x [N, ...] -> out [N, ...];
+    `launch` writes out[n0:n1].
+
+    process_group None: every chunk, in order, on this device. With a `torch.distributed` group the same chunks are
+    handed to its ranks as contiguous, balanced ranges (a rank may get none); each rank launches its own chunks exactly
+    as a single GPU would, so every frame gets bit-identical arithmetic, and then each rank broadcasts its rows of `out`
+    into the others' `out` on the device. Every rank returns the full `out`. Every rank must make the same call: the
+    ranks first compare N, `step` and the per-frame shapes and dtypes, and all raise ValueError on a mismatch."""
+    chunks = frame_chunks(x.shape[0], step)
+    if process_group is None:
+        for n0, n1 in chunks:
+            launch(n0, n1)
+        return out
+    _check_same_call(x, out, step, process_group)
+    per_rank = assign_windows([1] * len(chunks), dist.get_world_size(process_group))
+    for i in per_rank[dist.get_rank(process_group)]:
+        launch(*chunks[i])
+    for r, mine in enumerate(per_rank):
+        if mine:     # every rank knows the partition, so all skip an idle rank's empty range alike
+            rows = out[chunks[mine[0]][0]:chunks[mine[-1]][1]]
+            dist.broadcast(rows, src=dist.get_global_rank(process_group, r), group=process_group)
+    return out
+
+
 class EngineModel:
     """One engine handle behind a reference model's call surface: creation, weights by reference state-dict names,
     `.eval()`, `.to()`, and the grow-only workspace every call runs in. A subclass names its C entry points and
@@ -404,12 +457,12 @@ class EngineModel:
             raise MvbError(f"{self._forward} ({rc}): {self._error()}")
 
     def _launch_frames(self, x: torch.Tensor, out: torch.Tensor, h: int, w: int, latent_scale: float,
-                       postprocess: int) -> torch.Tensor:
+                       postprocess: int, process_group=None) -> torch.Tensor:
         """Runs an `mvb_vae_decode_args` model on x [N, ...] -> out [N, ...] in chunks of `frames_per_call` frames (bounds
-        the activation workspace); h, w = the size the model's entry point documents."""
-        step = max(1, self.frames_per_call)
-        for n0 in range(0, x.shape[0], step):
-            xc, oc = x[n0:n0 + step], out[n0:n0 + step]
+        the activation workspace); h, w = the size the model's entry point documents. With a process group the chunks
+        are shared out over its ranks and every rank returns the full output (`launch_frame_chunks`)."""
+        def launch(n0: int, n1: int) -> None:
+            xc, oc = x[n0:n1], out[n0:n1]
             a = MvbVaeDecodeArgs()
             a.latents, a.latents_is_f32 = xc.data_ptr(), _is_f32(xc)
             a.N, a.h, a.w = xc.shape[0], h, w
@@ -417,6 +470,8 @@ class EngineModel:
             a.out, a.out_is_f32 = oc.data_ptr(), _is_f32(oc)
             a.postprocess = int(postprocess)
             self._launch(a)
+
+        launch_frame_chunks(x, out, max(1, self.frames_per_call), launch, process_group)
         self._keep = x   # the input must outlive the asynchronous launches
         return out
 

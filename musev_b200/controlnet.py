@@ -309,8 +309,14 @@ class PoseGuider(EngineModel):
         return SimpleNamespace(missing_keys=[], unexpected_keys=unexpected)
 
     @torch.no_grad()
-    def embed_frames(self, images: torch.Tensor, out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
-        """images [N, c, H, W] (fp16 / fp32, frames on the batch axis) -> [N, emb, H / 2^(nb-1), W / 2^(nb-1)]."""
+    def embed_frames(self, images: torch.Tensor, out_dtype: Optional[torch.dtype] = None,
+                     process_group=None) -> torch.Tensor:
+        """images [N, c, H, W] (fp16 / fp32, frames on the batch axis) -> [N, emb, H / 2^(nb-1), W / 2^(nb-1)].
+
+        process_group: a `torch.distributed` group (or `group.WORLD`) shares the frames out over its ranks, in the chunks
+        of `frames_per_call` frames one GPU would launch, and exchanges the rows on the device
+        (`_capi.launch_frame_chunks`). Every rank must make the same call, with the same images, and every rank
+        receives the full embedding, bit-identical to the single-GPU one. None (the default) embeds every frame here."""
         self._check_loaded()
         f = 2 ** (len(self.cfg.block_out_channels) - 1)
         if images.dim() != 4 or images.shape[1] != self.cfg.conditioning_channels:
@@ -324,16 +330,17 @@ class PoseGuider(EngineModel):
         x = x.contiguous()
         h, w = H // f, W // f
         out = torch.empty((N, self.cfg.conditioning_embedding_channels, h, w), dtype=out_dtype or self.dtype, device=self.device)
-        return self._launch_frames(x, out, h, w, 1.0, 0)
+        return self._launch_frames(x, out, h, w, 1.0, 0, process_group)
 
     @torch.no_grad()
-    def forward(self, conditioning: torch.Tensor) -> torch.Tensor:
-        """PoseGuider.forward (controlnet.py:361-371): conditioning [b, c, t, H, W] -> [b, emb, t, H/8, W/8] (four blocks)."""
+    def forward(self, conditioning: torch.Tensor, process_group=None) -> torch.Tensor:
+        """PoseGuider.forward (controlnet.py:361-371): conditioning [b, c, t, H, W] -> [b, emb, t, H/8, W/8] (four blocks).
+        process_group: as in `embed_frames`."""
         if conditioning.dim() != 5:
             raise ValueError(f"conditioning must be [b, c, t, H, W], got {tuple(conditioning.shape)}")
         b, c, t, H, W = conditioning.shape
         x = conditioning.permute(0, 2, 1, 3, 4).reshape(b * t, c, H, W)                    # InflatedConv3d, :308-316
-        e = self.embed_frames(x)
+        e = self.embed_frames(x, process_group=process_group)
         return e.view(b, t, *e.shape[1:]).permute(0, 2, 1, 3, 4).contiguous()
 
     __call__ = forward

@@ -12,6 +12,12 @@ inside the library (`mvb_vae_encode`, `Engine::run_vae_encode`); `DiagonalGaussi
 torch ops on the small moments tensor here. The pipeline reads `vae.config.scaling_factor * vae.encode(x).latent_dist.mean`
 at three call sites (musev/pipelines/pipeline_controlnet.py:348-368, 809-811, 978-981); `encode_video` computes exactly that
 for a whole video in the library. `AutoencoderKL` holds both halves and stands in for `pipeline.vae`.
+
+Multi-GPU: every frame is encoded and decoded on its own, so `process_group=<torch.distributed group>` (or
+`torch.distributed.group.WORLD`) shares a call's frames out over the group's ranks: the chunks of `frames_per_call` frames
+a single GPU would launch go to the ranks in contiguous ranges, and the ranks then exchange their rows on the device
+(`_capi.launch_frame_chunks`). Every rank must make the same call, with the same input, and every rank receives the full
+result, bit-identical to the single-GPU one. `process_group=None` (the default) never looks at `torch.distributed`.
 """
 from __future__ import annotations
 
@@ -97,7 +103,8 @@ class AutoencoderKLDecoder(_VaeHalf):
     def _param_shapes(self):
         return vae_decoder_param_shapes(self.cfg)
 
-    def _run(self, z: torch.Tensor, latent_scale: float, postprocess: bool, out_dtype: torch.dtype) -> torch.Tensor:
+    def _run(self, z: torch.Tensor, latent_scale: float, postprocess: bool, out_dtype: torch.dtype,
+             process_group=None) -> torch.Tensor:
         self._check_loaded()
         if z.dim() != 4 or z.shape[1] != self.cfg.latent_channels:
             raise ValueError(f"latents must be [N, {self.cfg.latent_channels}, h, w], got {tuple(z.shape)}")
@@ -108,24 +115,27 @@ class AutoencoderKLDecoder(_VaeHalf):
         N, _, h, w = z.shape
         up = 2 ** (len(self.cfg.block_out_channels) - 1)
         out = torch.empty((N, self.cfg.out_channels, h * up, w * up), dtype=out_dtype, device=self.device)
-        return self._launch_frames(z, out, h, w, latent_scale, postprocess)
+        return self._launch_frames(z, out, h, w, latent_scale, postprocess, process_group)
 
     @torch.no_grad()
-    def decode(self, z: torch.Tensor, return_dict: bool = True):
-        """AutoencoderKL.decode (autoencoder_kl.py:275-302): z [N, 4, h, w] -> image [N, 3, 8h, 8w] (no scaling, no clamp)."""
-        img = self._run(z, 1.0, False, self.dtype)
+    def decode(self, z: torch.Tensor, return_dict: bool = True, process_group=None):
+        """AutoencoderKL.decode (autoencoder_kl.py:275-302): z [N, 4, h, w] -> image [N, 3, 8h, 8w] (no scaling, no clamp).
+        process_group: a `torch.distributed` group (or `group.WORLD`) shares the frames out over its ranks; see the module
+        notes. None (the default) decodes every frame here."""
+        img = self._run(z, 1.0, False, self.dtype, process_group)
         if not return_dict:
             return (img,)
         return DecoderOutput(sample=img)
 
     @torch.no_grad()
-    def decode_latents(self, latents: torch.Tensor) -> torch.Tensor:
+    def decode_latents(self, latents: torch.Tensor, process_group=None) -> torch.Tensor:
         """MusevControlNetPipeline.decode_latents (pipeline_controlnet.py:233-238): latents [b, c, f, h, w] ->
         video [b, c, f, H, W] float32 in [0, 1]. The reference returns a CPU numpy array; this returns the device tensor
-        (call `.cpu().numpy()` where the reference's `np.concatenate` of segments needs it)."""
+        (call `.cpu().numpy()` where the reference's `np.concatenate` of segments needs it). process_group: as in `decode`;
+        every rank holds the whole video afterwards (a 512-frame 512x768 video is 2.4 GB of fp32 per rank)."""
         b, c, f, h, w = latents.shape
         z = latents.permute(0, 2, 1, 3, 4).reshape(b * f, c, h, w)
-        img = self._run(z, 1.0 / self.cfg.scaling_factor, True, torch.float32)
+        img = self._run(z, 1.0 / self.cfg.scaling_factor, True, torch.float32, process_group)
         return img.view(b, f, *img.shape[1:]).permute(0, 2, 1, 3, 4).contiguous()
 
 
@@ -145,7 +155,7 @@ class AutoencoderKLEncoder(_VaeHalf):
     def _param_shapes(self):
         return vae_encoder_param_shapes(self.cfg)
 
-    def _run(self, x: torch.Tensor, postprocess: int, out_dtype: torch.dtype) -> torch.Tensor:
+    def _run(self, x: torch.Tensor, postprocess: int, out_dtype: torch.dtype, process_group=None) -> torch.Tensor:
         self._check_loaded()
         f = 2 ** (len(self.cfg.block_out_channels) - 1)
         if x.dim() != 4 or x.shape[1] != self.cfg.in_channels:
@@ -162,26 +172,30 @@ class AutoencoderKLEncoder(_VaeHalf):
         x = x.contiguous()
         zc = self.cfg.latent_channels
         out = torch.empty((N, zc if postprocess else 2 * zc, h, w), dtype=out_dtype, device=self.device)
-        return self._launch_frames(x, out, h, w, self.cfg.scaling_factor, postprocess)
+        return self._launch_frames(x, out, h, w, self.cfg.scaling_factor, postprocess, process_group)
 
     @torch.no_grad()
-    def encode(self, x: torch.Tensor, return_dict: bool = True):
+    def encode(self, x: torch.Tensor, return_dict: bool = True, process_group=None):
         """AutoencoderKL.encode (autoencoder_kl.py:256-297): images [N, 3, H, W] in [-1, 1] ->
-        latent_dist = DiagonalGaussianDistribution(moments [N, 8, H/8, W/8])."""
+        latent_dist = DiagonalGaussianDistribution(moments [N, 8, H/8, W/8]). process_group: a `torch.distributed` group
+        (or `group.WORLD`) shares the frames out over its ranks; see the module notes. None (the default) encodes every
+        frame here."""
         out_dtype = x.dtype if x.dtype in (torch.float16, torch.float32) else torch.float32
-        posterior = DiagonalGaussianDistribution(self._run(x, 0, out_dtype))
+        posterior = DiagonalGaussianDistribution(self._run(x, 0, out_dtype, process_group))
         if not return_dict:
             return (posterior,)
         return AutoencoderKLOutput(latent_dist=posterior)
 
     @torch.no_grad()
-    def encode_video(self, video: torch.Tensor, out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+    def encode_video(self, video: torch.Tensor, out_dtype: Optional[torch.dtype] = None,
+                     process_group=None) -> torch.Tensor:
         """`scaling_factor * encode(frames).latent_dist.mean` of every frame of video [b, 3, f, H, W] -> latents
         [b, 4, f, H/8, W/8] (the mirror of `decode_latents`): the `condition_latents` / video2video init latents of
-        pipeline_controlnet.py:348-368,978-981. Scale and the mean are applied in the library (fp32)."""
+        pipeline_controlnet.py:348-368,978-981. Scale and the mean are applied in the library (fp32). process_group: as
+        in `encode`."""
         b, c, f, H, W = video.shape
         x = video.permute(0, 2, 1, 3, 4).reshape(b * f, c, H, W)
-        lat = self._run(x, 1, out_dtype or self.dtype)
+        lat = self._run(x, 1, out_dtype or self.dtype, process_group)
         return lat.view(b, f, *lat.shape[1:]).permute(0, 2, 1, 3, 4).contiguous()
 
 
@@ -213,14 +227,15 @@ class AutoencoderKL:
     def eval(self):
         return self
 
-    def encode(self, x: torch.Tensor, return_dict: bool = True):
-        return self.encoder.encode(x, return_dict)
+    def encode(self, x: torch.Tensor, return_dict: bool = True, process_group=None):
+        return self.encoder.encode(x, return_dict, process_group=process_group)
 
-    def decode(self, z: torch.Tensor, return_dict: bool = True):
-        return self.decoder.decode(z, return_dict)
+    def decode(self, z: torch.Tensor, return_dict: bool = True, process_group=None):
+        return self.decoder.decode(z, return_dict, process_group=process_group)
 
-    def decode_latents(self, latents: torch.Tensor) -> torch.Tensor:
-        return self.decoder.decode_latents(latents)
+    def decode_latents(self, latents: torch.Tensor, process_group=None) -> torch.Tensor:
+        return self.decoder.decode_latents(latents, process_group=process_group)
 
-    def encode_video(self, video: torch.Tensor, out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
-        return self.encoder.encode_video(video, out_dtype)
+    def encode_video(self, video: torch.Tensor, out_dtype: Optional[torch.dtype] = None,
+                     process_group=None) -> torch.Tensor:
+        return self.encoder.encode_video(video, out_dtype, process_group=process_group)

@@ -248,6 +248,13 @@ typedef struct mvb_unet_args {
   const void* mid_refer_emb; int mid_refer_t, mid_refer_h, mid_refer_w;
   int refer_is_f32;                            /* refer maps are [B, C, t, h, w] */
   int n_down_residuals;                        /* ControlNet: 0 or 1 + num_blocks*(layers_per_block+1) - 1 tensors */
+  int cfg_shared_sample;                       /* since mvb_version 7: 1 = the caller guarantees that batches [0, B/2) and
+                                                  [B/2, B) of `sample` are equal (the CFG batch of a denoise step); nothing
+                                                  is promised about any other input. The layers before the first one that
+                                                  reads a per-batch input then run on the first half only. B must be even.
+                                                  It fills the alignment gap in front of down_residuals, so no field moved
+                                                  and the struct kept its size: a zero-initialised struct of an older
+                                                  caller reads as 0. */
   const void* down_residuals[MVB_MAX_REFER];   /* [(B T), C, h, w] */
   const void* mid_residual; int residual_is_f32;
   int skip_temporal_layers;

@@ -83,7 +83,7 @@ class MvbUnetArgs(C.Structure):
         ("refer_w", C.c_int * MAX_REFER),
         ("mid_refer_emb", C.c_void_p), ("mid_refer_t", C.c_int), ("mid_refer_h", C.c_int), ("mid_refer_w", C.c_int),
         ("refer_is_f32", C.c_int),
-        ("n_down_residuals", C.c_int), ("down_residuals", C.c_void_p * MAX_REFER),
+        ("n_down_residuals", C.c_int), ("cfg_shared_sample", C.c_int), ("down_residuals", C.c_void_p * MAX_REFER),
         ("mid_residual", C.c_void_p), ("residual_is_f32", C.c_int),
         ("skip_temporal_layers", C.c_int),
         ("out", C.c_void_p), ("out_is_f32", C.c_int),

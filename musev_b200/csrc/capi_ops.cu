@@ -35,8 +35,8 @@ extern "C" {
 const char* mvb_last_error(void) { return g_err; }
 
 // 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle; 4: the CLIP text handle, causal attention;
-// 5: mvb_fuse_cfg_multistep; 6: mvb_controlnet_args.accumulate
-int mvb_version(void) { return 6; }
+// 5: mvb_fuse_cfg_multistep; 6: mvb_controlnet_args.accumulate; 7: mvb_unet_args.cfg_shared_sample
+int mvb_version(void) { return 7; }
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   if (!d || !d->a0 || !d->weight || !d->out) return fail("mvb_op_conv_gemm: null pointer", cudaSuccess);
@@ -115,7 +115,7 @@ int mvb_op_groupnorm(const void* x0, int c0, const void* x1, int c1, int NF, int
                      float eps, const float* gamma, const float* beta, int silu, void* y, float* scratch, void* stream) {
   int chunks = 0;
   cudaError_t e = gn_stats((cudaStream_t)stream, (const __half*)x0, c0, (const __half*)x1, c1, NF, HW, groups, scratch,
-                           &chunks);
+                           &chunks, NF);
   if (e == cudaSuccess)
     e = gn_apply((cudaStream_t)stream, (const __half*)x0, c0, (const __half*)x1, c1, NF, HW, groups, scratch, chunks,
                  frames_per_stat, eps, gamma, beta, silu, (__half*)y);
@@ -131,7 +131,7 @@ int mvb_op_groupnorm_fused(const void* x0, int c0, const void* x1, int c1, int N
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaError_t e = gn_fused((cudaStream_t)stream, (const __half*)x0, c0, (const __half*)x1, c1, NF, HW, groups, scratch,
-                           frames_per_stat, eps, gamma, beta, silu, (__half*)y, sms, barrier_word, arrivals);
+                           frames_per_stat, eps, gamma, beta, silu, (__half*)y, sms, barrier_word, arrivals, NF);
   if (e != cudaSuccess) return fail("mvb_op_groupnorm_fused", e == cudaErrorInvalidValue ? cudaSuccess : e);
   return MVB_OK;
 }

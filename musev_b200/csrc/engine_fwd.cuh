@@ -42,6 +42,13 @@ struct Engine::Fwd {
   } cond;
   bool skip_temporal;
   bool ok = true;
+  // The shared prefix of a CFG forward whose two batch halves start from the same sample (mvb_unet_args::cfg_shared_sample):
+  // between halve_batch() and unhalve_batch() the layers run on the first half only (B and NF are halved). The arena
+  // still hands out full-batch buffers, so the workspace is laid out as in a full-batch forward, and GroupNorm keeps the
+  // full batch's chunk count, so every output row comes out in the bits the full batch gives it. unhalve_batch() then
+  // copies the first half of each kept tensor (keep(); every tap keeps its tensor) over its second half.
+  bool halved = false;
+  std::vector<std::pair<__half*, long long>> halved_keep;   // (tensor, elements of its first half)
 
   // Clears the taps of a real call. A kind that runs GroupNorm (`groups` > 0) takes its scratch as the first allocation of
   // the arena.
@@ -63,17 +70,43 @@ struct Engine::Fwd {
     return false;
   }
   __half* alloc_h(long long rows, int C) {
-    void* p = ar->alloc((size_t)rows * C * sizeof(__half));
+    void* p = ar->alloc((size_t)rows * (halved ? 2 : 1) * C * sizeof(__half));
     if (!p) fail("workspace too small", cudaSuccess);
     return (__half*)p;
   }
   float* alloc_f(long long n) {
-    void* p = ar->alloc((size_t)n * sizeof(float));
+    void* p = ar->alloc((size_t)n * (halved ? 2 : 1) * sizeof(float));
     if (!p) fail("workspace too small", cudaSuccess);
     return (float*)p;
   }
+  // rows: of the full batch
   void tap(const std::string& name, const __half* p, long long rows, int C) {
     if (!dry) E->taps_.push_back({name, p, rows, C});
+    keep(p, rows / 2 * C);
+  }
+  void halve_batch() {
+    B /= 2; NF /= 2;
+    halved = true;
+  }
+  // n: elements of the first half (NF frames while halved)
+  void keep(const __half* p, long long n) {
+    if (!halved) return;
+    for (const auto& k : halved_keep)
+      if (k.first == p) return;
+    halved_keep.push_back({const_cast<__half*>(p), n});
+  }
+  void unhalve_batch() {
+    if (!halved) return;
+    halved = false;
+    B *= 2; NF *= 2;
+    if (!dry)
+      for (const auto& k : halved_keep) {
+        if (!ok) break;
+        cudaError_t e = cudaMemcpyAsync(k.first + k.second, k.first, (size_t)k.second * sizeof(__half),
+                                        cudaMemcpyDeviceToDevice, s);
+        if (e != cudaSuccess) fail("shared prefix: second half copy", e);
+      }
+    halved_keep.clear();
   }
   size_t mark() const { return ar->off; }
   void release(size_t m) { ar->off = m; }
@@ -116,14 +149,15 @@ struct Engine::Fwd {
           __half* y) {
     if (!gn_part) { fail("groupnorm: the forward reserved no scratch", cudaSuccess); return; }
     if (!ok || dry) return;
+    const int chunk_nf = halved ? 2 * NF : NF;
     if (E->gn_fused_) {
       cudaError_t e = gn_fused(s, x0, C0, x1, C1, NF, HW, groups, gn_part, fps, eps, n.g, n.b, silu, y,
-                               E->num_sms_, E->gn_counter_dev_, &E->gn_base_);
+                               E->num_sms_, E->gn_counter_dev_, &E->gn_base_, chunk_nf);
       if (e != cudaSuccess) fail("groupnorm (fused)", e);
       return;
     }
     int chunks = 0;
-    cudaError_t e = gn_stats(s, x0, C0, x1, C1, NF, HW, groups, gn_part, &chunks);
+    cudaError_t e = gn_stats(s, x0, C0, x1, C1, NF, HW, groups, gn_part, &chunks, chunk_nf);
     if (e == cudaSuccess)
       e = gn_apply(s, x0, C0, x1, C1, NF, HW, groups, gn_part, chunks, fps, eps, n.g, n.b, silu, y);
     if (e != cudaSuccess) fail("groupnorm", e);
@@ -279,7 +313,7 @@ struct Engine::Fwd {
   // musev Transformer2DModel (transformer_2d.py:257-389) + BasicTransformerBlock (attention.py:172-431)
   __half* spatial(const SpatialT& st, const __half* x, int HW) {
     const int C = st.C, Hh = heads, d = C / Hh, dp = pad16(d), hd = Hh * dp;
-    const long long M = (long long)NF * HW;
+    long long M = (long long)NF * HW;
     __half* out = alloc_h(M, C);
     const size_t mk = mark();
     __half* nbuf = alloc_h(M, C);
@@ -317,6 +351,12 @@ struct Engine::Fwd {
       ln(h, M, C, 1e-5f, b.n2, nbuf);
       __half* q = alloc_h(M, hd);
       { Epilogue ep; ep.out = q; ep.ldc = hd; gemm(nbuf, M, C, b.q2, ep, false); }
+      // the text (and IP-Adapter) tokens differ between the CFG halves: a shared prefix ends here
+      if (halved) {
+        keep(x, M * C); keep(h, M * C); keep(q, M * hd);
+        unhalve_batch();
+        M = (long long)NF * HW;
+      }
       const long long Mt = (long long)B * cond.n_text;
       __half* kv = alloc_h(Mt, 2 * hd);
       { Epilogue ep; ep.out = kv; ep.ldc = 2 * hd; gemm(cond.enc, Mt, b.kv2.K, b.kv2, ep, b.kv2.bias != nullptr); }
@@ -414,8 +454,10 @@ struct Engine::Fwd {
     release(mk);
     return out;
   }
-  // reference feature map [B, C, t, h, w] -> tokens [B*t*h*w, C]
+  // reference feature map [B, C, t, h, w] -> tokens [B*t*h*w, C]; the maps differ between the CFG halves, so a shared
+  // prefix must have ended before
   __half* refer_tokens(const void* map, int C, int t, int h, int w) {
+    if (halved) { fail("refer_tokens: inside the shared prefix", cudaSuccess); return nullptr; }
     __half* tok = alloc_h((long long)B * t * h * w, C);
     if (ok && !dry) {
       cudaError_t e = ncthw_to_tokens(s, map, cond.refer_is_f32, B, C, t, h * w, tok, C, 1.f);

@@ -127,6 +127,7 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
   if (T > 32) { err_ = "at most 32 frames per window (temporal attention kernel)"; return false; }
   if (B < 1 || B > 64 || a.n_vis_cond > 64) { err_ = "batch (incl. CFG) must be in 1..64 and at most 64 vision-condition frames"; return false; }
   if (a.n_vis_cond < 0 || a.vis_cond_first < 0 || a.vis_cond_first + a.n_vis_cond > T) { err_ = "bad vision condition index range"; return false; }
+  if (a.cfg_shared_sample && B % 2) { err_ = "cfg_shared_sample needs an even batch"; return false; }
   if (c.need_refer_emb && a.n_refer != 0) {
     int expect = 1;
     for (int i = 0; i < nb; ++i) expect += c.layers_per_block + (i == nb - 1 ? 0 : 1);
@@ -194,6 +195,11 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
   cd.enc = enc; cd.n_text = a.n_text; cd.clip = clip; cd.n_clip = a.n_clip; cd.ip_adapter_scale = a.ip_adapter_scale;
   if (c.need_t2i_ip_adapter) { cd.n_vis_cond = a.n_vis_cond; cd.vis_cond_first = a.vis_cond_first; } cd.refer_is_f32 = a.refer_is_f32;
 
+  // ---- the shared prefix: with equal sample halves (cfg_shared_sample), every layer up to the first one that reads a
+  // per-half input computes the same rows for both halves, so it runs on the first half and its outputs are copied over
+  // the second (Fwd::halve_batch). The prefix ends at the first reference map (refer_tokens) or at the text K/V of the
+  // first spatial transformer (spatial); a pose_guider_emb, added in conv_in's epilogue, leaves it empty.
+  if (a.cfg_shared_sample && !a.pose_guider_emb) f.halve_batch();
   // ---- conv_in (unet_3d_condition.py:1008-1009)
   int Hc = a.H, Wc = a.W;
   const long long M = (long long)NF * Hc * Wc;
@@ -204,6 +210,7 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
   if (w.has_tin) { x = f.temporal(w.tin, x, Hc * Wc); f.tap("transformer_in", x, M, c0); }
   const bool use_ref = c.need_refer_emb && a.n_refer > 0;
   if (use_ref) {
+    f.unhalve_batch();   // x is conv_in's / transformer_in's output, kept by its tap
     __half* tok = f.refer_tokens(a.refer_embs[0], c0, a.refer_t[0], a.refer_h[0], a.refer_w[0]);
     x = f.refer_fuse(w.first_ref, x, Hc * Wc, tok, a.refer_t[0] * a.refer_h[0] * a.refer_w[0]);
     f.tap("first_refer", x, M, c0);
@@ -212,6 +219,7 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
   struct Skip { __half* p; int C, H, W; };
   std::vector<Skip> skips;
   skips.push_back({x, c0, Hc, Wc});
+  f.keep(x, (long long)f.NF * Hc * Wc * c0);
   int ch = c0;
   for (int i = 0; i < nb; ++i) {
     const bool final = i == nb - 1;
@@ -241,6 +249,7 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
         f.tap(pn + ".refer_emb_attns." + std::to_string(j), x, Ml, ch);
       }
       skips.push_back({x, ch, Hc, Wc});
+      f.keep(x, (long long)f.NF * Hc * Wc * ch);
     }
     if (!final) {
       x = f.downsample(x, ch, Hc, Wc, blk.sampler, 1);
@@ -252,6 +261,7 @@ bool Engine::run_unet(const mvb_unet_args& a, Arena& ar, cudaStream_t s) {
       }
       f.tap("down_blocks." + std::to_string(i) + ".down", x, (long long)NF * Hc * Wc, ch);
       skips.push_back({x, ch, Hc, Wc});
+      f.keep(x, (long long)f.NF * Hc * Wc * ch);
     }
   }
   // ---- mid (unet_3d_blocks.py:364-433)

@@ -138,19 +138,25 @@ gn_stats_kernel(const __half* __restrict__ x0, int C0, const __half* __restrict_
   gn_stats_unit(x0, C0, x1, C1, HW, G, part, gridDim.y - 1 - blockIdx.y, blockIdx.x, gridDim.x, spair);
 }
 
-cudaError_t gn_stats(cudaStream_t s, const __half* x0, int C0, const __half* x1, int C1, int NF, int HW, int G,
-                     float* part, int* chunks_out) {
-  ProfScope prof(s, KC_GROUPNORM);
-  const int C = C0 + (x1 ? C1 : 0);
-  if (!x1) C1 = 0;
-  if ((C0 % 8) || (C1 % 8) || (C % G) || ((C / G) % 2)) return cudaErrorInvalidValue;
-  const int threads = 256;
-  // ~8 resident blocks per SM (the kernel is latency-bound below that), at least ~32 pixels per block
-  int chunks = (8 * 132) / NF;          // rounded down: one full wave
+// Pixel chunks per frame of the statistics pass for chunk_nf frames: ~8 resident blocks per SM (the kernel is
+// latency-bound below that), at least ~32 pixels per block
+static int gn_chunks(int chunk_nf, int HW) {
+  int chunks = (8 * 132) / chunk_nf;    // rounded down: one full wave
   const int maxc = HW / 32 > 0 ? HW / 32 : 1;
   if (chunks > maxc) chunks = maxc;
   if (chunks > kGnMaxChunks) chunks = kGnMaxChunks;
   if (chunks < 1) chunks = 1;
+  return chunks;
+}
+
+cudaError_t gn_stats(cudaStream_t s, const __half* x0, int C0, const __half* x1, int C1, int NF, int HW, int G,
+                     float* part, int* chunks_out, int chunk_nf) {
+  ProfScope prof(s, KC_GROUPNORM);
+  const int C = C0 + (x1 ? C1 : 0);
+  if (!x1) C1 = 0;
+  if ((C0 % 8) || (C1 % 8) || (C % G) || ((C / G) % 2) || chunk_nf < 1) return cudaErrorInvalidValue;
+  const int threads = 256;
+  const int chunks = gn_chunks(chunk_nf, HW);
   *chunks_out = chunks;
   const int cols = (C / 8) < threads ? (C / 8) : threads;
   const size_t smem = (size_t)(threads / cols) * (C / 2) * sizeof(float2);
@@ -401,17 +407,14 @@ cudaError_t gn_apply(cudaStream_t s, const __half* x0, int C0, const __half* x1,
 // owned by the caller, `*base` the number of arrivals it has seen so far (host bookkeeping; launches must be stream-ordered).
 cudaError_t gn_fused(cudaStream_t s, const __half* x0, int C0, const __half* x1, int C1, int NF, int HW, int G, float* part,
                      int fps, float eps, const float* gamma, const float* beta, int silu, __half* y, int num_sms,
-                     unsigned int* counter, unsigned int* base) {
+                     unsigned int* counter, unsigned int* base, int chunk_nf) {
   ProfScope prof(s, KC_GROUPNORM);
   if (!x1) C1 = 0;
   const int C = C0 + C1;
-  if ((C0 % 8) || (C1 % 8) || (C % G) || ((C / G) % 2) || fps < 1 || (NF % fps) || G > 64) return cudaErrorInvalidValue;
+  if ((C0 % 8) || (C1 % 8) || (C % G) || ((C / G) % 2) || fps < 1 || (NF % fps) || G > 64 || chunk_nf < 1)
+    return cudaErrorInvalidValue;
   // same work decomposition as gn_stats / gn_apply
-  int chunks = (8 * 132) / NF;
-  const int maxc = HW / 32 > 0 ? HW / 32 : 1;
-  if (chunks > maxc) chunks = maxc;
-  if (chunks > kGnMaxChunks) chunks = kGnMaxChunks;
-  if (chunks < 1) chunks = 1;
+  const int chunks = gn_chunks(chunk_nf, HW);
   const int vecs = C / 8;
   int threads = 256;
   if (vecs <= 256 && (256 % vecs) != 0) threads = (256 / vecs) * vecs;

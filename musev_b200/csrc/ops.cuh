@@ -12,8 +12,10 @@ static constexpr int kGnMaxChunks = 64;
 // GroupNorm statistics. x0 [NF, HW, C0] (+ optional x1 [NF, HW, C1] = channel concat). Writes per-frame partial
 // (sum, sumsq) per group: part[NF][chunks][G][2] fp32. Returns the number of chunks used through *chunks.
 // The scratch behind `part` must hold NF*(kGnMaxChunks+1)*G*2 floats (gn_apply keeps mean/rstd after the partials).
+// The chunk count, and with it the bits of the statistics, follows from `chunk_nf` frames (NF for a standalone call): a
+// forward that runs some layers on half its batch passes its full frame count, so those layers keep the full batch's bits.
 cudaError_t gn_stats(cudaStream_t s, const __half* x0, int C0, const __half* x1, int C1, int NF, int HW, int G,
-                     float* part, int* chunks);
+                     float* part, int* chunks, int chunk_nf);
 // y = [SiLU]((x - mean) * rstd * gamma + beta); statistics are reduced over `frames_per_stat` consecutive frames
 // (1 = per-frame GroupNorm of the 2-D layers, T = the reference's 5-D GroupNorm over (c/g, t, h, w)).
 cudaError_t gn_apply(cudaStream_t s, const __half* x0, int C0, const __half* x1, int C1, int NF, int HW, int G,
@@ -47,10 +49,10 @@ cudaError_t expand_rows(cudaStream_t s, const __half* src, int B, int T, int D, 
 cudaError_t silu_copy(cudaStream_t s, const __half* x, long long n, __half* y);
 // GroupNorm as ONE persistent launch (statistics -> grid barrier -> finalize -> grid barrier -> apply); same arithmetic and
 // scratch layout as gn_stats + gn_apply. `counter`: zero-initialised device word owned by the caller; `*base`: host count of
-// the arrivals it has seen (launches on one stream).
+// the arrivals it has seen (launches on one stream). `chunk_nf` as in gn_stats.
 cudaError_t gn_fused(cudaStream_t s, const __half* x0, int C0, const __half* x1, int C1, int NF, int HW, int G, float* part,
                      int fps, float eps, const float* gamma, const float* beta, int silu, __half* y, int num_sms,
-                     unsigned int* counter, unsigned int* base);
+                     unsigned int* counter, unsigned int* base, int chunk_nf);
 // VAE decoder helpers: post_quant 1x1 conv on the latent channels, in-place row softmax, output layout change with the
 // image post-processing affine + clamp
 cudaError_t latent_pointwise(cudaStream_t s, const void* x, int is_f32, int N, int C, int HW, const float* w, const float* b,

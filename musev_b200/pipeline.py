@@ -19,6 +19,7 @@ from . import ops
 from .context import assign_windows, prepare_global_context
 from .samplers import multistep_update
 from .scheduler import DDIMScheduler, _PRED, _variance_noise
+from .unet import UNet3DConditionModel
 
 
 @dataclass
@@ -36,6 +37,9 @@ class ParallelDenoiser:
         # device_ops: module providing accumulate_window / fuse_cfg_*; the CUDA library unless a test injects a double
         self.ops = device_ops if device_ops is not None else ops
         self.unet = unet
+        # The engine UNet runs the layers before the first per-half input once for both CFG halves when told that their
+        # samples are equal; any other callable (a reference model, a test double) is called as the reference calls it.
+        self._shares_cfg_prefix = isinstance(unet, UNet3DConditionModel)
         self.scheduler = scheduler
         self.pg = process_group
         self._dist = None
@@ -182,6 +186,8 @@ class ParallelDenoiser:
                         down_res, mid_res = controlnet_fn(c, model_in, t, i)        # :2022-2038
                     kw["down_block_additional_residuals"] = down_res
                     kw["mid_block_additional_residual"] = mid_res
+                if self._shares_cfg_prefix:
+                    kw["cfg_shared_sample"] = not cfg_split    # cond2 and [lat_c] * 2: both halves of model_in are equal
                 eps = self.unet(model_in, t, prompt_embeds[rows] if cfg_split else prompt_embeds, sample_index=sub_idx,
                                 vision_conditon_frames_sample_index=vis_idx, sample_frame_rate=motion_speed,
                                 do_classifier_free_guidance=True, return_dict=False, **kw)[0]   # :2045-2067

@@ -123,8 +123,14 @@ class UNet3DConditionModel(EngineModel):
         ip_adapter_face_scale: float = 1.0,
         do_classifier_free_guidance: bool = False,
         pose_guider_emb: torch.Tensor = None,
+        cfg_shared_sample: bool = False,
     ):
-        """Reference: UNet3DConditionModel.forward, musev/models/unet_3d_condition.py:773-1280."""
+        """Reference: UNet3DConditionModel.forward, musev/models/unet_3d_condition.py:773-1280.
+
+        `cfg_shared_sample` (not in the reference): the caller guarantees that the two halves of the batch of `sample` are
+        equal, as in a CFG batch built from one latent. The engine then runs the layers before the first one that reads a
+        per-half input (text tokens, reference maps, pose embedding) on the first half only. Nothing is checked: halves
+        that differ give a wrong result. The library refuses the flag for an odd batch."""
         self._check_loaded()
         for name, v in (("class_labels", class_labels), ("timestep_cond", timestep_cond), ("attention_mask", attention_mask),
                         ("frame_index", frame_index), ("refer_self_attn_emb", refer_self_attn_emb),
@@ -204,6 +210,7 @@ class UNet3DConditionModel(EngineModel):
             keep.append(pose)
             a.pose_guider_emb, a.pose_is_f32 = pose.data_ptr(), _is_f32(pose)
         a.skip_temporal_layers = int(self.skip_temporal_layers)
+        a.cfg_shared_sample = int(cfg_shared_sample)
         out = torch.empty((B, self.cfg.out_channels, T, H, W), dtype=sample.dtype, device=dev)
         a.out, a.out_is_f32 = out.data_ptr(), _is_f32(out)
         self._launch(a)

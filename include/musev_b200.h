@@ -134,6 +134,11 @@ int mvb_op_groupnorm_fused(const void* x0, int c0, const void* x1, int c1, int N
 int mvb_op_layernorm(const void* x, long long M, int C, float eps, const float* gamma, const float* beta, void* y,
                      void* stream);
 
+/* In-place row softmax of an fp16 score matrix [M, N] with row stride ld (since mvb_version 8): each row becomes
+ * softmax(scale * row) with fp32 statistics: the softmax of the VAE mid-block attention. N % 8 == 0, N <= 8192,
+ * ld % 8 == 0; columns N..ld of a row are not touched. */
+int mvb_op_softmax_rows(void* x, long long M, int N, long long ld, float scale, void* stream);
+
 /* Fused overlap mean + classifier-free guidance + DDIM step
  * (musev/pipelines/pipeline_controlnet.py:2079,2101-2117; musev/schedulers/scheduling_ddim.py:198-295).
  *   eps = eps_sum / counter[t];  cfg: eps = uncond + g * (text - uncond)   (eps_sum fp32 [2B,C,T,HW], uncond first)

@@ -175,6 +175,7 @@ def _declare(l: C.CDLL) -> None:
     l.mvb_op_layernorm.argtypes = [C.c_void_p, C.c_longlong, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p]
     l.mvb_op_layernorm.restype = C.c_int
+    fn("mvb_op_softmax_rows", C.c_int, C.c_void_p, C.c_longlong, C.c_int, C.c_longlong, C.c_float, C.c_void_p)
     l.mvb_fuse_cfg_ddim.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int, C.c_float, C.c_int,
                                     C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -35,8 +35,8 @@ extern "C" {
 const char* mvb_last_error(void) { return g_err; }
 
 // 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle; 4: the CLIP text handle, causal attention;
-// 5: mvb_fuse_cfg_multistep; 6: mvb_controlnet_args.accumulate; 7: mvb_unet_args.cfg_shared_sample
-int mvb_version(void) { return 7; }
+// 5: mvb_fuse_cfg_multistep; 6: mvb_controlnet_args.accumulate; 7: mvb_unet_args.cfg_shared_sample; 8: mvb_op_softmax_rows
+int mvb_version(void) { return 8; }
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   if (!d || !d->a0 || !d->weight || !d->out) return fail("mvb_op_conv_gemm: null pointer", cudaSuccess);
@@ -113,6 +113,8 @@ int mvb_op_temporal_attention(const void* qkv, int ld, int B, int T, int HW, int
 
 int mvb_op_groupnorm(const void* x0, int c0, const void* x1, int c1, int NF, int HW, int groups, int frames_per_stat,
                      float eps, const float* gamma, const float* beta, int silu, void* y, float* scratch, void* stream) {
+  // the frame grouping is checked before the statistics pass is launched: a refused call launches nothing
+  if (frames_per_stat < 1 || NF % frames_per_stat) return fail("mvb_op_groupnorm", cudaSuccess);
   int chunks = 0;
   cudaError_t e = gn_stats((cudaStream_t)stream, (const __half*)x0, c0, (const __half*)x1, c1, NF, HW, groups, scratch,
                            &chunks, NF);
@@ -140,6 +142,12 @@ int mvb_op_layernorm(const void* x, long long M, int C, float eps, const float* 
                      void* stream) {
   cudaError_t e = layernorm((cudaStream_t)stream, (const __half*)x, M, C, eps, gamma, beta, (__half*)y);
   if (e != cudaSuccess) return fail("mvb_op_layernorm", e == cudaErrorInvalidValue ? cudaSuccess : e);
+  return MVB_OK;
+}
+
+int mvb_op_softmax_rows(void* x, long long M, int N, long long ld, float scale, void* stream) {
+  cudaError_t e = softmax_rows((cudaStream_t)stream, (__half*)x, M, N, ld, scale);
+  if (e != cudaSuccess) return fail("mvb_op_softmax_rows", e == cudaErrorInvalidValue ? cudaSuccess : e);
   return MVB_OK;
 }
 

@@ -69,15 +69,16 @@ __device__ __forceinline__ void gn_stats_unit(const __half* __restrict__ x0, int
       const __half* src = (c < C0) ? x0 + (size_t)f * HW * C0 + c : x1 + (size_t)f * HW * C1 + (c - C0);
       const int ld = (c < C0) ? C0 : C1;
       float s[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0};
-      __half2 piv2[4];
+      float piv[4];
       int p = p_begin + r0;
       {                                // pilot: the first sample of every channel pair (independent of the loads below)
         const Half8 h0 = ld_half8(src + (size_t)(p < p_end ? p : p_begin) * ld);
 #pragma unroll
-        for (int j = 0; j < 4; ++j) piv2[j] = __low2half2(h0.h[j]);
+        for (int j = 0; j < 4; ++j) piv[j] = __low2float(h0.h[j]);
       }
-      // four independent 16-byte loads in flight per thread; the deviation from the pilot is taken in fp16 (one HSUB2 per
-      // pair: exact for neighbours of the pilot, 2^-11 relative otherwise), everything after it in fp32
+      // four independent 16-byte loads in flight per thread; the deviation from the pilot is taken in fp32 (exact for
+      // neighbours of the pilot, 2^-24 relative otherwise). An fp16 subtraction would overflow to inf once the two channels
+      // of a pair lie more than 65504 apart, which turns the whole group into inf / NaN.
       for (; p + 3 * rows_per_iter < p_end; p += 4 * rows_per_iter) {
         Half8 hv[4];
 #pragma unroll
@@ -86,23 +87,26 @@ __device__ __forceinline__ void gn_stats_unit(const __half* __restrict__ x0, int
         for (int u = 0; u < 4; ++u)
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const float2 t = __half22float2(__hsub2(hv[u].h[j], piv2[j]));
-            s[j] += t.x + t.y;
-            q[j] = fmaf(t.x, t.x, fmaf(t.y, t.y, q[j]));
+            const float tx = __low2float(hv[u].h[j]) - piv[j];
+            s[j] += tx;
+            q[j] = fmaf(tx, tx, q[j]);
+            const float ty = __high2float(hv[u].h[j]) - piv[j];
+            s[j] += ty;
+            q[j] = fmaf(ty, ty, q[j]);
           }
       }
       for (; p < p_end; p += rows_per_iter) {
         const Half8 hv = ld_half8(src + (size_t)p * ld);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const float2 t = __half22float2(__hsub2(hv.h[j], piv2[j]));
-          s[j] += t.x + t.y;
-          q[j] = fmaf(t.x, t.x, fmaf(t.y, t.y, q[j]));
+          const float tx = __low2float(hv.h[j]) - piv[j];
+          s[j] += tx;
+          q[j] = fmaf(tx, tx, q[j]);
+          const float ty = __high2float(hv.h[j]) - piv[j];
+          s[j] += ty;
+          q[j] = fmaf(ty, ty, q[j]);
         }
       }
-      float piv[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) piv[j] = __low2float(piv2[j]);
       // (mean, M2) of this thread's 2 x count samples of each pair
       const int span = p_end - p_begin - r0;
       const float cnt = span > 0 ? 2.f * (float)((span + rows_per_iter - 1) / rows_per_iter) : 0.f;
@@ -151,10 +155,10 @@ static int gn_chunks(int chunk_nf, int HW) {
 
 cudaError_t gn_stats(cudaStream_t s, const __half* x0, int C0, const __half* x1, int C1, int NF, int HW, int G,
                      float* part, int* chunks_out, int chunk_nf) {
-  ProfScope prof(s, KC_GROUPNORM);
   const int C = C0 + (x1 ? C1 : 0);
   if (!x1) C1 = 0;
-  if ((C0 % 8) || (C1 % 8) || (C % G) || ((C / G) % 2) || chunk_nf < 1) return cudaErrorInvalidValue;
+  if ((C0 % 8) || (C1 % 8) || (C % G) || ((C / G) % 2) || G > 64 || chunk_nf < 1) return cudaErrorInvalidValue;
+  ProfScope prof(s, KC_GROUPNORM);
   const int threads = 256;
   const int chunks = gn_chunks(chunk_nf, HW);
   *chunks_out = chunks;
@@ -378,10 +382,10 @@ gn_fused_kernel(const __half* __restrict__ x0, int C0, const __half* __restrict_
 cudaError_t gn_apply(cudaStream_t s, const __half* x0, int C0, const __half* x1, int C1, int NF, int HW, int G,
                      const float* part, int chunks, int fps, float eps, const float* gamma, const float* beta, int silu,
                      __half* y) {
-  ProfScope prof(s, KC_GROUPNORM, 2);
   if (!x1) C1 = 0;
   const int C = C0 + C1;
   if (fps < 1 || (NF % fps) || G > 64) return cudaErrorInvalidValue;
+  ProfScope prof(s, KC_GROUPNORM, 2);
   // mean / rstd live right behind the partial sums in the caller's scratch: NF*(kGnMaxChunks+1)*G*2 floats in total
   float* stats = const_cast<float*>(part) + (size_t)NF * kGnMaxChunks * G * 2;
   if (fps * chunks > 64) gn_finalize_wide_kernel<<<dim3(NF / fps, G), kGnFinalizeWarps * 32, 0, s>>>(part, chunks, fps, G, HW, C / G, eps, stats);
@@ -408,11 +412,11 @@ cudaError_t gn_apply(cudaStream_t s, const __half* x0, int C0, const __half* x1,
 cudaError_t gn_fused(cudaStream_t s, const __half* x0, int C0, const __half* x1, int C1, int NF, int HW, int G, float* part,
                      int fps, float eps, const float* gamma, const float* beta, int silu, __half* y, int num_sms,
                      unsigned int* counter, unsigned int* base, int chunk_nf) {
-  ProfScope prof(s, KC_GROUPNORM);
   if (!x1) C1 = 0;
   const int C = C0 + C1;
   if ((C0 % 8) || (C1 % 8) || (C % G) || ((C / G) % 2) || fps < 1 || (NF % fps) || G > 64 || chunk_nf < 1)
     return cudaErrorInvalidValue;
+  ProfScope prof(s, KC_GROUPNORM);
   // same work decomposition as gn_stats / gn_apply
   const int chunks = gn_chunks(chunk_nf, HW);
   const int vecs = C / 8;
@@ -584,8 +588,8 @@ layernorm40_kernel(const __half* __restrict__ x, long long M, float eps, const f
 
 cudaError_t layernorm(cudaStream_t s, const __half* x, long long M, int C, float eps, const float* gamma,
                       const float* beta, __half* y) {
+  if ((C % 8) || C > 2560) return cudaErrorInvalidValue;
   ProfScope prof(s, KC_LAYERNORM);
-  if (C % 8) return cudaErrorInvalidValue;
   if (C == 320 || C == 640 || C == 1280) {
     const int L = C / 40;
     const long long groups = (M + 32 / L - 1) / (32 / L);
@@ -601,8 +605,7 @@ cudaError_t layernorm(cudaStream_t s, const __half* x, long long M, int C, float
   if (vecs <= 32) layernorm_kernel<1, 4><<<blocks_for(4), 256, 0, s>>>(x, M, C, eps, gamma, beta, y);
   else if (vecs <= 64) layernorm_kernel<2, 4><<<blocks_for(4), 256, 0, s>>>(x, M, C, eps, gamma, beta, y);
   else if (vecs <= 160) layernorm_kernel<5, 2><<<blocks_for(2), 256, 0, s>>>(x, M, C, eps, gamma, beta, y);
-  else if (vecs <= 320) layernorm_kernel<10, 1><<<blocks_for(1), 256, 0, s>>>(x, M, C, eps, gamma, beta, y);
-  else return cudaErrorInvalidValue;
+  else layernorm_kernel<10, 1><<<blocks_for(1), 256, 0, s>>>(x, M, C, eps, gamma, beta, y);   // C <= 2560
   return cudaGetLastError();
 }
 
@@ -1004,8 +1007,8 @@ softmax_rows_kernel(__half* __restrict__ x, long long M, int N, long long ld, fl
   }
 }
 cudaError_t softmax_rows(cudaStream_t s, __half* x, long long M, int N, long long ld, float scale) {
-  ProfScope prof(s, KC_OTHER);
   if ((N % 8) || N > 8192 || (ld % 8)) return cudaErrorInvalidValue;
+  ProfScope prof(s, KC_OTHER);
   const unsigned blocks = (unsigned)((M + 7) / 8);
   softmax_rows_kernel<<<blocks, 256, 0, s>>>(x, M, N, ld, scale * 1.4426950408889634f);
   return cudaGetLastError();

@@ -165,6 +165,17 @@ def layernorm(x, gamma, beta, eps):
     return y
 
 
+def softmax_rows(x, scale=1.0, N=None):
+    """In place: the first N columns (default all) of every row of x [M, ld] fp16 become softmax(scale * row); the
+    columns past N are left as they are. Returns x."""
+    assert x.dtype == torch.float16 and x.dim() == 2 and x.stride(1) == 1
+    M, ld = x.shape[0], x.stride(0)
+    N = x.shape[1] if N is None else N
+    assert N <= x.shape[1]
+    _capi.check(_capi.lib().mvb_op_softmax_rows(x.data_ptr(), M, N, ld, scale, _stream()))
+    return x
+
+
 def fuse_cfg_ddim(eps_sum, counter, latents, guidance, alpha_t, alpha_prev, prediction_type=0, clip_range=0.0,
                   out=None, eps_out=None, cfg=True, use_clipped=False, std_dev=0.0, noise=None, x0_out=None):
     """eps_sum fp32 [2B,C,T,H,W] (cfg) or [B,C,T,H,W]; counter fp32 [T] or None; latents fp32/fp16 [B,C,T,H,W]."""

@@ -18,7 +18,8 @@ def _declared_functions():
 def test_header_declares_expected_surface():
     names = _declared_functions()
     for must in ("mvb_create", "mvb_load_weight", "mvb_finalize", "mvb_workspace_bytes", "mvb_unet_forward",
-                 "mvb_fuse_cfg_ddim", "mvb_destroy", "mvb_last_error", "mvb_op_conv_gemm", "mvb_op_attention", "mvb_debug_attention_trace", "mvb_tensor_map_cache_stats"):
+                 "mvb_fuse_cfg_ddim", "mvb_destroy", "mvb_last_error", "mvb_op_conv_gemm", "mvb_op_attention", "mvb_debug_attention_trace", "mvb_tensor_map_cache_stats",
+                 "mvb_op_groupnorm", "mvb_op_groupnorm_fused", "mvb_op_layernorm", "mvb_op_softmax_rows"):
         assert must in names
 
 

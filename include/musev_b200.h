@@ -208,6 +208,29 @@ int mvb_fuse_cfg_multistep(const mvb_multistep_args* args, void* stream);
 int mvb_accumulate_window(float* eps_sum, int B2, int C, int T, int HW, const void* eps_window, int is_f32, int Tw,
                           int src_t0, const int* frames_dev, int nframes, void* stream);
 
+/* Histogram matching of video frames to a template frame (since mvb_version 9): the `need_hist_match` post-processing
+ * of text2video (musev/pipelines/pipeline_controlnet_predictor.py:745-749 -> MMCM correct_color.py:91-100
+ * `hist_match_video_bcthw` -> skimage 0.22 `exposure.match_histograms` on uint8 images). For every batch item b,
+ * channel c and frame f:
+ *   q      = uint8(fl32(x * 255)), truncated; values outside [0, 1] saturate to [0, 255] and NaN maps to 0
+ *   out    = fl32(np.interp(cdf_video(q), cdf_template, template_values) / 255)
+ * with the cumulative histograms of the frame's and of target[b, c]'s quantised pixels, evaluated in IEEE double exactly
+ * as numpy does, so the result is bit-identical to the reference's float32 output.
+ *   video   fp32 [B, C, F, H, W]; element strides stride_b, stride_c, stride_f (>= 0) of the first three axes, each H x W
+ *           plane contiguous (a frame slice such as video[:, :, 1:] of a contiguous tensor qualifies);
+ *   target  fp32 [B, C, 1, Ht, Wt] with strides tstride_b, tstride_c; Ht x Wt may differ from H x W;
+ *   out     fp32 [B, C, F, H, W] with strides ostride_*: either video itself (the same pointer and strides: in place) or
+ *           memory that overlaps neither video nor another plane of out;
+ *   workspace  device memory of at least mvb_op_hist_match_workspace_bytes(B, C, F, H, W, Ht, Wt) bytes (histograms and
+ *           tables; nothing in it needs initialising).
+ * Three kernel launches for any B and F. HBM traffic: 4 bytes read per video and target pixel (histograms), 4 read and
+ * 4 written per video pixel (apply). Bad sizes, strides or overlaps are rejected before any launch (MVB_ERR_INVALID). */
+long long mvb_op_hist_match_workspace_bytes(int B, int C, int F, int H, int W, int Ht, int Wt);
+int mvb_op_hist_match(const float* video, int B, int C, int F, int H, int W, long long stride_b, long long stride_c,
+                      long long stride_f, const float* target, int Ht, int Wt, long long tstride_b, long long tstride_c,
+                      float* out, long long ostride_b, long long ostride_c, long long ostride_f, void* workspace,
+                      long long workspace_bytes, void* stream);
+
 
 /* ---------------------------------------------------------------------------------------------------------
  * Whole-model level: the denoiser `UNet3DConditionModel` (musev/models/unet_3d_condition.py:179-1280).

@@ -188,6 +188,9 @@ def _declare(l: C.CDLL) -> None:
     l.mvb_accumulate_window.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                         C.c_int, C.c_void_p, C.c_int, C.c_void_p]
     l.mvb_accumulate_window.restype = C.c_int
+    fn("mvb_op_hist_match_workspace_bytes", C.c_longlong, *[C.c_int] * 7)
+    fn("mvb_op_hist_match", C.c_int, C.c_void_p, *[C.c_int] * 5, *[C.c_longlong] * 3, C.c_void_p, C.c_int, C.c_int,
+       C.c_longlong, C.c_longlong, C.c_void_p, *[C.c_longlong] * 3, C.c_void_p, C.c_longlong, C.c_void_p)
     l.mvb_launch_count.argtypes = [C.c_int]
     l.mvb_launch_count.restype = C.c_longlong
     l.mvb_profile_enable.argtypes = [C.c_int]

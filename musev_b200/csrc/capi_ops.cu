@@ -35,8 +35,9 @@ extern "C" {
 const char* mvb_last_error(void) { return g_err; }
 
 // 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle; 4: the CLIP text handle, causal attention;
-// 5: mvb_fuse_cfg_multistep; 6: mvb_controlnet_args.accumulate; 7: mvb_unet_args.cfg_shared_sample; 8: mvb_op_softmax_rows
-int mvb_version(void) { return 8; }
+// 5: mvb_fuse_cfg_multistep; 6: mvb_controlnet_args.accumulate; 7: mvb_unet_args.cfg_shared_sample; 8: mvb_op_softmax_rows;
+// 9: mvb_op_hist_match
+int mvb_version(void) { return 9; }
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   if (!d || !d->a0 || !d->weight || !d->out) return fail("mvb_op_conv_gemm: null pointer", cudaSuccess);
@@ -205,6 +206,59 @@ int mvb_accumulate_window(float* eps_sum, int B2, int C, int T, int HW, const vo
   cudaError_t e = accumulate_window((cudaStream_t)stream, eps_sum, B2, C, T, HW, eps_window, is_f32, Tw, src_t0,
                                     frames_dev, nframes);
   if (e != cudaSuccess) return fail("mvb_accumulate_window", e);
+  return MVB_OK;
+}
+
+static bool hist_match_sizes_ok(int B, int C, int F, int H, int W, int Ht, int Wt) {
+  if (B < 1 || C < 1 || F < 1 || H < 1 || W < 1 || Ht < 1 || Wt < 1) return false;
+  const long long hw = (long long)H * W, hw_t = (long long)Ht * Wt;
+  // 32-bit bin counts per plane, and the count pass's grid in one dimension
+  return hw <= INT32_MAX && hw_t <= INT32_MAX && hist_match_max_blocks(B, C, F, hw, hw_t) <= INT32_MAX;
+}
+
+long long mvb_op_hist_match_workspace_bytes(int B, int C, int F, int H, int W, int Ht, int Wt) {
+  if (!hist_match_sizes_ok(B, C, F, H, W, Ht, Wt))
+    return fail("mvb_op_hist_match_workspace_bytes: sizes must be >= 1, H*W and Ht*Wt < 2^31", cudaSuccess);
+  return hist_match_workspace_bytes(B, C, F, (long long)H * W, (long long)Ht * Wt);
+}
+
+int mvb_op_hist_match(const float* video, int B, int C, int F, int H, int W, long long stride_b, long long stride_c,
+                      long long stride_f, const float* target, int Ht, int Wt, long long tstride_b, long long tstride_c,
+                      float* out, long long ostride_b, long long ostride_c, long long ostride_f, void* workspace,
+                      long long workspace_bytes, void* stream) {
+  if (!video || !target || !out || !workspace) return fail("mvb_op_hist_match: null pointer", cudaSuccess);
+  if (!hist_match_sizes_ok(B, C, F, H, W, Ht, Wt))
+    return fail("mvb_op_hist_match: sizes must be >= 1, H*W and Ht*Wt < 2^31", cudaSuccess);
+  if (stride_b < 0 || stride_c < 0 || stride_f < 0 || tstride_b < 0 || tstride_c < 0 || ostride_b < 0 || ostride_c < 0 ||
+      ostride_f < 0)
+    return fail("mvb_op_hist_match: negative stride", cudaSuccess);
+  const long long hw = (long long)H * W, hw_t = (long long)Ht * Wt;
+  // the planes of out must not overlap one another: sorted by stride, each axis steps past everything inside it
+  struct Axis { long long n, s; } ax[3] = {{B, ostride_b}, {C, ostride_c}, {F, ostride_f}};
+  for (int i = 0; i < 3; ++i)
+    for (int j = i + 1; j < 3; ++j)
+      if (ax[j].s < ax[i].s) { Axis t = ax[i]; ax[i] = ax[j]; ax[j] = t; }
+  long long inner = hw;
+  for (const Axis& a : ax) {
+    if (a.n == 1) continue;
+    if (a.s < inner) return fail("mvb_op_hist_match: planes of out overlap (strides too small)", cudaSuccess);
+    inner = a.s * a.n;
+  }
+  const bool in_place = out == video && ostride_b == stride_b && ostride_c == stride_c && ostride_f == stride_f;
+  if (!in_place) {
+    const uintptr_t v0 = (uintptr_t)video, o0 = (uintptr_t)out;
+    const uintptr_t v1 = v0 + 4 * (uintptr_t)((B - 1) * stride_b + (C - 1) * stride_c + (F - 1) * stride_f + hw);
+    const uintptr_t o1 = o0 + 4 * (uintptr_t)((B - 1) * ostride_b + (C - 1) * ostride_c + (F - 1) * ostride_f + hw);
+    if (v0 < o1 && o0 < v1)
+      return fail("mvb_op_hist_match: out overlaps video without being video itself (same pointer and strides)",
+                  cudaSuccess);
+  }
+  if (workspace_bytes < hist_match_workspace_bytes(B, C, F, hw, hw_t))
+    return fail("mvb_op_hist_match: workspace smaller than mvb_op_hist_match_workspace_bytes", cudaSuccess);
+  const HistMatchPlanes src{video, stride_b, stride_c, stride_f, F, hw};
+  const HistMatchPlanes tmpl{target, tstride_b, tstride_c, 0, 1, hw_t};
+  cudaError_t e = hist_match((cudaStream_t)stream, B, C, src, tmpl, out, ostride_b, ostride_c, ostride_f, workspace);
+  if (e != cudaSuccess) return fail("mvb_op_hist_match", e);
   return MVB_OK;
 }
 

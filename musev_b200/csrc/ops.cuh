@@ -92,4 +92,19 @@ cudaError_t fuse_cfg_multistep(cudaStream_t s, const float* eps_sum, const float
 cudaError_t accumulate_window(cudaStream_t s, float* eps_sum, int B2, int C, int T, int HW, const void* eps_win,
                               int is_f32, int Tw, int src_t0, const int* frames_dev, int nframes);
 
+// hist_match.cu: B x C x F planes of hw contiguous fp32 pixels, plane (b, c, f) at x + b sb + c sc + f sf (elements)
+struct HistMatchPlanes {
+  const float* x;
+  long long sb, sc, sf;
+  int F;
+  long long hw;
+};
+long long hist_match_workspace_bytes(int B, int C, int F, long long hw, long long hw_t);
+// CTAs of the largest of the three launches (the count pass)
+long long hist_match_max_blocks(int B, int C, int F, long long hw, long long hw_t);
+// every source plane histogram-matched to the template plane of its (b, c) (tmpl.F = 1), written to out (may be src.x
+// with src's strides); three launches. Arguments are validated by the caller (mvb_op_hist_match).
+cudaError_t hist_match(cudaStream_t s, int B, int C, const HistMatchPlanes& src, const HistMatchPlanes& tmpl, float* out,
+                       long long ob, long long oc, long long of, void* workspace);
+
 }  // namespace mvb

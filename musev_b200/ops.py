@@ -247,3 +247,36 @@ def accumulate_window(eps_sum, eps_win, src_t0, frames_dev):
     _capi.check(_capi.lib().mvb_accumulate_window(eps_sum.data_ptr(), B2, Cc, T, HW, eps_win.data_ptr(),
                                                   int(eps_win.dtype == torch.float32), eps_win.shape[2], src_t0,
                                                   frames_dev.data_ptr(), frames_dev.numel(), _stream()))
+
+
+def hist_match(video: torch.Tensor, target: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Histogram-matches every frame of video [B, C, F, H, W] to target [B, C, 1, Ht, Wt] per batch item and channel
+    (`mvb_op_hist_match`): the float32 values MMCM's `hist_match_video_bcthw(video, target, 255.0)` stores, bit for bit.
+    Both fp32 CUDA tensors with values in [0, 1]; any strides on the first three axes, each H x W plane contiguous, so
+    a frame slice such as `x[:, :, 1:]` is taken as it is. out: a new tensor (None), or a tensor of video's shape that is
+    video itself (in place) or overlaps neither video nor itself. Returns out."""
+    for name, t in (("video", video), ("target", target)):
+        if t.dtype != torch.float32 or not t.is_cuda or t.dim() != 5:
+            raise TypeError(f"hist_match: {name} must be a 5-D float32 CUDA tensor, got {t.dim()}-D {t.dtype} on {t.device}")
+        if t.stride(4) != 1 or (t.shape[3] > 1 and t.stride(3) != t.shape[4]):
+            raise ValueError(f"hist_match: every H x W plane of {name} must be contiguous, strides {t.stride()}")
+    B, Cc, F, H, W = video.shape
+    if target.device != video.device or tuple(target.shape[:3]) != (B, Cc, 1):
+        raise ValueError(f"hist_match: target must be [{B}, {Cc}, 1, H', W'] on {video.device}, got "
+                         f"{list(target.shape)} on {target.device}")
+    if out is None:
+        out = torch.empty_like(video, memory_format=torch.contiguous_format)
+    elif out.dtype != torch.float32 or out.device != video.device or out.shape != video.shape or out.stride(4) != 1 or \
+            (H > 1 and out.stride(3) != W):
+        raise ValueError(f"hist_match: out must be a float32 tensor of shape {list(video.shape)} on {video.device} with "
+                         "contiguous H x W planes")
+    Ht, Wt = target.shape[3:]
+    l = _capi.lib()
+    need = l.mvb_op_hist_match_workspace_bytes(B, Cc, F, H, W, Ht, Wt)
+    if need < 0:
+        _capi.check(int(need))
+    ws = torch.empty(int(need), dtype=torch.uint8, device=video.device)
+    _capi.check(l.mvb_op_hist_match(video.data_ptr(), B, Cc, F, H, W, *video.stride()[:3], target.data_ptr(), Ht, Wt,
+                                    *target.stride()[:2], out.data_ptr(), *out.stride()[:3], ws.data_ptr(), ws.numel(),
+                                    _stream()))
+    return out

@@ -39,8 +39,9 @@ int mvb_version(void);
  * are accumulated, out-of-image taps read zeros. K index of the packed weight [N, ntaps*(c0+c1)] is
  * tap-major, then source-0 channels, then source-1 channels (torch.cat order of a skip connection).
  *   out[m, n] = act((acc + bias[n] + rowadd[m / rows_per_group, n]) * alpha + beta * residual[m, n])
- * with m = (frame*H + h)*W + w. geglu=1: packed columns come in [16 value | 16 gate] chunks and
- * out[m, j] = value * gelu_erf(gate) has N/2 columns.
+ * with m = (frame*H + h)*W + w: the activation comes after the residual. geglu=1: packed columns come in
+ * [16 value | 16 gate] chunks and out[m, j] = (value + bias) * gelu_erf(gate + bias) has N/2 columns; geglu takes a
+ * bias only, and a row-add, residual, alpha != 1 or act != 0 with it is refused.
  */
 typedef struct mvb_conv_gemm_desc {
   const void* a0; int c0; long long a0_stride_w, a0_stride_h, a0_stride_n;
@@ -54,9 +55,10 @@ typedef struct mvb_conv_gemm_desc {
   const void* residual; long long ld_res;
   float alpha, beta;
   int geglu;
-  int act; /* 0 none, 1 SiLU, 2 GELU (erf), 3 quick-GELU x * sigmoid(1.702 x); 2 / 3 ignore geglu = 1 */
+  int act; /* 0 none, 1 SiLU, 2 GELU (erf), 3 quick-GELU x * sigmoid(1.702 x); other values are refused */
   int out_f32; /* store fp32 (no residual / geglu) */
-  int stride2; /* 3x3 stride-2 conv of a contiguous [NF,H,W,c0] input with even H, W (taps ignored); 0: off,
+  int stride2; /* 3x3 stride-2 conv of a contiguous [NF,H,W,c0] input with even H, W (taps ignored; a1 or a0 strides
+                  other than the contiguous ones are refused); 0: off,
                   1: pad 1 on every side (UNet Downsample2D), 2: pad (0, 1, 0, 1) = right / bottom only
                   (VAE encoder Downsample2D(padding=0), diffusers models/resnet.py:213-278) */
 } mvb_conv_gemm_desc;

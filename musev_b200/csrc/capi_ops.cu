@@ -49,6 +49,11 @@ int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
   ep.ld_res = d->ld_res; ep.alpha = d->alpha; ep.beta = d->beta; ep.geglu = d->geglu; ep.act = d->act; ep.out_f32 = d->out_f32;
   const char* err = nullptr;
   if (d->stride2) {
+    // the four parity views of launch_conv_s2 are built from the base pointer of a contiguous [NF, H, W, c0] input
+    if (d->a1 || d->a0_stride_w != d->c0 || d->a0_stride_h != (long long)d->W * d->c0 ||
+        d->a0_stride_n != (long long)d->H * d->W * d->c0)
+      return fail("mvb_op_conv_gemm: stride2 takes one contiguous [NF, H, W, c0] input (no a1, no strided view)",
+                  cudaSuccess);
     cudaError_t e2 = launch_conv_s2((cudaStream_t)stream, (const __half*)d->a0, d->c0, d->W, d->H, d->NF,
                                     (const __half*)d->weight, d->N, ep, sm_count(), &err, d->stride2);
     if (e2 != cudaSuccess) return fail(err, e2);

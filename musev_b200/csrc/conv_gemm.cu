@@ -915,7 +915,8 @@ static void pick_box(int W, int H, int NF, int* bw, int* bh, int* bn) {
 }
 
 // tile widths the kernel is instantiated for (the wgmma N of one warpgroup). 160 divides the UNet's 320 / 640 / 1280
-// channels exactly; the GEGLU epilogue needs whole 64-column [value | gate] chunks.
+// channels exactly; the GEGLU epilogue needs whole 64-column [value | gate] chunks, so GEGLU runs at 64, 128 and 256
+// only and has no 160-column instantiation.
 static const int kBlockNs[4] = {64, 128, 160, 256};
 
 // 256-column tiles finish on the accumulator fragments, which the plain / residual / GEGLU variants do (wide_ok); the
@@ -945,7 +946,9 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
 #define MVB_GEMM_ROW(BN) \
   {conv_gemm_kernel<kEpiGeneric, BN>, conv_gemm_kernel<kEpiPlain, BN>, conv_gemm_kernel<kEpiResidual, BN>, \
    conv_gemm_kernel<kEpiGeglu, BN>, conv_gemm_kernel<kEpiAct, BN>}
-  static const KernelFn kernels[4][5] = {MVB_GEMM_ROW(64), MVB_GEMM_ROW(128), MVB_GEMM_ROW(160),
+  static const KernelFn kernels[4][5] = {MVB_GEMM_ROW(64), MVB_GEMM_ROW(128),
+                                         {conv_gemm_kernel<kEpiGeneric, 160>, conv_gemm_kernel<kEpiPlain, 160>,
+                                          conv_gemm_kernel<kEpiResidual, 160>, nullptr, conv_gemm_kernel<kEpiAct, 160>},
                                          {nullptr, conv_gemm_kernel<kEpiPlain, 256>, conv_gemm_kernel<kEpiResidual, 256>,
                                           conv_gemm_kernel<kEpiGeglu, 256>, nullptr}};
 #undef MVB_GEMM_ROW
@@ -964,11 +967,17 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
       }
     attr_set = true;
   }
+  // GEGLU takes a bias only: neither of its epilogues reads a row-add, residual, alpha or activation
+  if (ep.geglu && (ep.rowadd || ep.res || ep.alpha != 1.f || ep.act != 0)) {
+    *err = "conv_gemm: geglu takes a bias only (no row-add, residual, alpha or activation)";
+    return cudaErrorInvalidValue;
+  }
+  if (ep.act < 0 || ep.act > 3) { *err = "conv_gemm: act must be 0 (none), 1 (SiLU), 2 (GELU) or 3 (quick-GELU)"; return cudaErrorInvalidValue; }
   const long long tiles_m = (long long)p.tiles_w * p.tiles_h * p.tiles_n;
   // epilogue variant: the fast ones need whole 32-column chunks and the common alpha / beta
   int epi = kEpiGeneric;
   if (!ep.out_f32 && ep.act == 0) {
-    if (ep.geglu) { if (p.N % 64 == 0 && !ep.rowadd) epi = kEpiGeglu; }
+    if (ep.geglu) { if (p.N % 64 == 0) epi = kEpiGeglu; }
     else if (p.N % 32 == 0) {
       if (ep.res && ep.beta == 1.f) epi = kEpiResidual;
       else if (!ep.res && ep.alpha == 1.f) epi = kEpiPlain;
@@ -1027,17 +1036,20 @@ static cudaError_t launch_common(cudaStream_t stream, const CUtensorMap* maps, i
   static const bool trace = getenv("MVB_TRACE") != nullptr;
   if (trace) {
     // the trailing fields describe the launch fully enough to replay it (tools/gpu_gemm_census.py): output image, the
-    // channels of each A source, tap offsets, the stride-2 pad mode (0: not a stride-2 conv) and the epilogue options
+    // channels of each A source, tap offsets, the stride-2 pad mode (0: not a stride-2 conv), the epilogue options and
+    // the output / residual row strides, with res_is_out = 1 for a residual read from the output it is written to
     char taps[9 * 10 + 1];                            // up to 9 x ",-128:-128" without the leading comma
     int len = 0;
     for (int i = 0; i < p.ntaps; ++i) len += snprintf(taps + len, sizeof(taps) - len, "%s%d:%d", i ? "," : "", p.dy[i], p.dx[i]);
     int s2 = 0;
     for (int i = 0; i < p.ntaps; ++i) if (p.tap_src[i]) s2 = p.dy[0] < 0 ? 1 : 2;
-    fprintf(stderr, "MVB_TRACE gemm M=%lld N=%d K=%lld taps=%d block_n=%d tiles=%lld geglu=%d res=%d f32=%d epi=%d "
-            "epi_io=%s W=%d H=%d NF=%d c0=%d c1=%d offsets=%s s2=%d bias=%d rowadd=%d rpg=%d alpha=%.9g beta=%.9g act=%d\n",
-            (long long)p.W * p.H * p.NF, p.N, ktot, p.ntaps, p.block_n, num_tiles, p.geglu, p.res != nullptr, p.out_f32,
-            epi, tma_epi ? "tma" : "lsu", p.W, p.H, p.NF, p.kb0 * 64, p.kb1 * 64, taps, s2, p.bias != nullptr, p.rowadd != nullptr,
-            p.rows_per_group, p.alpha, p.beta, p.act);
+    fprintf(stderr, "MVB_TRACE gemm M=%lld N=%d K=%lld taps=%d block_n=%d tiles=%lld nstages=%d geglu=%d res=%d f32=%d epi=%d "
+            "epi_io=%s W=%d H=%d NF=%d c0=%d c1=%d offsets=%s s2=%d bias=%d rowadd=%d rpg=%d alpha=%.9g beta=%.9g act=%d "
+            "ldc=%lld ld_res=%lld res_is_out=%d\n",
+            (long long)p.W * p.H * p.NF, p.N, ktot, p.ntaps, p.block_n, num_tiles, p.nstages, p.geglu, p.res != nullptr,
+            p.out_f32, epi, tma_epi ? "tma" : "lsu", p.W, p.H, p.NF, p.kb0 * 64, p.kb1 * 64, taps, s2, p.bias != nullptr,
+            p.rowadd != nullptr, p.rows_per_group, p.alpha, p.beta, p.act, p.ldc, p.res ? p.ld_res : 0LL,
+            p.res != nullptr && (const void*)p.res == (const void*)p.out);
   }
   AMaps am;
   for (int i = 0; i < 4; ++i) am.m[i] = maps[i < nmaps ? i : 0];

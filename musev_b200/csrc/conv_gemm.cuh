@@ -28,7 +28,8 @@ struct ConvGemmParams {
   int N;         // GEMM N (packed width; with GEGLU the written width is N/2)
   int block_n, tiles_nn;
   int nstages, stage_bytes;   // operand ring: nstages x (16 KB A tile + block_n x 128 B weight tile)
-  // epilogue: v = (acc + bias[n] + rowadd[group(m), n]) * alpha + beta * res[m, n]
+  // epilogue: out = act((acc + bias[n] + rowadd[m / rows_per_group, n]) * alpha + beta * res[m, n]), the activation
+  // after the residual; GEGLU takes the bias only (row-add, residual, alpha != 1 and act != 0 are refused)
   __half* out;
   long long ldc;
   const float* bias;
@@ -38,9 +39,9 @@ struct ConvGemmParams {
   const __half* res;
   long long ld_res;
   float alpha, beta;
-  int geglu;  // packed columns are [16 value | 16 gate] chunks: out = value * gelu_erf(gate)
-  int act;    // 0 none, 1 SiLU, 2 GELU (erf), 3 quick-GELU x sigmoid(1.702 x)
-  int out_f32;  // store fp32 instead of fp16 (embedding tables)
+  int geglu;  // packed columns are [16 value | 16 gate] chunks: out = (value + bias) * gelu_erf(gate + bias)
+  int act;    // 0 none, 1 SiLU, 2 GELU (erf), 3 quick-GELU x sigmoid(1.702 x); anything else is refused
+  int out_f32;  // store fp32 instead of fp16 (embedding tables); refused with a residual or GEGLU
 };
 
 struct ASource {

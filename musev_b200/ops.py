@@ -62,7 +62,10 @@ def conv_gemm(
     d.ntaps = len(taps)
     for i, (dy, dx) in enumerate(taps):
         d.dy[i], d.dx[i] = dy, dx
-    assert stride2 or weight.shape[1] == len(taps) * (C0 + (a1.shape[3] if a1 is not None else 0))
+    if stride2:
+        assert weight.shape[1] == 9 * C0
+    else:
+        assert weight.shape[1] == len(taps) * (C0 + (a1.shape[3] if a1 is not None else 0))
     d.weight, d.N = weight.data_ptr(), N
     d.out, d.ldc = out.data_ptr(), out.stride(0)
     if bias is not None:

@@ -40,7 +40,7 @@ PEAK_TFLOPS, PEAK_TBS = 989.0, 3.35
 TRACE_RE = re.compile(r"MVB_TRACE gemm (.*)$")
 # fields that describe a launch (block_n, tiles and epi are the library's choices, not the launch's)
 KEY_FIELDS = ("N", "K", "geglu", "res", "f32", "W", "H", "NF", "c0", "c1", "offsets", "s2", "bias", "rowadd", "rpg",
-              "alpha", "beta", "act")
+              "alpha", "beta", "act", "ldc", "ld_res", "res_is_out")
 
 
 def _parse(line):
@@ -48,48 +48,13 @@ def _parse(line):
     if not m:
         return None
     kv = dict(x.split("=", 1) for x in m.group(1).split())
-    if "offsets" not in kv:
+    if "res_is_out" not in kv:
         raise SystemExit("the library's MVB_TRACE gemm lines lack the replay fields: capture with this tree's library")
     return kv
 
 
-def capture(preset: str) -> None:
-    """Child process (MVB_TRACE set): one forward's distinct GEMM launches and its profiled GEMM time, as JSON on stdout."""
-    from musev_b200 import _capi
-    from musev_b200.schema import preset_config
-    from musev_b200.synth import make_inputs, make_state_dict
-    from musev_b200.unet import UNet3DConditionModel
-    dev = "cuda"
-    cfg = preset_config(preset)
-    m = UNet3DConditionModel(cfg, device=dev, dtype=torch.float16)
-    m.load_state_dict(make_state_dict(cfg, seed=0, dtype=torch.float16))
-    inp = make_inputs(cfg, batch=2, frames=16, h=64, w=64, n_vis_cond=1)
-    kw = dict(sample_index=inp["sample_index"], vision_conditon_frames_sample_index=inp["vision_conditon_frames_sample_index"],
-              sample_frame_rate=8)
-    for k in ("down_block_refer_embs", "mid_block_refer_emb", "vision_clip_emb"):
-        if k in inp:
-            kw[k] = [x.half().to(dev) for x in inp[k]] if isinstance(inp[k], list) else inp[k].half().to(dev)
-    x, enc = inp["sample"].half().to(dev), inp["encoder_hidden_states"].half().to(dev)
-    sys.stderr.flush()
-    saved = os.dup(2)
-    with tempfile.TemporaryFile(mode="w+") as log:
-        devnull = os.open(os.devnull, os.O_WRONLY)
-        os.dup2(devnull, 2)                          # warm-up forwards: trace lines discarded
-        for _ in range(2):
-            m(x, 601, enc, **kw)
-        torch.cuda.synchronize()
-        os.dup2(log.fileno(), 2)                     # the traced forward
-        m(x, 601, enc, **kw)
-        torch.cuda.synchronize()
-        os.dup2(devnull, 2)
-        _capi.profile_enable(True)                   # the profiled forward (same launches)
-        m(x, 601, enc, **kw)
-        prof = _capi.profile_collect()
-        _capi.profile_enable(False)
-        os.dup2(saved, 2)
-        os.close(devnull)
-        log.seek(0)
-        lines = log.read().splitlines()
+def distinct_entries(lines):
+    """The distinct launches among MVB_TRACE lines, in first-seen order, each with its count."""
     counts, order = {}, []
     for line in lines:
         kv = _parse(line)
@@ -100,7 +65,62 @@ def capture(preset: str) -> None:
             counts[key] = 0
             order.append(key)
         counts[key] += 1
-    entries = [dict(zip(KEY_FIELDS, k), count=counts[k]) for k in order]
+    return [dict(zip(KEY_FIELDS, k), count=counts[k]) for k in order]
+
+
+def capture_forward(preset: str, batch: int = 2, frames: int = 16, h: int = 64, w: int = 64, warmup: int = 2,
+                    profile: bool = True):
+    """In a process with MVB_TRACE set: the distinct GEMM launches of one UNet forward of `preset` on synthetic weights
+    (batch x (frames + 1 vision-condition frame), h x w latents), and with `profile` the profiled GEMM time of a second
+    forward (None otherwise)."""
+    from musev_b200 import _capi
+    from musev_b200.schema import preset_config
+    from musev_b200.synth import make_inputs, make_state_dict
+    from musev_b200.unet import UNet3DConditionModel
+    dev = "cuda"
+    cfg = preset_config(preset)
+    m = UNet3DConditionModel(cfg, device=dev, dtype=torch.float16)
+    m.load_state_dict(make_state_dict(cfg, seed=0, dtype=torch.float16))
+    inp = make_inputs(cfg, batch=batch, frames=frames, h=h, w=w, n_vis_cond=1)
+    kw = dict(sample_index=inp["sample_index"], vision_conditon_frames_sample_index=inp["vision_conditon_frames_sample_index"],
+              sample_frame_rate=8)
+    for k in ("down_block_refer_embs", "mid_block_refer_emb", "vision_clip_emb"):
+        if k in inp:
+            kw[k] = [x.half().to(dev) for x in inp[k]] if isinstance(inp[k], list) else inp[k].half().to(dev)
+    x, enc = inp["sample"].half().to(dev), inp["encoder_hidden_states"].half().to(dev)
+    prof = None
+    sys.stderr.flush()
+    saved = os.dup(2)
+    with tempfile.TemporaryFile(mode="w+") as log:
+        devnull = os.open(os.devnull, os.O_WRONLY)
+        try:
+            os.dup2(devnull, 2)                      # warm-up forwards: trace lines discarded
+            for _ in range(warmup):
+                m(x, 601, enc, **kw)
+            torch.cuda.synchronize()
+            os.dup2(log.fileno(), 2)                 # the traced forward
+            m(x, 601, enc, **kw)
+            torch.cuda.synchronize()
+            os.dup2(devnull, 2)
+            if profile:
+                _capi.profile_enable(True)           # the profiled forward (same launches)
+                m(x, 601, enc, **kw)
+                prof = _capi.profile_collect()
+                _capi.profile_enable(False)
+        finally:
+            os.dup2(saved, 2)
+            os.close(saved)
+            os.close(devnull)
+        log.seek(0)
+        lines = log.read().splitlines()
+    del m
+    torch.cuda.empty_cache()
+    return distinct_entries(lines), prof
+
+
+def capture(preset: str) -> None:
+    """Child process (MVB_TRACE set): one forward's distinct GEMM launches and its profiled GEMM time, as JSON on stdout."""
+    entries, prof = capture_forward(preset)
     print(json.dumps({"entries": entries, "profiled_gemm_ms": prof["gemm"]["ms"], "profiled_gemm_launches": prof["gemm"]["launches"]}))
 
 
@@ -131,11 +151,21 @@ def make_case(e, dev, g):
         kw["rows_per_group"] = rpg
     nout = N // 2 if geglu else N
     if int(e["res"]):
-        kw["residual"] = rnd(M, nout)
+        kw["residual"] = rnd(M, max(int(e["ld_res"]), nout))[:, :nout]   # the engine's row stride
     kw.update(alpha=float(e["alpha"]), beta=float(e["beta"]), geglu=bool(geglu), act=int(e["act"]), out_f32=bool(f32))
     flops = 2.0 * M * N * K
     nbytes = (NF * Hi * Wi * c0 + M * c1) * 2 + N * K * 2 + M * nout * (4 if f32 else 2) + (M * nout * 2 if int(e["res"]) else 0)
     return kw, flops, nbytes, (M, nout)
+
+
+def make_out(e, kw, dev):
+    """The output of one entry's replay as the engine passed it: the residual itself (res_is_out), or a [M, ldc] buffer
+    whose leading columns are the output."""
+    if int(e["res_is_out"]):
+        return kw["residual"]
+    M, nout = int(e["W"]) * int(e["H"]) * int(e["NF"]), int(e["N"]) // (2 if int(e["geglu"]) else 1)
+    buf = torch.zeros(M, max(int(e["ldc"]), nout), dtype=torch.float32 if int(e["f32"]) else torch.float16, device=dev)
+    return buf[:, :nout]
 
 
 def _bits_equal(a, b):

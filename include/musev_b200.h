@@ -147,7 +147,12 @@ int mvb_op_softmax_rows(void* x, long long M, int N, long long ld, float scale, 
  *   x0 from eps / v / sample prediction (prediction_type 0 / 1 / 2), optional clip to +-clip_range (<= 0: off),
  *   x_prev = sqrt(a_prev) x0 + sqrt(1 - a_prev - std^2) eps (+ std * variance_noise when eta > 0).
  * cfg = 0: eps_sum is a single [B,C,T,HW] prediction -- this is plain `DDIMScheduler.step`. counter, variance_noise,
- * eps_out, x0_out may be NULL. latents fp32 (is_f32) or fp16 [B,C,T,HW]. */
+ * eps_out, x0_out may be NULL. latents fp32 (is_f32) or fp16 [B,C,T,HW]. eps_out receives the guided model output
+ * (eps above, before any v / sample conversion); x0_out the x0 after the clip. use_clipped_model_output re-derives the
+ * eps of the update from the clipped x0.
+ * Extents (this entry point, mvb_fuse_cfg_affine, mvb_fuse_cfg_multistep and mvb_accumulate_window): a call with a zero
+ * extent returns MVB_OK, launches nothing and touches no buffer; a negative extent is MVB_ERR_INVALID before any launch
+ * ("negative extent" in mvb_last_error()). */
 int mvb_fuse_cfg_ddim(const float* eps_sum, const float* counter, const void* latents_in, void* latents_out,
                       int is_f32, int B, int C, int T, int HW, int cfg, float guidance_scale, float alpha_prod_t,
                       float alpha_prod_t_prev, int prediction_type, float clip_range, int use_clipped_model_output,
@@ -161,7 +166,7 @@ int mvb_fuse_cfg_ddim(const float* eps_sum, const float* counter, const void* la
  *   LCMScheduler.step            musev/schedulers/scheduling_lcm.py:196-312: prev = sqrt(a_prev) denoised + sqrt(1-a_prev) z,
  *                                aux = denoised = c_out x0 + c_skip x;
  *   DDIMScheduler.step           eps prediction without clipping, any eta.
- * Same tensor conventions as mvb_fuse_cfg_ddim; noise, aux_out, eps_out may be NULL. */
+ * Same tensor conventions and extent rules as mvb_fuse_cfg_ddim; noise, aux_out, eps_out may be NULL. */
 int mvb_fuse_cfg_affine(const float* eps_sum, const float* counter, const void* latents_in, void* latents_out, int is_f32,
                         int B, int C, int T, int HW, int cfg, float guidance_scale, float c_x, float c_e, float c_n,
                         const float* noise, float a_x, float a_e, float* aux_out, float* eps_out, void* stream);
@@ -184,8 +189,8 @@ int mvb_fuse_cfg_affine(const float* eps_sum, const float* counter, const void* 
  * Aliasing: m0_out MAY BE m2 (the same pointer): every element reads m2 before it writes m0, so two history buffers rotate
  * without a third. No other pair of the buffers may overlap -- in particular latents_out overlaps none of eps_sum, counter,
  * latents_in, m1, m2, noise, m0_out, and m0_out overlaps none of them but m2 (exactly). Overlaps are rejected before a
- * launch (MVB_ERR_INVALID, "overlap" in mvb_last_error()). HBM-bound: (4 or 8 with cfg) + 2 * (2 or 4) + 4 per non-NULL
- * m1 / m2 / noise / m0_out bytes per element. */
+ * launch (MVB_ERR_INVALID, "overlap" in mvb_last_error()). Extents as mvb_fuse_cfg_ddim. HBM-bound: (4 or 8 with cfg)
+ * + 2 * (2 or 4) + 4 per non-NULL m1 / m2 / noise / m0_out bytes per element. */
 typedef struct mvb_multistep_args mvb_multistep_args;
 struct mvb_multistep_args {
   const float* eps_sum;     /* fp32 [2B, C, T, HW] (cfg, uncond half first) or [B, C, T, HW] */
@@ -205,8 +210,10 @@ struct mvb_multistep_args {
 };
 int mvb_fuse_cfg_multistep(const mvb_multistep_args* args, void* stream);
 
-/* eps_sum[:, :, frames[i]] += eps_window[:, :, src_t0 + i] (musev/pipelines/pipeline_controlnet.py:2068-2078).
- * eps_window [2B, C, Tw, HW] fp32/fp16; frames_dev: device int32[nframes]. */
+/* eps_sum[:, :, frames[i]] += eps_window[:, :, src_t0 + i] (musev/pipelines/pipeline_controlnet.py:2068-2078), one fp32
+ * add per element. eps_window [2B, C, Tw, HW] fp32/fp16; frames_dev: device int32[nframes], each in [0, T) (not checked:
+ * the list lives on the device). A zero extent (B2, C, T, HW or nframes) returns MVB_OK and launches nothing; a negative
+ * extent (Tw included), src_t0 < 0 or src_t0 + nframes > Tw is MVB_ERR_INVALID before any launch. */
 int mvb_accumulate_window(float* eps_sum, int B2, int C, int T, int HW, const void* eps_window, int is_f32, int Tw,
                           int src_t0, const int* frames_dev, int nframes, void* stream);
 

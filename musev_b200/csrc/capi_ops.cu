@@ -162,6 +162,7 @@ int mvb_fuse_cfg_ddim(const float* eps_sum, const float* counter, const void* la
                       float alpha_prod_t_prev, int prediction_type, float clip_range, int use_clipped_model_output,
                       float std_dev_t, const float* variance_noise, float* eps_out, float* x0_out, void* stream) {
   if (!eps_sum || !latents_in || !latents_out) return fail("mvb_fuse_cfg_ddim: null pointer", cudaSuccess);
+  if (B < 0 || C < 0 || T < 0 || HW < 0) return fail("mvb_fuse_cfg_ddim: negative extent", cudaSuccess);
   if (alpha_prod_t <= 0.f || alpha_prod_t > 1.f || prediction_type < 0 || prediction_type > 2)
     return fail("mvb_fuse_cfg_ddim: bad alpha / prediction_type", cudaSuccess);
   cudaError_t e = fuse_cfg_ddim((cudaStream_t)stream, eps_sum, counter, latents_in, latents_out, is_f32, B, C, T, HW, cfg,
@@ -175,6 +176,7 @@ int mvb_fuse_cfg_affine(const float* eps_sum, const float* counter, const void* 
                         int B, int C, int T, int HW, int cfg, float guidance_scale, float c_x, float c_e, float c_n,
                         const float* noise, float a_x, float a_e, float* aux_out, float* eps_out, void* stream) {
   if (!eps_sum || !latents_in || !latents_out) return fail("mvb_fuse_cfg_affine: null pointer", cudaSuccess);
+  if (B < 0 || C < 0 || T < 0 || HW < 0) return fail("mvb_fuse_cfg_affine: negative extent", cudaSuccess);
   cudaError_t e = fuse_cfg_affine((cudaStream_t)stream, eps_sum, counter, latents_in, latents_out, is_f32, B, C, T, HW, cfg,
                                   guidance_scale, c_x, c_e, c_n, noise, a_x, a_e, aux_out, eps_out);
   if (e != cudaSuccess) return fail("mvb_fuse_cfg_affine", e);
@@ -208,6 +210,11 @@ int mvb_fuse_cfg_multistep(const mvb_multistep_args* a, void* stream) {
 int mvb_accumulate_window(float* eps_sum, int B2, int C, int T, int HW, const void* eps_window, int is_f32, int Tw,
                           int src_t0, const int* frames_dev, int nframes, void* stream) {
   if (!eps_sum || !eps_window || !frames_dev) return fail("mvb_accumulate_window: null pointer", cudaSuccess);
+  if (B2 < 0 || C < 0 || T < 0 || HW < 0 || Tw < 0 || nframes < 0)
+    return fail("mvb_accumulate_window: negative extent", cudaSuccess);
+  // the window frames read are [src_t0, src_t0 + nframes) of Tw
+  if (src_t0 < 0 || (long long)src_t0 + nframes > Tw)
+    return fail("mvb_accumulate_window: src_t0 < 0 or src_t0 + nframes > Tw", cudaSuccess);
   cudaError_t e = accumulate_window((cudaStream_t)stream, eps_sum, B2, C, T, HW, eps_window, is_f32, Tw, src_t0,
                                     frames_dev, nframes);
   if (e != cudaSuccess) return fail("mvb_accumulate_window", e);

@@ -208,8 +208,13 @@ cudaError_t launch_t(cudaStream_t s, const void* x, int x_is_f32, int cin, int H
   constexpr size_t smem = smem_bytes<CIN, NT, S>();
   static_assert(smem <= 227 * 1024, "small_conv: shared memory");
   auto kern = small_conv_kernel<CIN, NT, S>;
-  static bool configured = false;
-  static int per_sm = 1;
+  // the opt-in is per device: key the "already set" state (and the occupancy it gives) by the current device ordinal
+  static bool configured_dev[64] = {};
+  static int per_sm_dev[64] = {};
+  int cur_dev = 0;
+  cudaGetDevice(&cur_dev);
+  bool& configured = configured_dev[cur_dev & 63];
+  int& per_sm = per_sm_dev[cur_dev & 63];
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(small_conv_kernel)"; return e; }

@@ -1275,8 +1275,9 @@ cudaError_t fuse_cfg_ddim(cudaStream_t s, const float* eps_sum, const float* cou
                           void* latents_out, int is_f32, int B, int C, int T, int HW, int cfg, float guidance,
                           float alpha_t, float alpha_prev, int prediction_type, float clip_range, int use_clipped,
                           float std_dev, const float* noise, float* eps_out, float* x0_out) {
-  ProfScope prof(s, KC_OTHER);
   const long long n = (long long)B * C * T * HW;
+  if (n <= 0) return cudaSuccess;   // before the ProfScope: an empty step launches nothing and counts no launch
+  ProfScope prof(s, KC_OTHER);
   const int blocks = (int)((n + 255) / 256 < 132 * 8 ? (n + 255) / 256 : 132 * 8);
   if (is_f32)
     fuse_cfg_ddim_kernel<float><<<blocks, 256, 0, s>>>(eps_sum, counter, (const float*)latents_in, (float*)latents_out,
@@ -1317,8 +1318,9 @@ __global__ void fuse_cfg_affine_kernel(const float* __restrict__ eps_sum, const 
 cudaError_t fuse_cfg_affine(cudaStream_t s, const float* eps_sum, const float* counter, const void* latents_in,
                             void* latents_out, int is_f32, int B, int C, int T, int HW, int cfg, float guidance, float c_x,
                             float c_e, float c_n, const float* noise, float a_x, float a_e, float* aux_out, float* eps_out) {
-  ProfScope prof(s, KC_OTHER);
   const long long n = (long long)B * C * T * HW;
+  if (n <= 0) return cudaSuccess;   // before the ProfScope: an empty step launches nothing and counts no launch
+  ProfScope prof(s, KC_OTHER);
   const int blocks = (int)((n + 255) / 256 < 132 * 8 ? (n + 255) / 256 : 132 * 8);
   if (is_f32)
     fuse_cfg_affine_kernel<float><<<blocks, 256, 0, s>>>(eps_sum, counter, (const float*)latents_in, (float*)latents_out, n, T,
@@ -1346,8 +1348,9 @@ __global__ void accumulate_window_kernel(float* __restrict__ eps_sum, int B2, in
 }
 cudaError_t accumulate_window(cudaStream_t s, float* eps_sum, int B2, int C, int T, int HW, const void* eps_win,
                               int is_f32, int Tw, int src_t0, const int* frames_dev, int nframes) {
-  ProfScope prof(s, KC_OTHER);
   const long long n = (long long)B2 * C * nframes * HW;
+  if (n <= 0 || T <= 0) return cudaSuccess;   // nothing to add, or no frame to add it to: no launch, no count
+  ProfScope prof(s, KC_OTHER);
   const int blocks = (int)((n + 255) / 256 < 132 * 8 ? (n + 255) / 256 : 132 * 8);
   if (is_f32)
     accumulate_window_kernel<float><<<blocks, 256, 0, s>>>(eps_sum, B2, C, T, HW, (const float*)eps_win, Tw, src_t0,

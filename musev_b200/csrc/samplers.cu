@@ -137,9 +137,9 @@ cudaError_t fuse_cfg_multistep(cudaStream_t s, const float* eps_sum, const float
                                void* latents_out, int is_f32, int B, int C, int T, int HW, int cfg, float guidance, float a_x,
                                float a_e, float clip, float c_x, float c0, float c1, float c2, float c_n, const float* m1,
                                const float* m2, const float* noise, float* m0_out) {
-  ProfScope prof(s, KC_OTHER);
   const long long n = (long long)B * C * T * HW;
-  if (n <= 0) return cudaSuccess;
+  if (n <= 0) return cudaSuccess;   // before the ProfScope: an empty step launches nothing and counts no launch
+  ProfScope prof(s, KC_OTHER);
   const MultistepCoef k{guidance, a_x, a_e, clip, c_x, c0, c1, c2, c_n};
   bool vec = (HW % 4) == 0 && aligned(eps_sum, 16) && aligned(latents_in, is_f32 ? 16 : 8) &&
              aligned(latents_out, is_f32 ? 16 : 8);

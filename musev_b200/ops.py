@@ -185,10 +185,11 @@ def fuse_cfg_ddim(eps_sum, counter, latents, guidance, alpha_t, alpha_prev, pred
     B, Cc, T = latents.shape[:3]
     HW = latents.shape[3] * latents.shape[4]
     assert eps_sum.dtype == torch.float32 and eps_sum.is_contiguous() and latents.is_contiguous()
+    assert eps_sum.numel() == latents.numel() * (2 if cfg else 1), "eps_sum must be [2B,...] with cfg, [B,...] without"
     assert latents.dtype in (torch.float16, torch.float32), f"latents must be fp16 or fp32, got {latents.dtype}"
     assert counter is None or (counter.dtype == torch.float32 and counter.is_contiguous() and counter.numel() == T)
     for t_ in (noise, eps_out, x0_out):
-        assert t_ is None or (t_.dtype == torch.float32 and t_.is_contiguous())
+        assert t_ is None or (t_.dtype == torch.float32 and t_.is_contiguous() and t_.numel() == latents.numel())
     if out is None:
         out = torch.empty_like(latents)
     _capi.check(_capi.lib().mvb_fuse_cfg_ddim(
@@ -204,6 +205,7 @@ def fuse_cfg_affine(eps_sum, counter, latents, guidance, c_x, c_e, c_n=0.0, nois
     B, Cc, T = latents.shape[:3]
     HW = latents.shape[3] * latents.shape[4]
     assert eps_sum.dtype == torch.float32 and eps_sum.is_contiguous() and latents.is_contiguous()
+    assert eps_sum.numel() == latents.numel() * (2 if cfg else 1), "eps_sum must be [2B,...] with cfg, [B,...] without"
     assert latents.dtype in (torch.float16, torch.float32), f"latents must be fp16 or fp32, got {latents.dtype}"
     assert counter is None or (counter.dtype == torch.float32 and counter.is_contiguous() and counter.numel() == T)
     for t_ in (noise, aux_out, eps_out):

@@ -240,6 +240,38 @@ int mvb_op_hist_match(const float* video, int B, int C, int F, int H, int W, lon
                       float* out, long long ostride_b, long long ostride_c, long long ostride_f, void* workspace,
                       long long workspace_bytes, void* stream);
 
+/* Stitch of a tiled VAE decode or encode: diffusers `AutoencoderKL.tiled_decode` / `tiled_encode`
+ * (models/autoencoder_kl.py:354-464) after the tiles have run, as ONE launch: blend_v, then blend_h, in place and in
+ * tile order as the reference does it, the [:row_limit, :row_limit] crops concatenated, then the post-processing and
+ * the conversion to the output dtype. Each blend is fl(fl(a * fl32(1 - t/e)) + fl(b * fl32(t/e))) in the tiles' dtype
+ * (t/e in double), so the result is bit-identical to the reference's torch ops in that dtype.
+ * The tile grid: tile row i belongs to row class r when it falls within the row_count of class r (classes in tile order);
+ * every tile of the class is row_size[r] pixels high (output pixels: image pixels for a decode, latent pixels for an
+ * encode). Columns likewise. tiles[r * MVB_VAE_TILE_CLASSES + c] holds the tiles of row class r and column class c as
+ * a contiguous [N, row_count[r], col_count[c], C, row_size[r], col_size[c]] tensor.
+ * Refused before any launch (MVB_ERR_INVALID, the condition in mvb_last_error()): a null pointer, sizes < 1, more than
+ * MVB_VAE_TILE_CLASSES classes per axis, a tile other than the last shorter than row_limit, crops that do not add up
+ * to H (W), and a grid where a tile's bottom (right) blend strip reaches into its own top (left) blend region,
+ * h[i-1] - min(h[i-1], h[i], extent) < min(h[i-2], h[i-1], extent): there the in-place blends have no closed form. */
+#define MVB_VAE_TILE_CLASSES 4
+typedef struct mvb_vae_tile_blend_args mvb_vae_tile_blend_args;
+struct mvb_vae_tile_blend_args {
+  const void* tiles[MVB_VAE_TILE_CLASSES * MVB_VAE_TILE_CLASSES];
+  int tiles_is_f32;     /* the blend dtype: 1 fp32 (decode), 0 fp16 (encode of fp16 images) */
+  int N, C;             /* frames; channels of every tile */
+  int n_row_classes, row_count[MVB_VAE_TILE_CLASSES], row_size[MVB_VAE_TILE_CLASSES];
+  int n_col_classes, col_count[MVB_VAE_TILE_CLASSES], col_size[MVB_VAE_TILE_CLASSES];
+  int extent;           /* blend_extent */
+  int row_limit;        /* the crop of every tile */
+  int H, W;             /* output frame size */
+  int mode;             /* 0: the blended tiles; 1: clamp(v / 2 + 0.5, 0, 1) in fp32 (decode_latents); 2: scale * v of the
+                           first C / 2 channels in fp32 (the scaled mean of encode_video) */
+  float scale;          /* mode 2 */
+  void* out;            /* [N, C or C / 2, H, W] */
+  int out_is_f32;
+};
+int mvb_op_vae_tile_blend(const mvb_vae_tile_blend_args* args, void* stream);
+
 
 /* ---------------------------------------------------------------------------------------------------------
  * Whole-model level: the denoiser `UNet3DConditionModel` (musev/models/unet_3d_condition.py:179-1280).

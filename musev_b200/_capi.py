@@ -120,6 +120,20 @@ class MvbVaeDecodeArgs(C.Structure):
                 ("latent_scale", C.c_float), ("out", C.c_void_p), ("out_is_f32", C.c_int), ("postprocess", C.c_int)]
 
 
+VAE_TILE_CLASSES = 4
+
+
+class MvbVaeTileBlendArgs(C.Structure):
+    _fields_ = [
+        ("tiles", C.c_void_p * (VAE_TILE_CLASSES * VAE_TILE_CLASSES)), ("tiles_is_f32", C.c_int), ("N", C.c_int),
+        ("C", C.c_int),
+        ("n_row_classes", C.c_int), ("row_count", C.c_int * VAE_TILE_CLASSES), ("row_size", C.c_int * VAE_TILE_CLASSES),
+        ("n_col_classes", C.c_int), ("col_count", C.c_int * VAE_TILE_CLASSES), ("col_size", C.c_int * VAE_TILE_CLASSES),
+        ("extent", C.c_int), ("row_limit", C.c_int), ("H", C.c_int), ("W", C.c_int), ("mode", C.c_int),
+        ("scale", C.c_float), ("out", C.c_void_p), ("out_is_f32", C.c_int),
+    ]
+
+
 class MvbMultistepArgs(C.Structure):
     _fields_ = [
         ("eps_sum", C.c_void_p), ("counter", C.c_void_p), ("latents_in", C.c_void_p), ("latents_out", C.c_void_p),
@@ -191,6 +205,7 @@ def _declare(l: C.CDLL) -> None:
     fn("mvb_op_hist_match_workspace_bytes", C.c_longlong, *[C.c_int] * 7)
     fn("mvb_op_hist_match", C.c_int, C.c_void_p, *[C.c_int] * 5, *[C.c_longlong] * 3, C.c_void_p, C.c_int, C.c_int,
        C.c_longlong, C.c_longlong, C.c_void_p, *[C.c_longlong] * 3, C.c_void_p, C.c_longlong, C.c_void_p)
+    fn("mvb_op_vae_tile_blend", C.c_int, C.POINTER(MvbVaeTileBlendArgs), C.c_void_p)
     l.mvb_launch_count.argtypes = [C.c_int]
     l.mvb_launch_count.restype = C.c_longlong
     l.mvb_profile_enable.argtypes = [C.c_int]

@@ -36,7 +36,7 @@ const char* mvb_last_error(void) { return g_err; }
 
 // 2: mvb_unet_args.pose_guider_emb, the PoseGuider handle; 3: the CLIP vision handle; 4: the CLIP text handle, causal attention;
 // 5: mvb_fuse_cfg_multistep; 6: mvb_controlnet_args.accumulate; 7: mvb_unet_args.cfg_shared_sample; 8: mvb_op_softmax_rows;
-// 9: mvb_op_hist_match
+// 9: mvb_op_hist_match. mvb_op_vae_tile_blend is an added export of version 9: probe for the symbol.
 int mvb_version(void) { return 9; }
 
 int mvb_op_conv_gemm(const mvb_conv_gemm_desc* d, void* stream) {
@@ -271,6 +271,27 @@ int mvb_op_hist_match(const float* video, int B, int C, int F, int H, int W, lon
   const HistMatchPlanes tmpl{target, tstride_b, tstride_c, 0, 1, hw_t};
   cudaError_t e = hist_match((cudaStream_t)stream, B, C, src, tmpl, out, ostride_b, ostride_c, ostride_f, workspace);
   if (e != cudaSuccess) return fail("mvb_op_hist_match", e);
+  return MVB_OK;
+}
+
+int mvb_op_vae_tile_blend(const mvb_vae_tile_blend_args* a, void* stream) {
+  if (!a) return fail("mvb_op_vae_tile_blend: null pointer", cudaSuccess);
+  VaeTileBlend p{};
+  for (int k = 0; k < kVaeTileClasses * kVaeTileClasses; ++k) p.tiles[k] = a->tiles[k];
+  p.tiles_is_f32 = a->tiles_is_f32; p.N = a->N; p.C = a->C;
+  p.n_row_classes = a->n_row_classes; p.n_col_classes = a->n_col_classes;
+  for (int k = 0; k < kVaeTileClasses; ++k) {
+    p.row_count[k] = a->row_count[k]; p.row_size[k] = a->row_size[k];
+    p.col_count[k] = a->col_count[k]; p.col_size[k] = a->col_size[k];
+  }
+  p.extent = a->extent; p.row_limit = a->row_limit; p.H = a->H; p.W = a->W; p.mode = a->mode; p.scale = a->scale;
+  p.out = a->out; p.out_is_f32 = a->out_is_f32;
+  if (const char* why = vae_tile_blend_check(p)) {
+    snprintf(g_err, sizeof(g_err), "mvb_op_vae_tile_blend: %s", why);
+    return MVB_ERR_INVALID;
+  }
+  cudaError_t e = vae_tile_blend((cudaStream_t)stream, p);
+  if (e != cudaSuccess) return fail("mvb_op_vae_tile_blend", e);
   return MVB_OK;
 }
 

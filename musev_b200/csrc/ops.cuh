@@ -64,6 +64,26 @@ cudaError_t tokens_to_ncthw_affine(cudaStream_t s, const __half* x, int ldx, int
 // moments [N, C2, HW] (postprocess 0) or scale * mean [N, C2/2, HW] (postprocess 1), fp16 or fp32
 cudaError_t vae_moments(cudaStream_t s, const float* x, int ldx, int N, int C2, int HW, const float* w, const float* b,
                         int postprocess, float scale, void* y, int is_f32);
+// vae_tiles.cu: the stitch of a tiled VAE decode / encode (mvb_op_vae_tile_blend). Tile row i of the grid belongs to
+// the row class whose counts it falls in (classes in tile order, equal tile heights row_size within a class); likewise
+// for columns. tiles[r * kVaeTileClasses + c] holds the tiles of row class r and column class c as
+// [N, row_count[r], col_count[c], C, row_size[r], col_size[c]] in the blend dtype (fp32 if tiles_is_f32, else fp16).
+// out [N, C (mode 0, 1) or C / 2 (mode 2), H, W]; mode 0 plain, 1 clamp(v / 2 + 0.5, 0, 1), 2 scale * v of the first
+// C / 2 channels.
+constexpr int kVaeTileClasses = 4;
+struct VaeTileBlend {
+  const void* tiles[kVaeTileClasses * kVaeTileClasses];
+  int tiles_is_f32, N, C;
+  int n_row_classes, row_count[kVaeTileClasses], row_size[kVaeTileClasses];
+  int n_col_classes, col_count[kVaeTileClasses], col_size[kVaeTileClasses];
+  int extent, row_limit, H, W, mode;
+  float scale;
+  void* out;
+  int out_is_f32;
+};
+// nullptr, or why the arguments cannot be blended exactly (checked on the host, before any launch)
+const char* vae_tile_blend_check(const VaeTileBlend& p);
+cudaError_t vae_tile_blend(cudaStream_t s, const VaeTileBlend& p);
 // temporal self-attention over the frame axis (musev/models/temporal_transformer.py:241-273 -> SDPA):
 // qkv [B, T, HW, 3*heads*dp] (q | k | v, head-padded), out [B, T, HW, heads*d].
 cudaError_t temporal_attention(cudaStream_t s, const __half* qkv, int ld, int B, int T, int HW, int heads, int d,

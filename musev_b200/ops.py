@@ -285,3 +285,43 @@ def hist_match(video: torch.Tensor, target: torch.Tensor, out: Optional[torch.Te
                                     *target.stride()[:2], out.data_ptr(), *out.stride()[:3], ws.data_ptr(), ws.numel(),
                                     _stream()))
     return out
+
+
+def vae_tile_blend(tiles, plan, out: torch.Tensor, mode: int = 0, scale: float = 1.0) -> torch.Tensor:
+    """The stitch of a tiled VAE decode / encode (`mvb_op_vae_tile_blend`): tiles[r][c] holds the tiles of row class r
+    and column class c of `plan` (a `musev_b200.vae_tiling.TilePlan`) as contiguous [N * count_r * count_c, C, h_r, w_c]
+    tensors in the blend dtype (fp32 or fp16, frame-major, then tile row, then tile column); out [N, C (mode 0, 1) or
+    C / 2 (mode 2), out_h, out_w], contiguous fp32 / fp16. mode 0: the blended tiles; 1: clamp(v / 2 + 0.5, 0, 1);
+    2: scale * v of the first C / 2 channels. Bit-identical to diffusers' `blend_v` / `blend_h` in the tiles' dtype."""
+    rows, cols = plan.rows.classes, plan.cols.classes
+    t0 = tiles[0][0]
+    if len(tiles) != len(rows) or any(len(t) != len(cols) for t in tiles):
+        raise ValueError(f"vae_tile_blend: tiles must be a {len(rows)} x {len(cols)} grid of shape groups")
+    ch = t0.shape[1]
+    N = out.shape[0]
+    for r, row in zip(rows, tiles):
+        for c, t in zip(cols, row):
+            want = (N * r.count * c.count, ch, r.size_out, c.size_out)
+            if tuple(t.shape) != want or t.dtype != t0.dtype or not t.is_contiguous() or t.device != out.device:
+                raise ValueError(f"vae_tile_blend: a tile group must be a contiguous {t0.dtype} tensor {list(want)} on "
+                                 f"{out.device}, got {list(t.shape)} {t.dtype}")
+    cout = ch // 2 if mode == 2 else ch
+    if tuple(out.shape) != (N, cout, plan.out_h, plan.out_w) or not out.is_contiguous():
+        raise ValueError(f"vae_tile_blend: out must be a contiguous [{N}, {cout}, {plan.out_h}, {plan.out_w}] tensor, "
+                         f"got {list(out.shape)}")
+    a = _capi.MvbVaeTileBlendArgs()
+    K = _capi.VAE_TILE_CLASSES
+    for i, row in enumerate(tiles):
+        for j, t in enumerate(row):
+            a.tiles[i * K + j] = t.data_ptr()
+    a.tiles_is_f32, a.N, a.C = _capi._is_f32(t0), N, ch
+    a.n_row_classes, a.n_col_classes = len(rows), len(cols)
+    for k, r in enumerate(rows):
+        a.row_count[k], a.row_size[k] = r.count, r.size_out
+    for k, c in enumerate(cols):
+        a.col_count[k], a.col_size[k] = c.count, c.size_out
+    a.extent, a.row_limit, a.H, a.W = plan.blend_extent, plan.row_limit, plan.out_h, plan.out_w
+    a.mode, a.scale = int(mode), float(scale)
+    a.out, a.out_is_f32 = out.data_ptr(), _capi._is_f32(out)
+    _capi.check(_capi.lib().mvb_op_vae_tile_blend(C.byref(a), _stream()))
+    return out

@@ -359,6 +359,8 @@ class VAEConfig:
     layers_per_block: int = 2
     norm_num_groups: int = 32
     scaling_factor: float = 0.18215
+    # SD-1.5's vae/config.json (diffusers' class default is 32): the tile size of tiled mode, in image pixels
+    sample_size: int = 512
 
 
 def _vae_resnet(out, p, cin, c):

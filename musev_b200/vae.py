@@ -27,7 +27,8 @@ from typing import Dict, Optional, Union
 
 import torch
 
-from ._capi import EngineModel, make_config
+from . import ops, vae_tiling
+from ._capi import EngineModel, _is_f32, frame_chunks, launch_frame_chunks, make_config
 # Names callers imported from this module before the binding moved to _capi; they are the binding's own objects.
 from ._capi import MvbVaeDecodeArgs, lib as _lib  # noqa: F401
 from .schema import VAEConfig, vae_decoder_param_shapes, vae_encoder_param_shapes
@@ -77,15 +78,78 @@ class AutoencoderKLOutput:
 
 class _VaeHalf(EngineModel):
     """One engine handle of a VAE half, created from a `VAEConfig`; entries of the other half in a full VAE state dict are
-    ignored by load_state_dict."""
+    ignored by load_state_dict.
+
+    Tiled mode (diffusers autoencoder_kl.py:127-171): `enable_tiling()` makes encode / decode split frames larger than
+    `tile_sample_min_size` image pixels (`tile_latent_min_size` latent pixels) into overlapping tiles, run each tile on
+    its own and blend them (`musev_b200.vae_tiling`, `mvb_op_vae_tile_blend`). `enable_slicing()` only records the flag:
+    frames are always run in chunks of `frames_per_call`, with the same bits per frame as one at a time."""
 
     def __init__(self, config: VAEConfig, device, dtype, frames_per_call, in_channels, out_channels):
         self.cfg = config
         self.config = SimpleNamespace(**asdict(config))
         self.frames_per_call = int(frames_per_call)
+        self.factor = 2 ** (len(config.block_out_channels) - 1)
+        self.use_slicing = False
+        self.use_tiling = False
+        self.tile_sample_min_size = config.sample_size
+        self.tile_latent_min_size = int(config.sample_size / self.factor)
+        self.tile_overlap_factor = 0.25
         c = make_config(in_channels, out_channels, config.block_out_channels, config.layers_per_block, 1, 64,
                         config.norm_num_groups, 1e-6)
         super().__init__(c, device, dtype)
+
+    def enable_tiling(self, use_tiling: bool = True):
+        self.use_tiling = use_tiling
+
+    def disable_tiling(self):
+        self.enable_tiling(False)
+
+    def enable_slicing(self):
+        self.use_slicing = True
+
+    def disable_slicing(self):
+        self.use_slicing = False
+
+    def _launch_tiles(self, x: torch.Tensor, out: torch.Tensor, plan: vae_tiling.TilePlan, latent_scale: float,
+                      tile_dtype: torch.dtype, mode: int, scale: float, process_group=None) -> torch.Tensor:
+        """x [N, c, H, W] -> out [N, c', H', W'] by the tile plan, per chunk of `frames_per_call` frames (shared out over
+        the ranks of a process group as untiled calls are): each shape group's tiles are cut out of the chunk's frames
+        with strided views and one copy, run as the N of engine calls of at most `frames_per_call` tiles (in
+        `tile_dtype`, no post-processing), and one `mvb_op_vae_tile_blend` stitches the chunk into out."""
+        step = max(1, self.frames_per_call)
+        S = plan.overlap_size
+        cout = self._tile_channels()
+
+        def launch(n0: int, n1: int) -> None:
+            xc = x[n0:n1]
+            nf = n1 - n0
+            bufs = {}
+            for rc, cc in plan.groups:
+                v = xc[:, :, rc.first * S:, cc.first * S:].unfold(2, rc.size_in, S)[:, :, :rc.count]
+                v = v.unfold(3, cc.size_in, S)[:, :, :, :cc.count]                   # [nf, c, nr, nc, th, tw]
+                tiles_in = v.permute(0, 2, 3, 1, 4, 5).contiguous().view(nf * rc.count * cc.count, xc.shape[1],
+                                                                          rc.size_in, cc.size_in)
+                tiles_out = torch.empty((tiles_in.shape[0], cout, rc.size_out, cc.size_out), dtype=tile_dtype,
+                                        device=self.device)
+                h, w = self._engine_hw(rc, cc)
+                for k0, k1 in frame_chunks(tiles_in.shape[0], step):
+                    ti, to = tiles_in[k0:k1], tiles_out[k0:k1]
+                    a = MvbVaeDecodeArgs()
+                    a.latents, a.latents_is_f32 = ti.data_ptr(), _is_f32(ti)
+                    a.N, a.h, a.w = ti.shape[0], h, w
+                    a.latent_scale = float(latent_scale)
+                    a.out, a.out_is_f32 = to.data_ptr(), _is_f32(to)
+                    a.postprocess = 0
+                    self._launch(a)
+                bufs[(rc, cc)] = tiles_out
+            ops.vae_tile_blend([[bufs[(rc, cc)] for cc in plan.cols.classes] for rc in plan.rows.classes], plan,
+                               out[n0:n1], mode, scale)
+
+        # the tile buffers are freed to the caching allocator in stream order, so they need no keeping
+        launch_frame_chunks(x, out, step, launch, process_group)
+        self._keep = x   # the input must outlive the asynchronous launches
+        return out
 
 
 class AutoencoderKLDecoder(_VaeHalf):
@@ -102,6 +166,44 @@ class AutoencoderKLDecoder(_VaeHalf):
 
     def _param_shapes(self):
         return vae_decoder_param_shapes(self.cfg)
+
+    def _tile_channels(self) -> int:
+        return self.cfg.out_channels
+
+    def _engine_hw(self, rc, cc):
+        return rc.size_in, cc.size_in          # mvb_vae_decode takes the latent size
+
+    def _tiled(self, z: torch.Tensor) -> bool:
+        """autoencoder_kl.py:300: tiled when tiling is on and a latent side exceeds tile_latent_min_size."""
+        return self.use_tiling and (z.shape[-1] > self.tile_latent_min_size or z.shape[-2] > self.tile_latent_min_size)
+
+    def _run_tiled(self, z: torch.Tensor, latent_scale: float, postprocess: bool, out_dtype: torch.dtype,
+                   process_group=None) -> torch.Tensor:
+        """`tiled_decode` (autoencoder_kl.py:420-466): tiles decoded to fp32 (decode's fp32 up-cast, :329-335), blended in
+        fp32 and rounded once to out_dtype by the blend kernel, which also applies decode_latents' post-processing after
+        the blend."""
+        self._check_loaded()
+        if z.dim() != 4 or z.shape[1] != self.cfg.latent_channels:
+            raise ValueError(f"latents must be [N, {self.cfg.latent_channels}, h, w], got {tuple(z.shape)}")
+        N, _, h, w = z.shape
+        plan = vae_tiling.plan_decode(h, w, self.tile_sample_min_size, self.tile_latent_min_size,
+                                      self.tile_overlap_factor, self.factor)
+        z = z.to(self.device)
+        if z.dtype not in (torch.float16, torch.float32):
+            z = z.float()
+        z = z.contiguous()
+        out = torch.empty((N, self.cfg.out_channels, plan.out_h, plan.out_w), dtype=out_dtype, device=self.device)
+        return self._launch_tiles(z, out, plan, latent_scale, torch.float32, 1 if postprocess else 0, 1.0, process_group)
+
+    @torch.no_grad()
+    def tiled_decode(self, z: torch.Tensor, return_dict: bool = True, process_group=None):
+        """AutoencoderKL.tiled_decode (autoencoder_kl.py:420-466) whatever the frame size: z [N, 4, h, w] -> image
+        [N, 3, 8h, 8w] in the handle's dtype. Raises ValueError, before any launch, for tile attributes the engine cannot
+        run (`musev_b200.vae_tiling.plan_decode`)."""
+        img = self._run_tiled(z, 1.0, False, self.dtype, process_group)
+        if not return_dict:
+            return (img,)
+        return DecoderOutput(sample=img)
 
     def _run(self, z: torch.Tensor, latent_scale: float, postprocess: bool, out_dtype: torch.dtype,
              process_group=None) -> torch.Tensor:
@@ -122,6 +224,8 @@ class AutoencoderKLDecoder(_VaeHalf):
         """AutoencoderKL.decode (autoencoder_kl.py:275-302): z [N, 4, h, w] -> image [N, 3, 8h, 8w] (no scaling, no clamp).
         process_group: a `torch.distributed` group (or `group.WORLD`) shares the frames out over its ranks; see the module
         notes. None (the default) decodes every frame here."""
+        if self._tiled(z):
+            return self.tiled_decode(z, return_dict, process_group=process_group)
         img = self._run(z, 1.0, False, self.dtype, process_group)
         if not return_dict:
             return (img,)
@@ -135,7 +239,8 @@ class AutoencoderKLDecoder(_VaeHalf):
         every rank holds the whole video afterwards (a 512-frame 512x768 video is 2.4 GB of fp32 per rank)."""
         b, c, f, h, w = latents.shape
         z = latents.permute(0, 2, 1, 3, 4).reshape(b * f, c, h, w)
-        img = self._run(z, 1.0 / self.cfg.scaling_factor, True, torch.float32, process_group)
+        run = self._run_tiled if self._tiled(z) else self._run
+        img = run(z, 1.0 / self.cfg.scaling_factor, True, torch.float32, process_group)
         return img.view(b, f, *img.shape[1:]).permute(0, 2, 1, 3, 4).contiguous()
 
 
@@ -154,6 +259,46 @@ class AutoencoderKLEncoder(_VaeHalf):
 
     def _param_shapes(self):
         return vae_encoder_param_shapes(self.cfg)
+
+    def _tile_channels(self) -> int:
+        return 2 * self.cfg.latent_channels
+
+    def _engine_hw(self, rc, cc):
+        return rc.size_out, cc.size_out        # mvb_vae_encode takes the latent size
+
+    def _tiled(self, x: torch.Tensor) -> bool:
+        """autoencoder_kl.py:267: tiled when tiling is on and an image side exceeds tile_sample_min_size."""
+        return self.use_tiling and (x.shape[-1] > self.tile_sample_min_size or x.shape[-2] > self.tile_sample_min_size)
+
+    def _run_tiled(self, x: torch.Tensor, postprocess: int, out_dtype: torch.dtype, process_group=None) -> torch.Tensor:
+        """`tiled_encode` (autoencoder_kl.py:366-418): encode dispatches to it before its fp32 up-cast (:267-276), so the
+        tiles' moments are blended in the image's dtype (fp16 / fp32; other dtypes run as fp32). postprocess 1 then
+        takes `scaling_factor * mean` in fp32, as the untiled path does, and rounds once to out_dtype."""
+        self._check_loaded()
+        if x.dim() != 4 or x.shape[1] != self.cfg.in_channels:
+            raise ValueError(f"images must have {self.cfg.in_channels} channels ([N, {self.cfg.in_channels}, H, W]), got {tuple(x.shape)}")
+        N, _, H, W = x.shape
+        plan = vae_tiling.plan_encode(H, W, self.tile_sample_min_size, self.tile_latent_min_size,
+                                      self.tile_overlap_factor, self.factor)
+        x = x.to(self.device)
+        if x.dtype not in (torch.float16, torch.float32):
+            x = x.float()
+        x = x.contiguous()
+        zc = self.cfg.latent_channels
+        out = torch.empty((N, zc if postprocess else 2 * zc, plan.out_h, plan.out_w), dtype=out_dtype, device=self.device)
+        return self._launch_tiles(x, out, plan, self.cfg.scaling_factor, x.dtype, 2 if postprocess else 0,
+                                  self.cfg.scaling_factor, process_group)
+
+    @torch.no_grad()
+    def tiled_encode(self, x: torch.Tensor, return_dict: bool = True, process_group=None):
+        """AutoencoderKL.tiled_encode (autoencoder_kl.py:366-418) whatever the image size: images [N, 3, H, W] ->
+        latent_dist of the blended moments, in the images' dtype. Raises ValueError, before any launch, for geometries
+        the engine cannot run (`musev_b200.vae_tiling.plan_encode`)."""
+        out_dtype = x.dtype if x.dtype in (torch.float16, torch.float32) else torch.float32
+        posterior = DiagonalGaussianDistribution(self._run_tiled(x, 0, out_dtype, process_group))
+        if not return_dict:
+            return (posterior,)
+        return AutoencoderKLOutput(latent_dist=posterior)
 
     def _run(self, x: torch.Tensor, postprocess: int, out_dtype: torch.dtype, process_group=None) -> torch.Tensor:
         self._check_loaded()
@@ -180,6 +325,8 @@ class AutoencoderKLEncoder(_VaeHalf):
         latent_dist = DiagonalGaussianDistribution(moments [N, 8, H/8, W/8]). process_group: a `torch.distributed` group
         (or `group.WORLD`) shares the frames out over its ranks; see the module notes. None (the default) encodes every
         frame here."""
+        if self._tiled(x):
+            return self.tiled_encode(x, return_dict, process_group=process_group)
         out_dtype = x.dtype if x.dtype in (torch.float16, torch.float32) else torch.float32
         posterior = DiagonalGaussianDistribution(self._run(x, 0, out_dtype, process_group))
         if not return_dict:
@@ -195,14 +342,16 @@ class AutoencoderKLEncoder(_VaeHalf):
         in `encode`."""
         b, c, f, H, W = video.shape
         x = video.permute(0, 2, 1, 3, 4).reshape(b * f, c, H, W)
-        lat = self._run(x, 1, out_dtype or self.dtype, process_group)
+        run = self._run_tiled if self._tiled(x) else self._run
+        lat = run(x, 1, out_dtype or self.dtype, process_group)
         return lat.view(b, f, *lat.shape[1:]).permute(0, 2, 1, 3, 4).contiguous()
 
 
 class AutoencoderKL:
     """Drop-in for the pipeline's `vae` (diffusers `AutoencoderKL` as MuseV uses it): one encoder and one decoder handle
     loaded from one full `AutoencoderKL.state_dict()`. `encode`, `decode`, `decode_latents`, `encode_video`, `config`
-    (`scaling_factor`, `block_out_channels`, ...), `dtype`, `device`, `eval`."""
+    (`scaling_factor`, `block_out_channels`, `sample_size`, ...), `dtype`, `device`, `eval`; tiled mode (`enable_tiling`,
+    `tiled_encode`, `tiled_decode` and the `tile_*` attributes, shared by both halves) and `enable_slicing`."""
 
     def __init__(self, config: VAEConfig = VAEConfig(), device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float16,
                  frames_per_call: int = 4):
@@ -239,3 +388,38 @@ class AutoencoderKL:
     def encode_video(self, video: torch.Tensor, out_dtype: Optional[torch.dtype] = None,
                      process_group=None) -> torch.Tensor:
         return self.encoder.encode_video(video, out_dtype, process_group=process_group)
+
+    def tiled_encode(self, x: torch.Tensor, return_dict: bool = True, process_group=None):
+        return self.encoder.tiled_encode(x, return_dict, process_group=process_group)
+
+    def tiled_decode(self, z: torch.Tensor, return_dict: bool = True, process_group=None):
+        return self.decoder.tiled_decode(z, return_dict, process_group=process_group)
+
+    def enable_tiling(self, use_tiling: bool = True):
+        """diffusers autoencoder_kl.py:144-150; what `pipeline.enable_vae_tiling()` calls."""
+        self.use_tiling = use_tiling
+
+    def disable_tiling(self):
+        self.enable_tiling(False)
+
+    def enable_slicing(self):
+        """autoencoder_kl.py:159-164 (pipeline_controlnet_predictor.py:284 calls it); records the flag only."""
+        self.use_slicing = True
+
+    def disable_slicing(self):
+        self.use_slicing = False
+
+
+def _both_halves(name: str) -> property:
+    """A tiling attribute of `AutoencoderKL`: read from the decoder, written to both halves."""
+    def get(self):
+        return getattr(self.decoder, name)
+
+    def set(self, value):
+        setattr(self.encoder, name, value)
+        setattr(self.decoder, name, value)
+    return property(get, set)
+
+
+for _name in ("use_slicing", "use_tiling", "tile_sample_min_size", "tile_latent_min_size", "tile_overlap_factor"):
+    setattr(AutoencoderKL, _name, _both_halves(_name))
